@@ -26,10 +26,7 @@ if ROOT not in sys.path:
 SR, P = 44100, 512
 OTHER_WORKLOADS = ("sins_cfg1", "combsub", "superfast", "combsubfast", "sinegen", "srcmod", "mel", "maskmul")
 
-# N -> (gather mode, chunks, compute streams) chosen by `--gather auto` (measured on B200, see DESIGN.md section 5)
-# round 2, ms/step at N=8 with 0.84 ms of kernels (profiles/r2_scale_m8_*.json): peer stores 1.077 | per-chunk peer stores
-# 4 chunks x 2 streams 1.069 | copy-engine push 2.42-2.49 | NCCL gather 1.425 | no gather 0.848.  The 7 x 56.4 MB
-# arrive while the FIR kernel (0.375 ms) runs: 395 MB / (0.375 + 0.23 ms exposed) = 653 GB/s into rank 0.
+# N -> (gather mode, chunks, compute streams) chosen by `--gather auto` (multi-GPU runs; not measured on H100)
 AUTO_GATHER = {2: ("peer", 1, 1), 4: ("peer", 1, 1), 8: ("peer", 1, 1)}
 
 WORKLOADS = {
@@ -185,23 +182,30 @@ class ClockSampler:
         return {"sm_mhz": statistics.median(sm), "sm_max_mhz": max(smax), "reasons": sorted(reasons), "samples": len(sm)}
 
 
-def ncu_traffic(workload, kernel_label):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed
-    ncu --set full capture (profiles/r2_traffic.json); None when no capture is recorded for it."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "r2_traffic.json")) as f:
-            ent = json.load(f).get(workload, {})
-        return ent.get("dram_bytes_per_launch") if ent.get("bench_kernel") == kernel_label else None
-    except Exception:
-        return None
-
-
 def measured_peak_hbm():
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (measured copy bandwidth)"
     except Exception:
-        return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md; MEASURED_PEAKS.json absent)"
+        return 3350.0, "H100 SXM data sheet, 3.35 TB/s (MEASURED_PEAKS.json absent)"
+
+
+DUMP_BYTES = 60 * 1024 * 1024           # below 64 MB with the .npy headers
+
+
+def dump_outputs(arrays, out_dir, torch):
+    """Write each array as out_dir/<name>.npy in float32, at most DUMP_BYTES in all: an array over its share is
+    replaced by a fixed sample of its flattened elements (seeded, sorted indices), the same from run to run."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    share = DUMP_BYTES // (4 * len(arrays))                  # elements per array
+    for i, (name, t) in enumerate(sorted(arrays.items())):
+        flat = t.detach().reshape(-1).float()
+        if flat.numel() > share:
+            g = torch.Generator().manual_seed(20240 + i)
+            idx = torch.randperm(flat.numel(), generator=g)[:share].sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(out_dir, name + ".npy"), flat.cpu().numpy().astype(np.float32))
 
 
 # ------------------------------------------------------------------------------------------
@@ -264,9 +268,8 @@ def metric_name(w):
 
 
 def run_reference_arm(args, w):
-    """--impl reference: the reference's own CPU implementation of the path on this box's host
-    cores.  /root/reference (Python) cannot travel to the GPU box, so this times the oracle port,
-    which is bit-identical to it on CPU (tests/test_oracle_vs_reference.py)."""
+    """--impl reference: the reference's own CPU implementation of the path on this host's cores: the oracle
+    port, which is bit-identical to it on CPU (tests/test_oracle_vs_reference.py)."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
@@ -356,12 +359,21 @@ class Runner:
         return self.frontend.mask_apply_(audio, self.mask_d[lo:lo + audio.shape[0]], P)
 
     def step(self, f0=None):
+        """one pass; self.last keeps every array a caller of the path receives from it (for --dump-outputs)"""
         if self.w["kind"] in ("mel", "maskmul"):
-            return self._wave_op(self.audio_d)
+            out = self._wave_op(self.audio_d)
+            self.last = {"out": out}
+            return out
         f0 = self.f0_d if f0 is None else f0
         if self.sg:
-            return self.model(f0[..., 0], P, rand_ini=self.rand_ini, utterance_offset=self.rank * self.B)
-        return self.model(None, f0, None, utterance_offset=self.rank * self.B)[0]
+            out = self.model(f0[..., 0], P, rand_ini=self.rand_ini, utterance_offset=self.rank * self.B)
+            self.last = {"out": out}
+            return out
+        signal, _, (harmonic, noise) = self.model(None, f0, None, utterance_offset=self.rank * self.B)
+        self.last = {"signal": signal}             # CombSubFast / SuperFast return the signal three times
+        if harmonic is not signal:
+            self.last.update(harmonic=harmonic, noise=noise)
+        return signal
 
     # rows [lo, hi) of the local batch (for the chunked synth+gather pipeline) -> [hi-lo, row_len]
     @property
@@ -517,7 +529,7 @@ def time_other_workload(name, dev, flush, torch, steps=10, warmup=3):
            "e2e_value": n / (e2e_ms * 1e-3) / 1e6, "e2e_ms_per_step": e2e_ms,
            "roofline": {"kernel": dom, "frac": alg / (kt[dom] * 1e-3) / 1e9 / peak,
                         "whole_path_frac": alg / (ms * 1e-3) / 1e9 / peak, "algorithmic_bytes_per_launch": alg,
-                        "traffic": ncu_traffic(name, dom), "kernel_ms": kt}}
+                        "kernel_ms": kt}}
     del run
     torch.cuda.empty_cache()
     return out
@@ -533,26 +545,6 @@ def eager_gpu_baseline(w, run, flush, torch, reps=3):
         f0, ctrls = run.f0_d, run.ctrl_d
     kind, what = "port", "oracle port of the reference (same ATen operators)"
     fwd = lambda f, c: oracle_forward(w, f, c)
-    if w["kind"] == "sins":
-        try:                                   # the unmodified reference class when its sources travelled (baseline/_ref)
-            import contextlib, io
-            from oracle import ref_loader
-            if ref_loader.available():
-                with contextlib.redirect_stdout(io.StringIO()):
-                    V = ref_loader.load()[0]
-                    ref = V.Sins(SR, P, w["H"], w["Ma"], w["Mn"], n_unit=8, n_spk=1).to(run.dev).eval()
-
-                class Fixed(torch.nn.Module):
-                    def forward(self, *a, **k):
-                        return self.c, None
-                ref.unit2ctrl = Fixed()
-
-                def fwd(f, c):                 # noqa: F811 -- Sins.forward of the reference, DSP only (controls preset)
-                    ref.unit2ctrl.c = c
-                    return ref(None, f, None)
-                kind, what = "reference", "the reference's own ddsp.vocoder.Sins.forward (unmodified sources staged under baseline/_ref, Unit2Control replaced by preset controls)"
-        except Exception as e:                 # fall back to the port, say why
-            what += " [reference classes unavailable: %s]" % (str(e).splitlines()[0][:80] if str(e) else type(e).__name__)
     fwd(f0[:2], {k: v[:2] for k, v in ctrls.items()} if ctrls else None)     # cuFFT plans, allocator
     ts = []
     for _ in range(reps):
@@ -591,8 +583,7 @@ def main():
                     help="device-timed step only: skip the host-buffer e2e, per-kernel and CPU legs (sweeps)")
     ap.add_argument("--e2e-chunks", default="6,10,10,6",
                     help="utterance chunks of the host-buffer pipeline: a count (1 = serial) or comma-separated "
-                         "relative sizes (default tapered: short fill and drain; round-2 sweep on the Sins workload, "
-                         "gpurun_out/e2e_sweep.txt: 6,10,10,6 -> 2.02 ms, 4,8,12,6,2 -> 2.10, 16,16 -> 2.35)")
+                         "relative sizes (default tapered: short fill and drain)")
     ap.add_argument("--e2e-streams", type=int, default=1,
                     help="compute streams of the host-buffer pipeline (HostPipeline(compute_streams=...); >1 not yet measured)")
     ap.add_argument("--fir-impl", default="auto", choices=["auto", "cuda", "tc", "cuda8", "fft"],
@@ -607,7 +598,13 @@ def main():
     ap.add_argument("--sinegen-impl", default="auto", choices=["auto", "v1", "v2", "v2p", "v2r7"],
                     help="A/B switch for the SineGen / source-module kernel (ops.set_sinegen_impl)")
     ap.add_argument("--breakdown", action="store_true", help="also print per-kernel times to stderr")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last step returned as DIR/<name>.npy (float32, at most "
+                         "64 MB in all; larger outputs as a fixed seeded sample of their elements); --gpus 1 only")
     args = ap.parse_args()
+    if args.dump_outputs and (args.e2e_only or args.impl != "b200" or args.steps < 1):
+        ap.error("--dump-outputs writes the last timed step of the device path: it needs --steps >= 1 and no --e2e-only "
+                 "or --impl reference")
     w = WORKLOADS[args.workload]
     if args.impl == "reference":
         return run_reference_arm(args, w)
@@ -616,12 +613,15 @@ def main():
     import torch
     import torch.distributed as dist
     from ddsp_svc_b200 import ops, sharding
+    torch.manual_seed(0)          # the in-kernel noise seeds come from torch's CPU generator: same inputs every run
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
         raise SystemExit("bench.py needs a CUDA device (no CPU fallback for the product path)")
+    if args.dump_outputs and world > 1:
+        raise SystemExit("--dump-outputs needs --gpus 1")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -643,7 +643,7 @@ def main():
         run.ops.set_fft_arith(args.fft_arith)
     B, nF, T = run.B, run.nF, run.T
     do_gather = world > 1 and not args.no_gather
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     n_chunks, n_streams = args.gather_chunks, args.gather_streams
     peer = None
@@ -736,6 +736,8 @@ def main():
         wall = time.perf_counter() - wall0
         launches = ops.launches() - n0
         dev_ms = sum(a.elapsed_time(b) for a, b in ev)
+        if args.dump_outputs:
+            dump_outputs(run.last, args.dump_outputs, torch)
         gather_checked = check_gather() if do_gather else None
 
         # ---- end to end through the public module API with HOST buffers ----
@@ -781,7 +783,7 @@ def main():
                        "l2": "flushed between steps (256 MiB memset, untimed); per-step CUDA events summed",
                        "wall_ms_per_step_incl_flush": 1e3 * wall / args.steps},
             "roofline": {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": ncu_traffic(args.workload, dom), "peak_source": peak_src,
+                         "frac": achieved / peak, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": alg_bytes, "kernel_ms": kt,
                          "whole_path_frac": alg_bytes / (ms_per_step * 1e-3) / 1e9 / peak if world == 1 else None,
                          "note": "achieved = algorithmic bytes of the whole path / duration of the dominant kernel; "

@@ -1,4 +1,4 @@
-"""ddsp_svc_b200 -- B200 (sm_100a) kernels for the DDSP harmonic-plus-noise synthesis path of
+"""ddsp_svc_b200 -- H100 (sm_90a) kernels for the DDSP harmonic-plus-noise synthesis path of
 yxlllc/DDSP-SVC, behind the reference's Sins / CombSub / CombSubFast / CombSubSuperFast / SineGen forward()
 API.  See DESIGN.md for the path, its boundary and the kernels; include/b200ddsp.h for the C ABI.
 """

@@ -1,6 +1,6 @@
 """ctypes binding of libb200ddsp.so (the C ABI declared in include/b200ddsp.h).
 
-The library is built in-tree by ``build()`` (nvcc, sm_100a only) and travels with the repo.
+The library is built in-tree by ``build()`` (nvcc, sm_90a only) and travels with the repo.
 There is NO fallback: if the shared library is missing or fails to load, importing the ops
 raises -- the product path never degrades to PyTorch or to the oracle.
 """
@@ -16,7 +16,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB_PATH = os.environ.get("B2D_LIB_PATH") or os.path.join(HERE, "libb200ddsp.so")
 HEADER = os.path.join(ROOT, "include", "b200ddsp.h")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
 c_f32p = ctypes.c_void_p   # device pointers travel as integers
@@ -115,7 +115,7 @@ def _stale():
 
 
 def build(force=False, verbose=False, out=None, defines=()):
-    """Compile every CUDA source for sm_100a into ddsp_svc_b200/libb200ddsp.so (in-tree).
+    """Compile every CUDA source for sm_90a into ddsp_svc_b200/libb200ddsp.so (in-tree).
     ``out`` / ``defines``: build a compile-time variant (-DNAME=VALUE ...) into another file for A/B runs
     (loaded with B2D_LIB_PATH=<file>)."""
     default = os.path.join(HERE, "libb200ddsp.so")

@@ -40,11 +40,23 @@ int sins_fused_launch(const float* f0, const double* frame_phase, const float* c
 
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+int num_sms() {
+    static std::atomic<int> cache[64];
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) { cudaGetLastError(); return 132; }
+    int n = cache[dev].load(std::memory_order_relaxed);
+    if (n <= 0) {
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) { cudaGetLastError(); n = 132; }
+        cache[dev].store(n, std::memory_order_relaxed);
+    }
+    return n;
+}
+
 }  // namespace b2d
 
 namespace b2d {
-// Packed f32x2 complex additions are the default since round 2 (whole GPU suite green with them, 2.5 % / 1.2 % faster FIR /
-// SuperFast kernels).  B2D_FFT_ARITH=scalar in the environment picks the scalar instantiations as the initial value
+// The "packed" instantiations are the default (on Hopper they compile to the same scalar additions as the others).
+// B2D_FFT_ARITH=scalar in the environment picks the scalar instantiations as the initial value
 // (whole-suite A/B runs); b2d_set_fft_arith overrides at run time.
 static int fft_arith_default() {
     const char* e = getenv("B2D_FFT_ARITH");
@@ -114,11 +126,9 @@ static SideLane* side_lane() {
 }
 }  // namespace b2d
 
-// 0 = auto = 1 (separate bank kernel, measured faster), 1 = separate bank kernel, 2 = bank fused into the FFT-domain FIR
-// kernel.  Measured on B200 (B = 32 x 10 s): fused 0.800 ms/step, separate 0.789: with 168 registers only three 4-warp CTAs
-// fit an SM, and ONE warp per scheduler in the bank phase cannot keep the FMA pipe busy (the stand-alone bank kernel has
-// four), so the fused kernel takes bank + FIR = 0.64 ms -- the expected filling of the FIR's idle issue slots does not
-// happen.  It stays selectable: one launch less, no [B, T] sinusoid round trip.
+// 0 = auto = 1 (separate bank kernel), 1 = separate bank kernel, 2 = bank fused into the FFT-domain FIR kernel: with 168
+// registers only three 4-warp CTAs fit an SM, and ONE warp per scheduler in the bank phase cannot keep the FMA pipe busy
+// (the stand-alone bank kernel has four).  It stays selectable: one launch less, no [B, T] sinusoid round trip.
 namespace b2d { std::atomic<int> g_sins_impl{0}; }
 extern "C" int b2d_set_sins_impl(int impl) {
     if (impl < 0 || impl > 3) return b2d::fail(B2D_ERR_UNSUPPORTED, "set_sins_impl: %d not in {0, 1, 2, 3}", impl);
@@ -217,11 +227,10 @@ extern "C" int b2d_sins_synth(const float* f0_frames, const double* frame_phase,
     };
     // ---- spectrum path (opt-in, b2d_set_sins_impl(3)): impulse responses -> their packed spectra once per frame (both on
     // the side stream, beside the bank), then the FIR kernel reads the spectra: a quarter of its transforms and a third of
-    // its shared memory disappear (126 registers, 53 KB: 4 CTAs per SM instead of 3).  Measured on B200 (B = 32 x 10 s):
-    // 0.819 ms per step against 0.789 for the default -- the transform of the impulse responses is only MOVED (the extra
-    // kernel costs ~0.06 ms) and the FIR kernel now waits for 226 MB of spectra right before its products; it pays only
-    // once the tcgen05 GEMM of the impulse-response stage emits these spectra itself (DESIGN.md section 9).  Kept as the
-    // tested consumer side of that plan. ----
+    // its shared memory disappear (126 registers, 53 KB: 4 CTAs per SM instead of 3).  The transform of the impulse
+    // responses is only MOVED and the FIR kernel waits for the spectra right before its products; it pays only once the
+    // tensor-core GEMM of the impulse-response stage emits these spectra itself.  Kept as the tested consumer side of that
+    // plan. ----
     {
         const int simpl0 = b2d::g_sins_impl.load(std::memory_order_relaxed);
         const bool can_spec = b2d::fir_spec_supported(block, La, Ln) && b2d::fir_fft_selected();
@@ -292,7 +301,7 @@ extern "C" int b2d_sins_synth(const float* f0_frames, const double* frame_phase,
     if (e != cudaSuccess) return b2d::fail((int)e, "sins_synth: fork: %s", cudaGetErrorString(e));
     // a small launch (one utterance, one pipeline chunk) leaves most SMs idle: its two impulse-response builds are latency
     // bound single waves, so they run side by side on the two side streams instead of one after the other
-    const bool two_lanes = nsplit == 1 && (long long)B * n_frames <= 148LL * 64;
+    const bool two_lanes = nsplit == 1 && (long long)B * n_frames <= (long long)b2d::num_sms() * 64;
     cudaStream_t side2 = two_lanes ? (side == lane->hi ? lane->lo : lane->hi) : side;
     if (two_lanes) {
         e = cudaStreamWaitEvent(side2, lane->fork, 0);

@@ -1,4 +1,4 @@
-// Shared host/device helpers for libb200ddsp (sm_100a only).
+// Shared host/device helpers for libb200ddsp (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -13,6 +13,10 @@
 // ---------------------------------------------------------------------------------------
 namespace b2d {
 
+// SM count of the current device (cached per device; 132 on the H100 SXM): the launch heuristics size grids and chunk
+// lengths so that a launch fills one or a few waves
+int num_sms();
+
 char* err_buf();                                   // thread-local, defined in api.cu
 int   fail(int code, const char* fmt, ...);       // formats into err_buf, returns code
 
@@ -22,7 +26,7 @@ inline int check_launch(const char* what) {
     return 0;
 }
 
-// b2d_set_fft_arith(1): the FFT kernels (ltv_fir_fft, superfast, combsubfast) use packed f32x2 complex additions
+// b2d_set_fft_arith(1): the FFT kernels (ltv_fir_fft, superfast, combsubfast) use their "packed" instantiations
 extern std::atomic<int> g_fft_packed;   // debug A/B switch (b2d_set_fft_arith), read once per call
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 

@@ -6,7 +6,7 @@
 //     S_q   = rfft(w * comb_q) * exp(m_h + j pi p_h) + rfft(w * noise_q) * exp(m_n) / 128     (row min(q, nF-1))
 //     out   = overlap-add( w * irfft(S_q) ), cropped by P on both sides; no envelope division (w^2 is COLA)
 //
-// Design (B200).  HBM traffic: 3 x 513 control values per frame = 12 B per output sample, + 4 B comb in and 4 B
+// Design.  HBM traffic: 3 x 513 control values per frame = 12 B per output sample, + 4 B comb in and 4 B
 // out; everything else stays on chip.  23.4 KB shared memory, 128 registers -> 4 CTAs per SM.
 //  * one CTA owns G consecutive hops (G even) of one utterance and walks the G+1 frames that touch them plus the one
 //    that completes the last pair, TWO frames per iteration;
@@ -64,7 +64,7 @@ __device__ __forceinline__ BinFilter make_filter(float hm, float hp, float nm) {
 constexpr size_t kSmemBytes = (size_t)2 * kPad * sizeof(float2) + (size_t)(kTw2 + kTw3) * sizeof(float2) +
                               (size_t)kN * sizeof(float);      // 17408 + 1920 + 4096 = 23424 B
 
-// PK: complex additions as packed f32x2 instructions (fft_regs.cuh Ar<true>)
+// PK: the "packed" complex-addition policy (fft_regs.cuh Ar<true>; scalar on Hopper)
 template <bool PK>
 __global__ void __launch_bounds__(kThreads, 4) combsubfast_kernel(CfParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -233,7 +233,7 @@ extern "C" int b2d_combsubfast_filter(const float* comb, const float* c_harmonic
     p.c_hm = c_harmonic_magnitude; p.c_hp = c_harmonic_phase; p.c_nm = c_noise_magnitude;
     p.ctrl_stride = ctrl_stride; p.out = signal; p.nF = n_frames;
     int G = 32;            // hops per CTA: shorter chunks when the launch would not fill the GPU (cf. ltv_fir_fft.cu)
-    while (G > 2 && (long long)B * ((n_frames + G - 1) / G) < 148LL * 2) G >>= 1;
+    while (G > 2 && (long long)B * ((n_frames + G - 1) / G) < (long long)b2d::num_sms() * 2) G >>= 1;
     p.G = G;
     p.seed = seed; p.utt_off = utterance_offset;
     const dim3 grid((unsigned)((n_frames + p.G - 1) / p.G), B);

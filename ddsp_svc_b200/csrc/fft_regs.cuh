@@ -14,30 +14,12 @@ __device__ __forceinline__ float2 cmul(float2 a, float2 b) {
 }
 __device__ __forceinline__ float2 mul_mj(float2 a) { return make_float2(a.y, -a.x); }  // a * (-j)
 
-// Complex add / subtract policy.  PK = false: two scalar FADDs.  PK = true: one packed add.rn.f32x2 / sub.rn.f32x2
-// (SASS FADD2; a float2 that comes from a 64-bit shared-memory load is already an aligned register pair, so the
-// mov.b64 pack / unpack disappear).  Identical results (per-lane IEEE add); half the issue slots for the ~2/3 of an
-// FFT's instructions that are butterfly additions.
+// Complex add / subtract policy.  PK selects the "packed" instantiation of the FFT kernels (b2d_set_fft_arith); Hopper
+// has no packed FP32 add (f32x2 needs sm_100), so both policies are two scalar FADDs and give identical results.
 template <bool PK> struct Ar {
     static __device__ __forceinline__ float2 add(float2 a, float2 b) { return cadd(a, b); }
     static __device__ __forceinline__ float2 sub(float2 a, float2 b) { return csub(a, b); }
 };
-#ifndef B2D_HOST_EMU
-template <> struct Ar<true> {
-    static __device__ __forceinline__ unsigned long long pk(float2 a) {
-        unsigned long long r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a.x), "f"(a.y)); return r;
-    }
-    static __device__ __forceinline__ float2 upk(unsigned long long v) {
-        float2 a; asm("mov.b64 {%0, %1}, %2;" : "=f"(a.x), "=f"(a.y) : "l"(v)); return a;
-    }
-    static __device__ __forceinline__ float2 add(float2 a, float2 b) {
-        unsigned long long d; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(pk(a)), "l"(pk(b))); return upk(d);
-    }
-    static __device__ __forceinline__ float2 sub(float2 a, float2 b) {
-        unsigned long long d; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(pk(a)), "l"(pk(b))); return upk(d);
-    }
-};
-#endif
 
 // forward DFT of 2^n points, natural order in and out (recursive decimation in time, unrolled)
 template <int R, bool PK = false> struct Dft;

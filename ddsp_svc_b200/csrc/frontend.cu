@@ -143,7 +143,7 @@ extern "C" int b2d_mask_apply(float* signal, const float* mask_frames, int B, in
     const bool vec = (block % 4 == 0) && b2d::aligned16(signal);
     const size_t work = vec ? T / 4 : T;
     unsigned gx = (unsigned)((work + 255) / 256);
-    if (gx > 148u * 16u) gx = 148u * 16u;
+    if (gx > (unsigned)b2d::num_sms() * 16u) gx = (unsigned)b2d::num_sms() * 16u;
     if (gx == 0) gx = 1;
     dim3 grid(gx, B);
     if (vec) mask_apply_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(signal, mask_frames, n_mask_frames, frame_offset, n_frames, block);
@@ -158,7 +158,7 @@ extern "C" int b2d_cross_fade(const float* a, int64_t len_a, const float* b, int
                          (long long)len_a, (long long)len_b, (long long)idx);
     const long long total = idx + len_b;
     long long gx = (total + 255) / 256;
-    if (gx > 148 * 16) gx = 148 * 16;
+    if (gx > b2d::num_sms() * 16) gx = b2d::num_sms() * 16;
     cross_fade_kernel<<<(unsigned)gx, 256, 0, (cudaStream_t)stream>>>(a, len_a, b, len_b, idx, out);
     return b2d::check_launch("cross_fade");
 }

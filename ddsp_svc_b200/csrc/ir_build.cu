@@ -253,7 +253,7 @@ extern "C" int b2d_dft_tables(int n_mag, float* dft_tables, void* stream) {
     if (!dft_tables) return b2d::fail(B2D_ERR_NULL, "dft_tables: null pointer");
     if (n_mag < 2 || n_mag > 4097) return b2d::fail(B2D_ERR_SHAPE, "dft_tables: n_mag=%d out of range", n_mag);
     if ((reinterpret_cast<uintptr_t>(dft_tables) & 255u) != 0) return b2d::fail(B2D_ERR_ALIGN, "dft_tables: buffer must be 256-byte aligned");
-    dft_tables_kernel<<<148 * 2, 256, 0, (cudaStream_t)stream>>>(n_mag, dft_tables);
+    dft_tables_kernel<<<b2d::num_sms() * 2, 256, 0, (cudaStream_t)stream>>>(n_mag, dft_tables);
     int rc = b2d::check_launch("dft_tables");
     if (rc) return rc;
     float* img = reinterpret_cast<float*>(reinterpret_cast<char*>(dft_tables) + b2d::cc_table_bytes(n_mag));

@@ -1,25 +1,25 @@
-// K3-TC: impulse responses from raw controls on the tensor cores (tcgen05.mma kind::tf32, 3xTF32).
+// K3-TC: impulse responses from raw controls on the Hopper tensor cores (wgmma tf32, 3xTF32).
 // Same math as ir_build.cu (reference ddsp/core.py:254-270 + windows + activations): per frame
 //   C(t) = Ce + Co, C(M-1-t) = Ce - Co, S(t) = Se + So, S(M-1-t) = So - Se,
 //   Ce[t] = sum_{m even} R_m cos(w m t), Se = sum_{m even} I_m sin(w m t), (Co, So: odd m)
-// i.e. four GEMMs  [frames x K] . [K x Nt]  against CONSTANT tables -- a proper GEMM (M = 128 frames
-// per CTA, N = Nt = 128 columns, K = 128 bins per parity), unlike the FIR: every table element is
-// reused by 128 frames, so the operands are worth their shared-memory traffic.
+// i.e. four GEMMs  [frames x K] . [K x Nt]  against CONSTANT tables -- a proper GEMM (M = 64 frames
+// per CTA, N = Nt <= 128 columns, K = 128 bins per parity), unlike the FIR: every table element is
+// reused by 64 frames, so the operands are worth their shared-memory traffic.
 //
-// Pipeline per CTA (128 frames = 128 TMEM lanes, 512 threads):
+// Pipeline per CTA (64 frames = one wgmma M tile, 512 threads = 4 warpgroups):
 //   * tables live in global memory already in the K-major no-swizzle operand image, hi/lo split,
 //     one contiguous block per (chunk of 8 K, table): they are fetched with 1-D bulk async copies
-//     (TMA) on an mbarrier, double buffered;
-//   * per chunk of 16 bins all threads evaluate pi*tanh(c) (coalesced), 128 threads carry the
+//     (TMA) on an mbarrier, double buffered, one chunk ahead;
+//   * per chunk of 16 bins all threads evaluate pi*tanh(c) (coalesced), 64 threads carry the
 //     per-frame running sum (sequential along K: fp64 accumulate / fp32 emit like torch's CPU
 //     cumsum), then all threads evaluate sincos / exp, split into tf32 hi + lo and write the A
-//     operand chunk (canonical layout) to shared memory;
-//   * thread 0 issues 3 MMAs (hi*hi, lo*hi, hi*lo) per accumulator and chunk, tcgen05.commit frees
-//     the stage; accumulators Ce | Se | Co | So sit side by side in TMEM (4 x 128 columns);
-//   * epilogue: 16 warps = 4 TMEM lane quarters x 4 column groups read the accumulators
-//     (tcgen05.ld), form the four taps per column, apply the window, stage them in shared memory
-//     (XOR-swizzled) and the CTA writes the IR rows with coalesced 64-byte segments.
-// fp32 TMEM accumulation truncates (~0.5 ulp per step, 48 steps per accumulator): <= 3e-6 relative
+//     operand chunk to shared memory;
+//   * warpgroup w owns the 16-column tiles w, w + 4, ... of every accumulator (Ce | Se | Co | So), in
+//     registers: it loads its A fragments from shared memory into registers and issues 3 wgmmas
+//     (hi*hi, lo*hi, hi*lo) per accumulator tile, B straight from the TMA-filled stage;
+//   * epilogue: each thread holds all accumulators of its (frame, column) pairs, forms the four taps per
+//     column, applies the window and stores them.
+// fp32 tensor-core accumulation truncates (~0.5 ulp per step, 48 steps per accumulator): <= 3e-6 relative
 // gain error on the taps, far below the parity gate.
 #include "b2d_common.cuh"
 
@@ -34,9 +34,9 @@ __host__ __device__ inline size_t tc_image_floats(int M) { return (size_t)(tc_kp
 namespace {
 
 constexpr int kThreads = 512;
-constexpr int kRows = 128;               // frames per CTA = TMEM lanes
-constexpr int kABlock = kRows * 8;       // floats per A block: [2 k-chunks][128 rows][4]
-constexpr int kStagingFloats = 4 * 4 * kRows * 16;   // epilogue staging (128 KB); also >= the two operand stages
+constexpr int kRows = 64;                // frames per CTA = wgmma M
+constexpr int kABlock = kRows * 8;       // floats per A block: [64 rows][4 k pairs (k, k + 4)]
+constexpr int kAccRegs = 64;             // accumulator registers per thread: NACC x (16-column tiles per warpgroup) x 8
 
 __device__ __forceinline__ uint32_t tf32_rn_bits(float x) {
     uint32_t u = __float_as_uint(x);
@@ -47,29 +47,25 @@ __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
     hi = __uint_as_float(tf32_rn_bits(x));
     lo = __uint_as_float(tf32_rn_bits(x - hi));
 }
+// wgmma shared-memory descriptor, K-major, no swizzle: LBO = byte stride between the two core matrices along K,
+// SBO = byte stride between 8-row groups
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFF);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
     return d;
 }
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t acc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n"
-                 ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(acc) : "memory");
+// D[64 x 16] += A[64 x 8] (registers, tf32) . B[8 x 16] (shared memory, tf32)
+__device__ __forceinline__ void wgmma_tf32_m64n16k8(float (&d)[8], const uint32_t (&a)[4], uint64_t db) {
+    asm volatile("wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, 1, 1, 1;\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
+// keeps a register live (and unmoved) across asynchronous wgmma reads of it
+__device__ __forceinline__ void fence_reg(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+__device__ __forceinline__ void fence_reg(uint32_t& r) { asm volatile("" : "+r"(r)::"memory"); }
 
 struct IrTcParams {
     const float* c;
@@ -77,72 +73,71 @@ struct IrTcParams {
     const float* f0;
     const float* image;      // tensor-core table image
     int n_total, M;
-    int rows;                // frames a CTA actually fills of its 128 TMEM lanes: 128, or 64 / 32 for small launches
     float hw_num;
     float* ir;
 };
 
-// MODE as in b200ddsp.h.  NACC = 4 (all-pass: Ce Se Co So) or 2 (magnitude: Ce Co).
-// 512 threads: every phase except the 16-term per-frame prefix sum is spread over all 16 warps
-// (the first version ran one thread per frame on 4 warps and was latency bound at 15 % issue).
-// Register cap: one CTA per SM either way (shared memory, TMEM), but with 64 registers x 512 threads the CTA leaves half
-// of the register file to the oscillator-bank CTAs that b2d_sins_synth runs beside it (api.cu, fork/join).
-#ifndef B2D_IR_TC_MAXREG
-#define B2D_IR_TC_MAXREG 0
-#endif
-#if B2D_IR_TC_MAXREG > 0
-#define B2D_IR_TC_BOUNDS __maxnreg__(B2D_IR_TC_MAXREG)
-#else
-#define B2D_IR_TC_BOUNDS __launch_bounds__(kThreads, 1)
-#endif
+// MODE as in b200ddsp.h.  NACC = 4 (all-pass: Ce Se Co So; Npad <= 128) or 2 (magnitude: Ce Co; Npad <= 256): either
+// way NACC x JT tiles x 8 = 64 accumulator registers per thread.  ROWS = frames a CTA actually fills of its 64 tile
+// rows: 64, or 32 for small launches (latency bound: the activations and the write-out scale with the rows, the MMAs do
+// not care -- a D row depends on its own A row only; the unused A rows are never written and their D rows never read).
 template <int MODE, int ROWS>
-__global__ void B2D_IR_TC_BOUNDS ir_build_tc_kernel(IrTcParams p) {
+__global__ void __launch_bounds__(kThreads, 1) ir_build_tc_kernel(IrTcParams p) {
     constexpr bool kAllpass = (MODE == B2D_IR_ALLPASS);
     constexpr int NACC = kAllpass ? 4 : 2;
+    constexpr int JT = kAccRegs / (8 * NACC);                      // 16-column tiles per warpgroup
+    static_assert(ROWS == 32 || ROWS == 64, "rows per CTA");
+    constexpr int rows = ROWS, urows = ROWS >> 5;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int M = p.M, L = 2 * (M - 1), Nt = (M - 1) / 2 + 1;
-    const int Npad = b2d::tc_npad(M), NC = b2d::tc_kpad(M) / 8;
+    const int Npad = b2d::tc_npad(M), NC = b2d::tc_kpad(M) / 8, NT16 = Npad / 16;
     const int bblock = Npad * 8;                                   // floats per B block
-    const int stage_floats = NACC * 2 * kABlock + NACC * 2 * bblock;
-    float* stage0 = reinterpret_cast<float*>(smem_raw);            // 2 operand stages; reused as output staging
-    float* wtab = stage0 + kStagingFloats;                         // [L] Hann window (MAG_HANN)
-    float* gds = wtab + ((L + 3) & ~3);                            // [128][17] pi*tanh(c) of the chunk, then the fp32 phase
-    __shared__ __align__(8) uint64_t b_full[2], mma_done[2];
-    __shared__ uint32_t tmem_base_s;
+    const int sa_floats = NACC * 2 * kABlock, sb_floats = NACC * 2 * bblock;
+    float* sA0 = reinterpret_cast<float*>(smem_raw);               // [2 stages][kind][hi|lo][64 rows][4][2]
+    float* sB0 = sA0 + 2 * sa_floats;                              // [2 stages][table][hi|lo][2 k-chunks][Npad][4]
+    float* wtab = sB0 + 2 * sb_floats;                             // [L] Hann window (MAG_HANN)
+    float* gds = wtab + ((L + 3) & ~3);                            // [64][17] pi*tanh(c) of the chunk, then the fp32 phase
+    __shared__ __align__(8) uint64_t b_full[2];
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    // Small launches (one utterance of a real-time caller, a chunk of the host pipeline) are latency bound: a CTA then
-    // fills only `rows` of its 128 lanes -- the activations and the write-out scale with the rows, the MMAs do not care
-    // (a D row depends on its own A row only; the unused A rows are never written and their D rows never read).
-    constexpr int rows = ROWS, urows = ROWS >> 5;
-    static_assert(ROWS == 32 || ROWS == 64 || ROWS == 128, "rows per CTA");
+    const int tid = threadIdx.x, wg = tid >> 7, wtid = tid & 127, lane = tid & 31;
     const int F0 = blockIdx.x * rows;
     const float invL = 1.0f / (float)L;
-    constexpr uint32_t kTmemCols = 512;
 
+    // tables of chunk ch -> stage ch & 1 (TMA bulk copies).  Image: [chunk][cosE hi lo, sinE hi lo, cosO hi lo, sinO hi lo]
+    auto load_tables = [&](int ch) {
+        float* sB = sB0 + (ch & 1) * sb_floats;
+        uint64_t* bar = &b_full[ch & 1];
+        b2d::mbar_arrive_expect_tx(bar, (uint32_t)(NACC * 2 * bblock * 4));
+        const float* src = p.image + (size_t)ch * 8 * bblock;
+        if (kAllpass) {
+            b2d::tma_load_1d(sB, src, (uint32_t)(8 * bblock * 4), bar);
+        } else {                                                   // cosE hi/lo and cosO hi/lo only
+            b2d::tma_load_1d(sB, src, (uint32_t)(2 * bblock * 4), bar);
+            b2d::tma_load_1d(sB + 2 * bblock, src + 4 * bblock, (uint32_t)(2 * bblock * 4), bar);
+        }
+    };
     if (tid == 0) {
         b2d::mbar_init(&b_full[0], 1); b2d::mbar_init(&b_full[1], 1);
-        b2d::mbar_init(&mma_done[0], 1); b2d::mbar_init(&mma_done[1], 1);
         b2d::fence_mbar_init();
-    }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(b2d::smem_u32(&tmem_base_s)), "n"(kTmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+        load_tables(0);
     }
     if (MODE == B2D_IR_MAG_HANN)
         for (int i = tid; i < L; i += kThreads) wtab[i] = 0.5f - 0.5f * cospif(2.0f * invL * (float)i);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_d = tmem_base_s;
-    // D = F32, A = B = TF32, K-major, M = 128, N = Npad
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(Npad >> 3) << 17) | (8u << 24);
 
-    double run = 0.0;      // threads 0..127: group-delay cumsum of frame F0 + tid (fp64 accumulate, fp32 emit)
+    float acc[NACC][JT][8];
+#pragma unroll
+    for (int a = 0; a < NACC; ++a)
+#pragma unroll
+        for (int j = 0; j < JT; ++j)
+#pragma unroll
+            for (int i = 0; i < 8; ++i) acc[a][j][i] = 0.f;
+
+    double run = 0.0;      // threads 0..rows-1: group-delay cumsum of frame F0 + tid (fp64 accumulate, fp32 emit)
 
     // raw controls of a chunk (element e = tid + 512 u -> row e >> 4, bin 16 ch + (e & 15)); fetched one chunk ahead so
-    // the global-load latency hides behind the previous chunk's barriers (it was the top stall of the first version)
-    float cpre[4];
+    // the global-load latency hides behind the previous chunk's barriers
+    float cpre[urows];
     auto fetch = [&](int ch) {
 #pragma unroll
         for (int u = 0; u < urows; ++u) {
@@ -154,23 +149,9 @@ __global__ void B2D_IR_TC_BOUNDS ir_build_tc_kernel(IrTcParams p) {
 
     for (int ch = 0; ch < NC; ++ch) {
         const int st = ch & 1;
-        float* sA = stage0 + st * stage_floats;                    // A blocks: [kind][hi|lo][2][128][4]
-        float* sB = sA + NACC * 2 * kABlock;                       // B blocks: [table][hi|lo][2][Npad][4]
-        if (ch >= 2) {                                             // stage reuse: its MMAs (chunk ch-2) must be done
-            b2d::mbar_wait(&mma_done[st], (uint32_t)(((ch >> 1) - 1) & 1));
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        }
-        if (tid == 0) {                                            // tables of this chunk: TMA bulk copies
-            b2d::mbar_arrive_expect_tx(&b_full[st], (uint32_t)(NACC * 2 * bblock * 4));
-            const float* src = p.image + (size_t)ch * 8 * bblock;  // image: [chunk][cosE hi lo, sinE hi lo, cosO hi lo, sinO hi lo]
-            if (kAllpass) {
-                b2d::tma_load_1d(sB, src, (uint32_t)(8 * bblock * 4), &b_full[st]);
-            } else {                                               // cosE hi/lo and cosO hi/lo only
-                b2d::tma_load_1d(sB, src, (uint32_t)(2 * bblock * 4), &b_full[st]);
-                b2d::tma_load_1d(sB + 2 * bblock, src + 4 * bblock, (uint32_t)(2 * bblock * 4), &b_full[st]);
-            }
-        }
-        // element e = (row, i): bins 16 ch + i, i = 0..15;  2048 elements, 4 per thread, 16 lanes per row
+        float* sA = sA0 + st * sa_floats;                          // A blocks: [kind][hi|lo][64][4][2]
+        const float* sB = sB0 + st * sb_floats;
+        // element e = (row, i): bins 16 ch + i, i = 0..15;  16 lanes per row
         if (kAllpass) {
             // phase 1: pi * tanh(c)   (:581)
 #pragma unroll
@@ -213,9 +194,9 @@ __global__ void B2D_IR_TC_BOUNDS ir_build_tc_kernel(IrTcParams p) {
                 if (MODE == B2D_IR_MAG_HANN) v *= 0.0078125f;
                 r = v * wgt;
             }
-            // A element (row, k) of parity par: ((k >> 2) * 128 + row) * 4 + (k & 3)
+            // A element (row, k) of parity par: k and k + 4 side by side, the pair a thread's fragment needs
             const int par = i & 1, k = i >> 1;
-            const int pos = ((k >> 2) * kRows + row) * 4 + (k & 3);
+            const int pos = row * 8 + (k & 3) * 2 + (k >> 2);
             float h, l;
             split_tf32(r, h, l);
             const int kindR = kAllpass ? 2 * par : par;            // all-pass kinds: Re, Ie, Ro, Io ; magnitude: Re, Ro
@@ -228,44 +209,70 @@ __global__ void B2D_IR_TC_BOUNDS ir_build_tc_kernel(IrTcParams p) {
             }
         }
         if (!kAllpass && ch + 1 < NC) fetch(ch + 1);
-        b2d::fence_proxy_async();
         __syncthreads();
-        if (tid == 0) {
-            b2d::mbar_wait(&b_full[st], (uint32_t)((ch >> 1) & 1));
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t a0 = b2d::smem_u32(sA), b0 = b2d::smem_u32(sB);
+        // the other stage's last readers (chunk ch - 1's wgmmas) completed before this barrier: prefetch into it
+        if (tid == 0 && ch + 1 < NC) load_tables(ch + 1);
+
+        // ---- MMAs of warpgroup wg: A fragments (rows 16 warp + lane / 4 (+ 8), k = lane % 4 (+ 4)) from shared memory ----
+        uint32_t af[NACC][2][4];
+        {
+            const int r0 = 16 * (wtid >> 5) + (lane >> 2), kq = lane & 3;
 #pragma unroll
-            for (int a = 0; a < NACC; ++a) {
-                // accumulator a pairs A kind a with table a (all-pass: Re.cosE, Ie.sinE, Ro.cosO, Io.sinO)
-                const uint32_t ah = a0 + (a * 2 + 0) * kABlock * 4, al = a0 + (a * 2 + 1) * kABlock * 4;
-                const uint32_t bh = b0 + (a * 2 + 0) * bblock * 4, bl = b0 + (a * 2 + 1) * bblock * 4;
-                const uint32_t d = tmem_d + (uint32_t)(a * Npad);
-                const uint32_t lbo_a = kRows * 16, lbo_b = (uint32_t)Npad * 16;
-                mma_tf32(d, make_desc(ah, lbo_a, 128), make_desc(bh, lbo_b, 128), idesc, ch > 0 ? 1u : 0u);
-                mma_tf32(d, make_desc(al, lbo_a, 128), make_desc(bh, lbo_b, 128), idesc, 1u);
-                mma_tf32(d, make_desc(ah, lbo_a, 128), make_desc(bl, lbo_b, 128), idesc, 1u);
+            for (int a = 0; a < NACC; ++a)
+#pragma unroll
+                for (int hl = 0; hl < 2; ++hl) {
+                    const float* blk = sA + (a * 2 + hl) * kABlock;
+                    const float2 v0 = *reinterpret_cast<const float2*>(blk + r0 * 8 + kq * 2);
+                    const float2 v1 = *reinterpret_cast<const float2*>(blk + (r0 + 8) * 8 + kq * 2);
+                    af[a][hl][0] = __float_as_uint(v0.x); af[a][hl][1] = __float_as_uint(v1.x);
+                    af[a][hl][2] = __float_as_uint(v0.y); af[a][hl][3] = __float_as_uint(v1.y);
+                }
+        }
+        b2d::mbar_wait(&b_full[st], (uint32_t)((ch >> 1) & 1));
+#pragma unroll
+        for (int a = 0; a < NACC; ++a)
+#pragma unroll
+            for (int j = 0; j < JT; ++j)
+#pragma unroll
+                for (int i = 0; i < 8; ++i) fence_reg(acc[a][j][i]);
+        asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+        {
+            const uint32_t b0 = b2d::smem_u32(sB);
+            const uint32_t lbo_b = (uint32_t)Npad * 16;
+#pragma unroll
+            for (int j = 0; j < JT; ++j) {
+                // 16-column tile: columns 16 t .. 16 t + 15.  A tile past Npad recomputes the last one (never stored):
+                // a branch around wgmma would make ptxas serialise every wgmma of the kernel
+                const int t = min(wg + 4 * j, NT16 - 1);
+#pragma unroll
+                for (int a = 0; a < NACC; ++a) {
+                    // accumulator a pairs A kind a with table a (all-pass: Re.cosE, Ie.sinE, Ro.cosO, Io.sinO)
+                    const uint32_t bh = b0 + (uint32_t)((a * 2 + 0) * bblock * 4 + t * 256);
+                    const uint32_t bl = b0 + (uint32_t)((a * 2 + 1) * bblock * 4 + t * 256);
+                    wgmma_tf32_m64n16k8(acc[a][j], af[a][0], make_desc(bh, lbo_b, 128));
+                    wgmma_tf32_m64n16k8(acc[a][j], af[a][1], make_desc(bh, lbo_b, 128));
+                    wgmma_tf32_m64n16k8(acc[a][j], af[a][0], make_desc(bl, lbo_b, 128));
+                }
             }
-            asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(b2d::smem_u32(&mma_done[st])) : "memory");
+        }
+        asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+        asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+#pragma unroll
+        for (int a = 0; a < NACC; ++a) {
+#pragma unroll
+            for (int hl = 0; hl < 2; ++hl)
+#pragma unroll
+                for (int i = 0; i < 4; ++i) fence_reg(af[a][hl][i]);
+#pragma unroll
+            for (int j = 0; j < JT; ++j)
+#pragma unroll
+                for (int i = 0; i < 8; ++i) fence_reg(acc[a][j][i]);
         }
     }
-    // ---- all MMAs done? (the last use of each stage) ----
-    {
-        const int last0 = (NC - 1) - ((NC - 1) & 1), last1 = (NC >= 2) ? (NC - 1) - (((NC - 1) & 1) ^ 1) : -1;
-        b2d::mbar_wait(&mma_done[0], (uint32_t)((last0 >> 1) & 1));
-        if (last1 >= 0) b2d::mbar_wait(&mma_done[1], (uint32_t)((last1 >> 1) & 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    }
-    __syncthreads();
 
-    // ---- epilogue: warp (q, cg): TMEM lanes 32 q .. 32 q + 31, column blocks t0 = 16 (4 round + cg) ----
-    const int q = warp & 3, cg = warp >> 2;
-    const int row = 32 * q + lane;
-    const bool live = row < rows && F0 + row < p.n_total;
-    float* stg = stage0;                                           // [cg][4 groups][128 rows][16], XOR-swizzled columns
-    const uint32_t lane_base = tmem_d + ((uint32_t)(32 * q) << 16);
-    float hw = 1.f;
-    if (MODE == B2D_IR_MAG_DYNAMIC) hw = p.hw_num / ((live ? p.f0[F0 + row] : 0.f) + 1e-3f);
-    auto window = [&](int idx) -> float {
+    // ---- epilogue: accumulator register i of tile j holds row 16 warp + lane / 4 + 8 ((i >> 1) & 1),
+    //      column 16 t + 8 (i >> 2) + 2 (lane % 4) + (i & 1) ----
+    auto window = [&](int idx, float hw) -> float {
         if (MODE == B2D_IR_MAG_HANN) return wtab[idx];
         if (MODE == B2D_IR_MAG_DYNAMIC) {                          // (ddsp/core.py:244-246), cos(pi u) via exact reduction
             float u = (float)(idx - (M - 1)) / hw;
@@ -275,69 +282,41 @@ __global__ void B2D_IR_TC_BOUNDS ir_build_tc_kernel(IrTcParams p) {
         }
         return 1.f;
     };
-    const int nblk = Npad / 16;
-    for (int rnd = 0; rnd * 4 < nblk; ++rnd) {
-        const int blk = rnd * 4 + cg;
-        if (blk < nblk && 32 * q < rows) {
-            const int t0 = blk * 16;
-            float Ce[16], Co[16], Se[16], So[16];
-            if (kAllpass) {
-                tmem_ld16(lane_base + (uint32_t)(0 * Npad + t0), Ce);
-                tmem_ld16(lane_base + (uint32_t)(1 * Npad + t0), Se);
-                tmem_ld16(lane_base + (uint32_t)(2 * Npad + t0), Co);
-                tmem_ld16(lane_base + (uint32_t)(3 * Npad + t0), So);
-            } else {
-                tmem_ld16(lane_base + (uint32_t)(0 * Npad + t0), Ce);
-                tmem_ld16(lane_base + (uint32_t)(1 * Npad + t0), Co);
 #pragma unroll
-                for (int i = 0; i < 16; ++i) Se[i] = So[i] = 0.f;
-            }
-            float* sg = stg + cg * (4 * kRows * 16);
+    for (int hrow = 0; hrow < 2; ++hrow) {
+        const int row = 16 * (wtid >> 5) + (lane >> 2) + 8 * hrow;
+        if (row >= rows || F0 + row >= p.n_total) continue;
+        float hw = 1.f;
+        if (MODE == B2D_IR_MAG_DYNAMIC) hw = p.hw_num / (p.f0[F0 + row] + 1e-3f);
+        float* dst = p.ir + (size_t)(F0 + row) * L;
 #pragma unroll
-            for (int i = 0; i < 16; ++i) {
-                const int tl = t0 + i, th = M - 1 - tl;
-                const float Cl = Ce[i] + Co[i], Ch = Ce[i] - Co[i];
-                const float Sl = Se[i] + So[i], Sh = So[i] - Se[i];
-                const int col = i ^ (row & 15);                    // swizzle: rows are 64 B apart
-                // taps: g0 -> M-1+tl, g1 -> M-1-tl, g2 -> M-1+th, g3 -> M-1-th = tl
-                sg[(0 * kRows + row) * 16 + col] = (Cl - Sl) * ((tl < Nt && tl <= M - 2) ? window(M - 1 + tl) : 0.f);
-                sg[(1 * kRows + row) * 16 + col] = (Cl + Sl) * ((tl < Nt && tl >= 1) ? window(M - 1 - tl) : 0.f);
-                sg[(2 * kRows + row) * 16 + col] = (Ch - Sh) * ((tl < Nt && th != tl && th <= M - 2) ? window(M - 1 + th) : 0.f);
-                sg[(3 * kRows + row) * 16 + col] = (Ch + Sh) * ((tl < Nt && th != tl && th >= 1) ? window(tl) : 0.f);
-            }
-        }
-        __syncthreads();
-        // coalesced write-out: a half-warp owns rows hw, hw + 32, ...; its 16 lanes are the 16 columns of a (column
-        // block, tap group) segment = 64 contiguous bytes of an IR row.  Everything that depends only on the column is
-        // hoisted out of the row loop (the first version decoded a flat segment index per element: ~25 instructions per
-        // 4-byte store, 44 M warp instructions per launch, 80 % of the kernel).
-        {
-            const int hw = tid >> 4, i = tid & 15;
-            const int swz = i ^ (hw & 15);                               // rows advance by 32: r2 & 15 == hw & 15
+        for (int j = 0; j < JT; ++j) {
+            const int t = wg + 4 * j;
+            if (t >= NT16) continue;
 #pragma unroll
-            for (int c2 = 0; c2 < 4; ++c2) {
-                const int blk2 = rnd * 4 + c2;
-                const int tl = blk2 * 16 + i, th = M - 1 - tl;
-                if (blk2 < nblk && tl < Nt) {
-                    const int idx4[4] = {M - 1 + tl, M - 1 - tl, M - 1 + th, tl};
-                    const bool ok4[4] = {tl <= M - 2, tl >= 1, th != tl && th <= M - 2, th != tl && th >= 1};
+            for (int s = 0; s < 2; ++s)
 #pragma unroll
-                    for (int gI = 0; gI < 4; ++gI) {
-                        if (!ok4[gI]) continue;
-                        const float* src = stg + (c2 * 4 + gI) * (kRows * 16) + swz;
-                        float* dst = p.ir + (size_t)F0 * L + idx4[gI];
-#pragma unroll
-                        for (int r2 = hw; r2 < rows; r2 += 32)
-                            if (F0 + r2 < p.n_total) dst[(size_t)r2 * L] = src[r2 * 16];
-                    }
+                for (int e = 0; e < 2; ++e) {
+                    const int i = 4 * s + 2 * hrow + e;
+                    const int tl = 16 * t + 8 * s + 2 * (lane & 3) + e, th = M - 1 - tl;
+                    if (tl >= Nt) continue;
+                    const float Ce = acc[0][j][i], Co = acc[kAllpass ? 2 : 1][j][i];
+                    const float Se = kAllpass ? acc[1][j][i] : 0.f, So = kAllpass ? acc[3][j][i] : 0.f;
+                    const float Cl = Ce + Co, Ch = Ce - Co;
+                    const float Sl = Se + So, Sh = So - Se;
+                    // taps: M-1+tl, M-1-tl, M-1+th, M-1-th = tl
+                    if (tl <= M - 2) dst[M - 1 + tl] = (Cl - Sl) * window(M - 1 + tl, hw);
+                    if (tl >= 1) dst[M - 1 - tl] = (Cl + Sl) * window(M - 1 - tl, hw);
+                    if (th != tl && th <= M - 2) dst[M - 1 + th] = (Ch - Sh) * window(M - 1 + th, hw);
+                    if (th != tl && th >= 1) dst[tl] = (Ch + Sh) * window(tl, hw);
                 }
-            }
         }
-        __syncthreads();
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "n"(kTmemCols) : "memory");
+}
+
+size_t tc_smem_bytes(int nacc, int M) {
+    const int Npad = b2d::tc_npad(M), L = 2 * (M - 1);
+    return (size_t)2 * (nacc * 2 * kABlock + nacc * 2 * Npad * 8) * 4 + (size_t)((L + 3) & ~3) * 4 + (size_t)kRows * 17 * 4;
 }
 
 // table image: [chunk][cosE hi, cosE lo, sinE hi, sinE lo, cosO hi, cosO lo, sinO hi, sinO lo][2 k-chunks][Npad][4]
@@ -367,17 +346,13 @@ __global__ void dft_image_kernel(int M, float* __restrict__ img) {
 }
 
 template <int MODE>
-int launch_tc(const IrTcParams& p, cudaStream_t st) {
+int launch_tc(const IrTcParams& p, int rows, cudaStream_t st) {
     constexpr int NACC = (MODE == B2D_IR_ALLPASS) ? 4 : 2;
-    const int Npad = b2d::tc_npad(p.M), L = 2 * (p.M - 1);
-    const size_t stage = (size_t)(NACC * 2 * kABlock + NACC * 2 * Npad * 8) * 4;
-    if (2 * stage > (size_t)kStagingFloats * 4) return b2d::fail(B2D_ERR_UNSUPPORTED, "ir_build_tc: stages do not fit");
-    const size_t smem = (size_t)kStagingFloats * 4 + (size_t)((L + 3) & ~3) * 4 + (size_t)kRows * 17 * 4 + 128;
-    auto kern = p.rows == 32 ? ir_build_tc_kernel<MODE, 32> : p.rows == 64 ? ir_build_tc_kernel<MODE, 64>
-                                                                         : ir_build_tc_kernel<MODE, 128>;
+    const size_t smem = tc_smem_bytes(NACC, p.M);
+    auto kern = rows == 32 ? ir_build_tc_kernel<MODE, 32> : ir_build_tc_kernel<MODE, 64>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return b2d::fail((int)e, "ir_build_tc: smem attr (%zu B): %s", smem, cudaGetErrorString(e));
-    kern<<<(p.n_total + p.rows - 1) / p.rows, kThreads, smem, st>>>(p);
+    kern<<<(p.n_total + rows - 1) / rows, kThreads, smem, st>>>(p);
     return b2d::check_launch("ir_build_tc");
 }
 
@@ -388,17 +363,16 @@ namespace b2d {
 size_t tc_image_floats_host(int M) { return tc_image_floats(M); }
 
 int dft_image_launch(int M, float* img, cudaStream_t st) {
-    dft_image_kernel<<<148 * 4, 256, 0, st>>>(M, img);
+    dft_image_kernel<<<num_sms() * 4, 256, 0, st>>>(M, img);
     return check_launch("dft_image");
 }
 
-// tensor-core IR build is available when the accumulators fit TMEM and the stages fit shared memory
+// tensor-core IR build is available when the accumulators fit their 64 registers per thread and the two stages fit
+// shared memory (227 KB per block on H100)
 bool ir_tc_supported(int mode, int M) {
     const int nacc = (mode == B2D_IR_ALLPASS) ? 4 : 2;
-    const int Npad = tc_npad(M);
-    if (nacc * Npad > 512 || Npad > 256) return false;
-    const size_t stage = (size_t)(nacc * 2 * kABlock + nacc * 2 * Npad * 8) * 4;
-    return 2 * stage <= (size_t)kStagingFloats * 4 && (size_t)kStagingFloats * 4 + (size_t)2 * M * 4 + kRows * 17 * 4 + 256 <= 220 * 1024;
+    if (nacc * tc_npad(M) > 512) return false;
+    return tc_smem_bytes(nacc, M) <= 227 * 1024;
 }
 
 int ir_build_tc_launch(const float* c, int64_t ctrl_stride, int mode, const float* f0, const float* image, int B,
@@ -406,14 +380,12 @@ int ir_build_tc_launch(const float* c, int64_t ctrl_stride, int mode, const floa
     IrTcParams p;
     p.c = c; p.ctrl_stride = ctrl_stride; p.f0 = f0; p.image = image;
     p.n_total = B * nF; p.M = M; p.hw_num = 1.5f * (float)sr; p.ir = ir;
-    // fewest rows per CTA that still run as a single wave of one CTA per SM; 128 once the grid fills the GPU anyway
-    p.rows = 128;
-    for (int r = 32; r < 128; r <<= 1)
-        if ((p.n_total + r - 1) / r <= 148) { p.rows = r; break; }
+    // 32 frames per CTA when that still runs as a single wave of one CTA per SM; 64 once the grid fills the GPU anyway
+    const int rows = (p.n_total + 31) / 32 <= num_sms() ? 32 : 64;
     switch (mode) {
-        case B2D_IR_ALLPASS: return launch_tc<B2D_IR_ALLPASS>(p, st);
-        case B2D_IR_MAG_HANN: return launch_tc<B2D_IR_MAG_HANN>(p, st);
-        default: return launch_tc<B2D_IR_MAG_DYNAMIC>(p, st);
+        case B2D_IR_ALLPASS: return launch_tc<B2D_IR_ALLPASS>(p, rows, st);
+        case B2D_IR_MAG_HANN: return launch_tc<B2D_IR_MAG_HANN>(p, rows, st);
+        default: return launch_tc<B2D_IR_MAG_DYNAMIC>(p, rows, st);
     }
 }
 

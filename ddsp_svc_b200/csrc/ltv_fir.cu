@@ -251,10 +251,7 @@ __global__ void __launch_bounds__(MAXT, MINB) ltv_fir_kernel(FirParams p) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// Variant with 16 outputs per thread and packed FP32x2 FMAs (fma.rn.f32x2, sm_100 FFMA2).
-// The scalar kernel above sits at ~62 % of the FP32 peak: LDS.128 lands window / table values in
-// both register banks, so many 3-source FFMAs have all operands in one bank (a register-only
-// replica of its inner step reaches 73 %, the FFMA2 form 83 %, scratch/fir_pattern.cu).  Here the
+// Variant with 16 outputs per thread and register-pair FMAs (ffma2: two FFMAs on Hopper).  Here the
 // accumulators are (a1[r], a2[r]) pairs, the table entries (G, E) pairs straight from LDS.128, and
 // each input value is duplicated into a pair once per step; 16 outputs per thread halve the shared
 // loads per FMA.  One warp per filter (32 threads x 16 outputs = P = 512), window of 5 chunks
@@ -263,7 +260,11 @@ __global__ void __launch_bounds__(MAXT, MINB) ltv_fir_kernel(FirParams p) {
 typedef unsigned long long u64;
 __device__ __forceinline__ u64 pack2(float lo, float hi) { u64 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
 __device__ __forceinline__ void unpack2(u64 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ void ffma2(u64& d, u64 a, u64 b) { asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(d) : "l"(a), "l"(b)); }
+__device__ __forceinline__ void ffma2(u64& d, u64 a, u64 b) {   // lane-wise: two FFMAs on Hopper
+    float a0, a1, b0, b1, d0, d1;
+    unpack2(a, a0, a1); unpack2(b, b0, b1); unpack2(d, d0, d1);
+    d = pack2(fmaf(a0, b0, d0), fmaf(a1, b1, d1));
+}
 
 __device__ __forceinline__ int swz4(int c) { return c ^ ((c >> 3) & 3); }
 
@@ -492,15 +493,14 @@ int ltv_fir_fft_launch(const float* x1, const float* ir1, int taps1, float* y1, 
 
 // 0 = auto (FFT-domain kernel where it applies, else CUDA cores), 1 = CUDA-core kernel, 2 = tensor-core kernel
 // (block size 512 only), 4 = FFT-domain kernel where it applies (block size 512, <= 1024 taps; other shapes fall
-// through to the CUDA-core kernel).  Measured on B200 (B = 32 x 10 s, two 510-tap filters): FFT domain 0.33 ms, CUDA-core
-// direct form 1.18 ms, tcgen05 4.20 ms (with N = 8 columns every MMA re-reads its 4 KB Hankel operand from shared memory
-// for 16 kflop: operand-bandwidth bound, ~56 cycles per 128x8x8 MMA).
+// through to the CUDA-core kernel).   The tensor-core kernel is
+// operand-bandwidth bound: with N = 8 columns every MMA re-reads its Hankel operand from shared memory.
 static std::atomic<int> g_fir_impl{0};
-// CUDA-core variant: 0 = auto (16 outputs/thread + FFMA2 when the block size is a multiple of 512), 1 = 8 outputs/thread scalar
+// CUDA-core variant: 0 = auto (16 outputs/thread + register pairs when the block size is a multiple of 512), 1 = 8 outputs/thread scalar
 static std::atomic<int> g_fir_variant{0};
 
-// what "auto" means: the FFT-domain kernel wherever it applies (block size 512, <= 1024 taps; measured on B200:
-// 0.372 ms against 1.18 ms for Sins' two 510-tap filters, B = 32 x 10 s), the CUDA-core kernel otherwise.
+// what "auto" means: the FFT-domain kernel wherever it applies (block size 512, <= 1024 taps), the CUDA-core kernel
+// otherwise.
 // B2D_FIR_AUTO=cuda in the environment restores the direct form as the automatic choice (A/B runs of whole programs).
 static int fir_auto_impl() {
     static const int v = [] {
@@ -578,7 +578,7 @@ int ltv_fir_launch(const float* x1, const float* ir1, int taps1, float* y1, cons
         kern<<<dim3(ntiles, B), threads, smem, st>>>(p);
         return check_launch("ltv_fir");
     };
-    if (g_fir_variant.load(std::memory_order_relaxed) != 1 && P % 512 == 0) {            // 16 outputs/thread, FFMA2 (one warp per filter at P = 512)
+    if (g_fir_variant.load(std::memory_order_relaxed) != 1 && P % 512 == 0) {            // 16 outputs/thread, register pairs (one warp per filter at P = 512)
         const int threads16 = njobs * (P / 16);
         const size_t smem = (size_t)(njobs * (6 * P + 8 + P + (P >> 4) + 8) + P) * sizeof(float);
         auto go16 = [&](auto kern) -> int {

@@ -22,8 +22,7 @@
 // instructions.  A CTA owns G hops (G even) of one utterance and processes the G+2 input hops that reach them (they
 // form whole pairs); white-noise input (x2 == nullptr) is the same Philox stream as in the direct-form kernels.
 //
-// Measured on B200 (Sins, B = 32 x 10 s, two 510-tap filters): 0.372 ms against 1.18 ms for the direct form -> this is
-// the automatic dispatch for block size 512 and <= 1024 taps (ltv_fir.cu).  Logic additionally pinned on the CPU by
+// This is the automatic dispatch for block size 512 and <= 1024 taps (ltv_fir.cu).  Logic additionally pinned on the CPU by
 // the host emulation in tests/emu/ (tests/test_emu_ltv_fir_fft.py, race check in tests/test_emu_tsan.py).
 #ifndef B2D_HOST_EMU
 #include "b2d_common.cuh"
@@ -86,7 +85,7 @@ __device__ __forceinline__ void split2(float2 zk, float2 zm, float2& A, float2& 
     C = make_float2(0.5f * (zk.y + zm.y), 0.5f * (zm.x - zk.x));
 }
 
-// PK: complex additions as packed f32x2 instructions (fft_regs.cuh Ar<true>): same results, fewer issue slots
+// PK: the "packed" complex-addition policy (fft_regs.cuh Ar<true>; scalar on Hopper)
 // NBANK: 0 = inputs from memory / Philox; 4 or 8 = job 0 is the sinusoid bank with that many bases of 16 harmonics
 // SPEC: job[j].ir holds the packed 1024-point spectra of the impulse responses instead of the taps
 template <int N, int NJ, bool PK, int NBANK = 0, bool SPEC = false>
@@ -129,8 +128,7 @@ __global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ?
         }
     };
     // Global loads of a hop pair (input samples read from memory, impulse-response taps), issued ONE ITERATION AHEAD into
-    // registers: they are in flight during the previous pair's transforms instead of stalling the head of the iteration
-    // (ncu, round 2: 18 % of the stall samples were long-scoreboard waits on exactly these loads).
+    // registers: they are in flight during the previous pair's transforms instead of stalling the head of the iteration.
     constexpr int kTau = kN / 2 / kThreads;
     struct Prefetch { float4 xa[NJ], xb[NJ]; float ha[NJ][kTau], hb[NJ][kTau]; };
     auto fetch = [&](int g, Prefetch& q) {
@@ -510,7 +508,7 @@ int ltv_fir_fft_launch(const float* x1, const float* ir1, int taps1, float* y1, 
     // caller, one chunk of the host pipeline -- latency-bound; halve G (25 % / 50 % / 100 % recomputation at 8 / 4 / 2)
     // until there are at least two CTAs per SM.
     int G = 32;
-    while (G > 2 && (long long)B * ((nF + G - 1) / G) < 148LL * 2) G >>= 1;
+    while (G > 2 && (long long)B * ((nF + G - 1) / G) < (long long)b2d::num_sms() * 2) G >>= 1;
     p.G = G;
     const dim3 grid((unsigned)((nF + p.G - 1) / p.G), B);
     const int tmax = njobs == 2 ? (taps1 > taps2 ? taps1 : taps2) : taps1;
@@ -543,7 +541,7 @@ int sins_fused_launch(const float* f0, const double* frame_phase, const float* c
     p.bank.H = H; p.bank.inv_sr = 1.0 / sampling_rate; p.bank.nyquist = (float)(sampling_rate / 2.0);
     p.bank.round_fp32 = round_fp32;
     int G = 32;
-    while (G > 2 && (long long)B * ((nF + G - 1) / G) < 148LL * 2) G >>= 1;
+    while (G > 2 && (long long)B * ((nF + G - 1) / G) < (long long)b2d::num_sms() * 2) G >>= 1;
     p.G = G;
     const dim3 grid((unsigned)((nF + p.G - 1) / p.G), B);
     const bool pk = g_fft_packed.load(std::memory_order_relaxed) != 0;
@@ -584,7 +582,7 @@ int ltv_fir_fft_spec_launch(const float* x1, const float* spec1, int taps1, floa
     p.job[1] = {x2, spec2, y2, taps2};
     p.addend = nullptr; p.mix = mix; p.seed = seed; p.utt_off = utt_off; p.nF = nF;
     int G = 32;
-    while (G > 2 && (long long)B * ((nF + G - 1) / G) < 148LL * 2) G >>= 1;
+    while (G > 2 && (long long)B * ((nF + G - 1) / G) < (long long)b2d::num_sms() * 2) G >>= 1;
     p.G = G;
     const dim3 grid((unsigned)((nF + p.G - 1) / p.G), B);
     return g_fft_packed.load(std::memory_order_relaxed) ? launch_fir_fft_as<1024, 2, true, 0, true>(p, grid, st)

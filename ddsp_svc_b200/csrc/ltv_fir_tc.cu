@@ -1,5 +1,5 @@
-// K4-TC: the linear time-varying FIR of ltv_fir.cu on the 5th-generation tensor cores
-// (tcgen05.mma kind::tf32, accumulators in TMEM), 3xTF32 split for fp32-level accuracy.
+// K4-TC: the linear time-varying FIR of ltv_fir.cu on the Hopper tensor cores (wgmma tf32,
+// accumulators in registers), 3xTF32 split for fp32-level accuracy.
 //
 // Same tiling and algebra as ltv_fir.cu: a tile is P = 512 consecutive outputs
 // n = f P - (L/2+1) + i; per tap segment the inputs are the 2P samples xs[q], q = m - (gP - P), and
@@ -10,29 +10,27 @@
 //     Y = Hankel(x+) . Toep(A tables) + Hankel(x-) . Toep(B tables)
 // with  Hankel(x)[r, c] = x[4 r + c]           (128 rows r, i = 4 r + j)
 //       Toep(T)[c, (t, j)] = T_t[P-1+j-c]      (t in {G,E}, j = 0..3  ->  N = 8 columns)
-// A Hankel matrix with row shift 4 is exactly a K-major, no-swizzle UMMA operand VIEW of the linear
+// A Hankel matrix with row shift 4 is exactly a K-major, no-swizzle wgmma operand VIEW of the linear
 // signal in shared memory (rows 16 B apart, K-chunks 16 B apart: SBO = 128 B, LBO = 16 B -- core
-// matrices overlap, which the hardware accepts; verified on B200 by scratch/umma_test.cu), so the
-// 512 x 515 operand is never materialised.  The small Toeplitz operand (8 x 520) is.
+// matrices overlap; the descriptor only describes addresses), so the 512 x 515 operand is never
+// materialised.  The small Toeplitz operand (8 x 520) is.
 //
 // fp32 accuracy: the tensor core truncates fp32 inputs to tf32, so every operand is split with
 // round-to-nearest into hi + lo (lo rounded to tf32 as well) and each product is accumulated as
-// hi*hi + lo*hi + hi*lo in the fp32 TMEM accumulator (3xTF32): relative error ~2^-21 per term,
+// hi*hi + lo*hi + hi*lo in the fp32 accumulator (3xTF32): relative error ~2^-21 per term,
 // i.e. the same level as an fp32 FMA chain over 510 taps.
 //
 // STATUS: correct (parity tests run it), NOT the default.  Work per (tile, filter, segment) is
-// 2 regions x 3 split products x 65 K-steps = 390 MMAs of 128x8x8.  The tensor-pipe floor for that
-// shape is 4 cycles, but each MMA also fetches its 128 x 32 B Hankel operand from shared memory,
-// and with only N = 8 columns to amortise it the kernel is operand-bandwidth bound: measured
-// 4.20 ms for B=32 x 10 s x two filters (~56 cycles per MMA) against 1.26 ms for the CUDA-core
-// kernel (ltv_fir.cu).  A time-varying FIR is matrix-VECTOR shaped (every (utterance, frame) has its
-// own input and its own impulse response), so there is no second large dimension to batch along N.
-// Also note the fp32 TMEM accumulator truncates: ~5e-6 relative error after 390 accumulation steps.
-// Kept as a tested alternative (b2d_set_fir_impl(2)) and as the tcgen05 building block for the
-// GEMM-shaped impulse-response construction.  One CTA per (tile, filter): 128 threads build the operands (tables,
-// hi/lo splits, Toeplitz matrices: ~91 KB shared memory -> 2 CTAs per SM, so one CTA's operand build
-// overlaps the other's MMAs), thread 0 issues the MMAs, tcgen05.commit signals an mbarrier, the four
-// warps read their 32 TMEM lanes (tcgen05.ld), apply the (i-1)/P recombination and store float4s.
+// 2 regions x 3 split products x 65 K-steps x 2 row halves = 780 wgmmas of 64x8x8, and each also
+// fetches its 64 x 32 B Hankel operand from shared memory: with only N = 8 columns to amortise it the
+// kernel is operand-bandwidth bound.  A time-varying FIR is matrix-VECTOR shaped (every (utterance,
+// frame) has its own input and its own impulse response), so there is no second large dimension to
+// batch along N.  Also note the fp32 tensor-core accumulator truncates: ~5e-6 relative error after 390
+// accumulation steps.  Kept as a tested alternative (b2d_set_fir_impl(2)).  One CTA (one warpgroup) per
+// (tile, filter): its 128 threads build the operands (tables, hi/lo splits, Toeplitz matrices: ~91 KB
+// shared memory -> 2 CTAs per SM, so one CTA's operand build overlaps the other's MMAs), issue the
+// wgmmas for rows 0..63 and 64..127 of the tile, stage the accumulators through shared memory, apply
+// the (i-1)/P recombination and store float4s.
 // `mix` (signal = harmonic + noise) is formed with red.global.add.v4.f32 into a zeroed buffer; with
 // exactly two addends the result does not depend on arrival order.
 #include "b2d_common.cuh"
@@ -71,24 +69,27 @@ __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
     hi = __uint_as_float(tf32_rn_bits(x));
     lo = __uint_as_float(tf32_rn_bits(x - hi));
 }
+// wgmma shared-memory descriptor, K-major, layout type 0 = no swizzle
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFF);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;   // descriptor version 1 (sm_100); layout type 0 = no swizzle
     return d;
 }
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t acc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n"
-                 ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(acc) : "memory");
+// D[64 x 8] += A[64 x 8] . B[8 x 8], both tf32 from shared memory
+__device__ __forceinline__ void wgmma_tf32_m64n8k8(float (&d)[4], uint64_t da, uint64_t db) {
+    asm volatile("wgmma.mma_async.sync.aligned.m64n8k8.f32.tf32.tf32 {%0, %1, %2, %3}, %4, %5, 1, 1, 1;\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "l"(da), "l"(db));
 }
+__device__ __forceinline__ void fence_reg(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 __device__ __forceinline__ void red_add_v4(float* p, float4 v) {
     asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
 
 // shared memory: xs[4][kXLen] (x+hi, x+lo, x-hi, x-lo) | bm[4][kBmat] (A hi, A lo, B hi, B lo) | tab[4][kP]
+// (tab doubles as the [128][8] accumulator staging of the epilogue)
 constexpr size_t kSmem = (size_t)(4 * kXLen + 4 * kBmat + 4 * kP) * sizeof(float) + 64;
 
 __global__ void __launch_bounds__(kThreads, 2) ltv_fir_tc_kernel(TcParams p) {
@@ -96,10 +97,8 @@ __global__ void __launch_bounds__(kThreads, 2) ltv_fir_tc_kernel(TcParams p) {
     float* xs = reinterpret_cast<float*>(smem_raw);     // 4 arrays
     float* bm = xs + 4 * kXLen;                         // 4 Toeplitz operands
     float* tab = bm + 4 * kBmat;                        // GA, EA, GB, EB  [kP] each
-    __shared__ __align__(8) uint64_t bar;
-    __shared__ uint32_t tmem_base_s;
 
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int f = blockIdx.x, b = blockIdx.y, jobi = blockIdx.z;
     TcJob jb;
     jb.x = jobi ? p.job[1].x : p.job[0].x;
@@ -112,33 +111,20 @@ __global__ void __launch_bounds__(kThreads, 2) ltv_fir_tc_kernel(TcParams p) {
     const float* irb = jb.ir + (size_t)b * nF * L;
     const float invP = 1.0f / (float)kP;
 
-    if (tid == 0) {
-        b2d::mbar_init(&bar, 1);
-        b2d::fence_mbar_init();
-    }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 32;" ::"r"(b2d::smem_u32(&tmem_base_s)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     // zero the Hankel sources' tails once (q >= 2P are never written)
     for (int i = tid; i < 4 * kXLen; i += kThreads) xs[i] = 0.f;
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_d = tmem_base_s;
-    // instruction descriptor: D = F32, A = B = TF32, both K-major, N = 8, M = 128
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | (1u << 17) | (8u << 24);
 
-    uint32_t phase = 0;
+    float acc[2][4];                                   // rows 0..63 and 64..127 of the tile, N = 8
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) acc[h][i] = 0.f;
     bool any = false;
     for (int s = 0; s < NS; ++s) {
         const int g = f - s;
         if (g < 0 || g > nF) continue;                 // no inputs inside [0,T) for this segment
-        if (any) {                                     // previous segment's MMAs must be done before operands are rebuilt
-            b2d::mbar_wait(&bar, phase);
-            phase ^= 1;
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        }
+        if (any) __syncthreads();                      // previous segment's MMAs are done (wait_group): operands may be rebuilt
         // ---- input tile m in [gP-P, gP+P): split into x+ / x- and hi / lo ----
         const int mbase = g * kP - kP;
         for (int c = tid; c < (kP >> 1); c += kThreads) {
@@ -196,8 +182,12 @@ __global__ void __launch_bounds__(kThreads, 2) ltv_fir_tc_kernel(TcParams p) {
         b2d::fence_proxy_async();                      // generic-proxy writes -> visible to the tensor core
         __syncthreads();
         // ---- MMAs: regions (x+, A tables), (x-, B tables); products hi*hi, lo*hi, hi*lo ----
-        if (tid == 0) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) fence_reg(acc[h][i]);
+        asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+        {
             const uint32_t xs_a = b2d::smem_u32(xs), bm_a = b2d::smem_u32(bm);
 #pragma unroll 1
             for (int R = 0; R < 2; ++R) {
@@ -205,38 +195,50 @@ __global__ void __launch_bounds__(kThreads, 2) ltv_fir_tc_kernel(TcParams p) {
                 for (int pr = 0; pr < 3; ++pr) {
                     const int xi = 2 * R + (pr == 1 ? 1 : 0);          // x hi, lo, hi
                     const int bi = 2 * R + (pr == 2 ? 1 : 0);          // T hi, hi, lo
-                    // Hankel view: rows 16 B apart (8-row blocks 128 B), K chunks 16 B apart; K-step = 32 B
+                    // Hankel view: rows 16 B apart (8-row blocks 128 B), K chunks 16 B apart; K-step = 32 B;
+                    // rows 64..127 start 64 x 16 B later
                     uint64_t da = make_desc(xs_a + xi * kXLen * 4, 16, 128);
                     // Toeplitz operand: [chunk][8 rows][4]: chunks 128 B apart; K-step = 2 chunks = 256 B
                     uint64_t db = make_desc(bm_a + bi * kBmat * 4, 128, 128);
-#pragma unroll 1
+#pragma unroll 5
                     for (int ks = 0; ks < kSteps; ++ks) {
-                        mma_tf32(tmem_d, da, db, idesc, (any || R || pr || ks) ? 1u : 0u);
+                        wgmma_tf32_m64n8k8(acc[0], da, db);
+                        wgmma_tf32_m64n8k8(acc[1], da + 64, db);
                         da += 2;     // +32 B  (start address field is in 16-byte units)
                         db += 16;    // +256 B
                     }
                 }
             }
-            asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(b2d::smem_u32(&bar)) : "memory");
         }
+        asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+        asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) fence_reg(acc[h][i]);
         any = true;
     }
 
-    // ---- epilogue: TMEM -> registers -> y = acc1 + ((i-1)/P) acc2 ----
+    // ---- epilogue: registers -> [128][8] staging -> y = acc1 + ((i-1)/P) acc2 ----
+    // accumulator fragment: acc[h][i] is row 64 h + 16 warp + lane / 4 + 8 (i >> 1), column 2 (lane % 4) + (i & 1)
     float4 yv = make_float4(0.f, 0.f, 0.f, 0.f);
     if (any) {
-        b2d::mbar_wait(&bar, phase);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        uint32_t v[8];
-        const uint32_t taddr = tmem_d + ((uint32_t)(warp * 32) << 16);
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]) : "r"(taddr));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        __syncthreads();                               // every thread is done with tab
+        float* stg = tab;
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+                stg[(64 * h + 16 * warp + (lane >> 2) + 8 * (i >> 1)) * 8 + 2 * (lane & 3) + (i & 1)] = acc[h][i];
+        __syncthreads();
+        float v[8];
+#pragma unroll
+        for (int c = 0; c < 8; ++c) v[c] = stg[tid * 8 + c];
         const float i0m1 = (float)(4 * tid - 1);
-        yv.x = fmaf((i0m1 + 0.f) * invP, __uint_as_float(v[4]), __uint_as_float(v[0]));
-        yv.y = fmaf((i0m1 + 1.f) * invP, __uint_as_float(v[5]), __uint_as_float(v[1]));
-        yv.z = fmaf((i0m1 + 2.f) * invP, __uint_as_float(v[6]), __uint_as_float(v[2]));
-        yv.w = fmaf((i0m1 + 3.f) * invP, __uint_as_float(v[7]), __uint_as_float(v[3]));
+        yv.x = fmaf((i0m1 + 0.f) * invP, v[4], v[0]);
+        yv.y = fmaf((i0m1 + 1.f) * invP, v[5], v[1]);
+        yv.z = fmaf((i0m1 + 2.f) * invP, v[6], v[2]);
+        yv.w = fmaf((i0m1 + 3.f) * invP, v[7], v[3]);
     }
     const int n0 = f * kP - Mh + 4 * tid;
     const bool vec_ok = ((n0 & 3) == 0) && n0 >= 0 && (n0 + 4) <= T;
@@ -270,9 +272,6 @@ __global__ void __launch_bounds__(kThreads, 2) ltv_fir_tc_kernel(TcParams p) {
             }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 32;" ::"r"(tmem_d) : "memory");
 }
 
 }  // namespace

@@ -183,9 +183,8 @@ __global__ void __launch_bounds__(kTile) sinegen_kernel(SgParams p) {
 //     assembled with integer ops, rint() by the add-magic-constant trick: the SFU pipe only sees 4 MUFU per
 //     normal pair and one per sine;
 //   * frame lookup, f0/sr, rand_ini and the Linear weights once per thread instead of once per sample;
-//   * MODE 1 only: the fp32 chain of two samples at a time in f32x2 instructions.  NOT bit-compatible with the scalar
-//     chain: ptxas fuses mul.rn.f32x2 + add.rn.f32x2 into one FFMA2 (SASS: "FFMA2 R18, R46.F32x2, 2, R67.F32"), so
-//     theta = rad*(h+1) + rho is rounded once instead of twice (max output error 3e-6 vs 3e-8) -- kept as an option;
+//   * MODE 1 only: the fp32 chain of two samples at a time as register pairs (mul2 / add2 / fma2 below, scalar
+//     instructions on Hopper) -- kept as an option;
 //   * FUSED (SourceModuleHnNSF): no shared-memory tile at all, one 128-bit store of 4 merged samples.
 constexpr int kQ = 4;
 constexpr int kThreads4 = 128;
@@ -195,9 +194,18 @@ typedef unsigned long long u64;
 __device__ __forceinline__ u64 pack2(float lo, float hi) { u64 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
 __device__ __forceinline__ void unpack2(u64 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
 __device__ __forceinline__ u64 dup2(float x) { return pack2(x, x); }
-__device__ __forceinline__ u64 mul2(u64 a, u64 b) { u64 d; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ u64 add2(u64 a, u64 b) { u64 d; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) { u64 d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
+// lane-wise pair arithmetic: Hopper has no f32x2 instructions, so each is two scalar ones (the explicit _rn
+// intrinsics are never contracted into an FMA)
+__device__ __forceinline__ u64 mul2(u64 a, u64 b) {
+    float a0, a1, b0, b1; unpack2(a, a0, a1); unpack2(b, b0, b1); return pack2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
+}
+__device__ __forceinline__ u64 add2(u64 a, u64 b) {
+    float a0, a1, b0, b1; unpack2(a, a0, a1); unpack2(b, b0, b1); return pack2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
+}
+__device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
+    float a0, a1, b0, b1, c0, c1; unpack2(a, a0, a1); unpack2(b, b0, b1); unpack2(c, c0, c1);
+    return pack2(fmaf(a0, b0, c0), fmaf(a1, b1, c1));
+}
 __device__ __forceinline__ float lg2_ftz(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float sin_ftz(float x) { float y; asm("sin.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float cos_ftz(float x) { float y; asm("cos.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
@@ -233,10 +241,7 @@ __device__ __forceinline__ float sin_turns(float theta) {
     return __sinf(r);
 }
 
-// MODE 0: scalar arithmetic (default); MODE 1: packed f32x2 arithmetic.  80 registers, 6 CTAs per SM.
-// Measured dead ends (B200, 64 x 10 s x 9): compiling for 8 CTAs/SM (64 registers) 0.357 vs 0.345 ms -- the
-// kernel is bound by the issue slots / pipe mix, not by latency; a streaming variant (one Philox block -> 4
-// outputs -> one 128-bit shared store, 48 registers) 0.42 ms, 320 M vs 248 M warp instructions.
+// MODE 0: scalar arithmetic (default); MODE 1: register-pair arithmetic.
 // ROUNDS: Philox rounds of the in-kernel noise (10 standard; 7 = `v2r7`, see b2d_common.cuh)
 template <int DIM, bool FUSED, int MODE, int ROUNDS = 10>
 __global__ void __launch_bounds__(kThreads4, 6) sinegen4_kernel(SgParams p) {
@@ -396,7 +401,7 @@ void launch_v2(const SgParams& p, int B, long long T, int impl, cudaStream_t st)
     }
 }
 
-std::atomic<int> g_sinegen_impl{0};   // 0 auto, 1 v1 (one sample per thread), 2 v2 scalar, 3 v2 packed f32x2, 4 v2 scalar with Philox-7 noise
+std::atomic<int> g_sinegen_impl{0};   // 0 auto, 1 v1 (one sample per thread), 2 v2 scalar, 3 v2 register pairs, 4 v2 scalar with Philox-7 noise
 
 }  // namespace
 
@@ -456,11 +461,8 @@ static int sinegen_launch(const float* f0, const float* rand_ini, const float* n
     p.seed = seed; p.utt_off = utterance_offset;
     p.lin_w = lin_w; p.lin_b = lin_b; p.merged = merged;
     const long long T = (long long)n_frames * upp;
-    // auto = the scalar 4-samples-per-thread kernel: the packed variant is ~3-5 % faster, but ptxas contracts its
-    // mul.rn.f32x2 + add.rn.f32x2 pairs into FFMA2 (one rounding instead of the reference's two), which moves the sine
-    // argument by an ulp: max error 3e-6 instead of 3e-8 against the reference (still inside the 2e-6 RMS gate)
     const int sel = g_sinegen_impl.load(std::memory_order_relaxed);
-    // auto = four samples per thread, scalar arithmetic, Philox4x32-7 normals (round 2: 0.356 -> 0.318 ms, KS / correlation
+    // auto = four samples per thread, scalar arithmetic, Philox4x32-7 normals (KS / correlation
     // tests in tests/test_gpu_combsub_sinegen.py); 2 selects the same kernel with the standard 10 rounds
     const int impl = sel == 0 ? 4 : sel;
     if (impl >= 2 && (dim == 9 || dim == 1)) {

@@ -2,7 +2,7 @@
 //
 //   sinusoids[t] = sum_{h=1..H} sin(h * phase[t]) * ((1-j/P) A[k,h] + (j/P) A[k+1,h]),  t = kP + j
 //
-// Mapping (B200): one CTA owns a chunk of consecutive frames of ONE utterance.  The raw
+// Mapping: one CTA owns a chunk of consecutive frames of ONE utterance.  The raw
 // amplitude rows of the chunk are staged to shared memory by 1-D bulk async copies (TMA,
 // UBLKCP) tracked by an mbarrier; exp()/128 and the Nyquist mask are applied once per frame
 // there.  Lanes own consecutive samples (4 per thread -> one 128-bit coalesced store), and

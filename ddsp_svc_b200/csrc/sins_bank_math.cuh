@@ -1,10 +1,10 @@
 // Arithmetic of the additive sinusoid bank shared by sins_bank.cu (stand-alone kernel) and ltv_fir_fft.cu (bank fused
-// into the FFT-domain FIR kernel): harmonic factoring h = a + 16 b, packed FFMA2 accumulation.  See sins_bank.cu for the
+// into the FFT-domain FIR kernel): harmonic factoring h = a + 16 b, paired (register-pair) accumulation.  See sins_bank.cu for the
 // derivation; reference ddsp/vocoder.py:580,585-594.
 #pragma once
 #include "b2d_common.cuh"
 
-// 1 (default since round 2: bank 0.307 -> 0.273 ms, parity unchanged): even anchors by double-angle chains (halves the SFU
+// 1 (default): even anchors by double-angle chains (halves the SFU
 // work of the anchors); 0: every anchor by __sincosf (round-1 code)
 #ifndef B2D_BANK_DOUBLE_ANGLE
 #define B2D_BANK_DOUBLE_ANGLE 1
@@ -38,12 +38,16 @@ __device__ __forceinline__ int slot_of(int hh) {
 typedef unsigned long long u64;
 __device__ __forceinline__ u64 pack2(float lo, float hi) { u64 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
 __device__ __forceinline__ void unpack2(u64 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ u64 ffma2(u64 a, u64 b, u64 c) { u64 d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
+// lane-wise fma of two register pairs (Hopper has no packed FP32 FMA: two FFMAs, same roundings)
+__device__ __forceinline__ u64 ffma2(u64 a, u64 b, u64 c) {
+    float a0, a1, b0, b1, c0, c1;
+    unpack2(a, a0, a1); unpack2(b, b0, b1); unpack2(c, c0, c1);
+    return pack2(fmaf(a0, b0, c0), fmaf(a1, b1, c1));
+}
 
 // One group of (up to) 128 harmonics for 4 samples.  NB = bases actually present (1..8).
-// Packed FP32x2 FMAs (sm_100 FFMA2): the amplitudes of two neighbouring bases are interpolated by
-// one instruction, and (P_b, Q_b) += (sin, cos) * amp is one instruction, so a harmonic costs 1.5
-// issue slots instead of 3 (the kernel is issue bound, measured 78 % issue-active).
+// The amplitudes of two neighbouring bases are interpolated as one register pair, and (P_b, Q_b) += (sin, cos) * amp
+// is one pair update.
 template <int NB, bool TRIVIAL0>
 __device__ __forceinline__ void bank_group(const float* __restrict__ arow, const float* __restrict__ drow,
                                            int group, const float (&x32)[4], const float (&phase)[4],

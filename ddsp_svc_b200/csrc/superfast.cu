@@ -7,7 +7,7 @@
 //   Y_q   = X_q exp(m_h + j pi p_h) + N_q exp(m_n + j pi p_n) / 128        (frame nF reuses nF-1)
 //   out   = iSTFT(Y) = OLA(irfft(Y_q) * win) / OLA(win^2), trimmed by n_fft/2
 //
-// Design (B200).  HBM traffic is dominated by the 4 x 1025 control values per frame (36 B per
+// Design.  HBM traffic is dominated by the 4 x 1025 control values per frame (36 B per
 // output sample); everything else stays on chip:
 //  * one CTA owns a chunk of G consecutive hops of one utterance and walks the G+3 frames that
 //    touch them in order, two frames per iteration;
@@ -212,7 +212,7 @@ constexpr size_t kSmemBytes = (size_t)2 * kPadN * sizeof(float2) + (size_t)kN * 
                               (size_t)kRingHops * kHop * sizeof(float) + (size_t)kWinLen * sizeof(float) +
                               (size_t)(15 * 16 + 256) * sizeof(float2);
 
-// PK: complex additions of the FFT butterflies as packed f32x2 instructions (fft_regs.cuh Ar<true>)
+// PK: the "packed" complex-addition policy of the FFT butterflies (fft_regs.cuh Ar<true>; scalar on Hopper)
 template <bool PK>
 __global__ void __launch_bounds__(kThreads, 3) superfast_kernel(SfParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -450,7 +450,7 @@ extern "C" int b2d_superfast_synth(const void* workspace, const float* c_harmoni
     p.nF = n_frames; p.P = block;
     // chunk length: G+3 frames are transformed for G hops; keep >= ~4 CTAs per SM when the work allows
     int G = 29;
-    while (G > 5 && (long long)B * ((n_frames + G - 1) / G) < 4 * 148) G -= 4;
+    while (G > 5 && (long long)B * ((n_frames + G - 1) / G) < 4 * b2d::num_sms()) G -= 4;
     p.G = G;
     p.seed = seed; p.utt_off = utterance_offset;
     const size_t smem = kSmemBytes;

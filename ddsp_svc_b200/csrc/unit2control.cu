@@ -194,7 +194,7 @@ extern "C" int b2d_split_tf32(const float* x, float* hi, float* lo, size_t n, vo
     const size_t n4 = n / 4;
     const int tail = (int)(n - n4 * 4);
     size_t gx = (n4 + 255) / 256;
-    if (gx > 148 * 16) gx = 148 * 16;
+    if (gx > b2d::num_sms() * 16) gx = b2d::num_sms() * 16;
     if (gx == 0) gx = 1;
     u2c_split_tf32_kernel<<<(unsigned)gx, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const float4*>(x), reinterpret_cast<float4*>(hi),
                                                                           reinterpret_cast<float4*>(lo), n4, x + n4 * 4, hi + n4 * 4,
@@ -207,7 +207,7 @@ extern "C" int b2d_u2c_embed(float* x, const float* f0, const float* phase, cons
     if (!x || !f0 || !phase || !volume || !embed_table) return b2d::fail(B2D_ERR_NULL, "u2c_embed: null pointer");
     if (B <= 0 || T <= 0 || (spk && spk_rows != 1 && spk_rows != B)) return b2d::fail(B2D_ERR_SHAPE, "u2c_embed: bad shape");
     const int n = B * T;
-    u2c_embed_kernel<<<min(n, 148 * 8), 256, 0, (cudaStream_t)stream>>>(x, f0, phase, volume, embed_table, spk, spk_rows, aug_shift, n, T);
+    u2c_embed_kernel<<<min(n, b2d::num_sms() * 8), 256, 0, (cudaStream_t)stream>>>(x, f0, phase, volume, embed_table, spk, spk_rows, aug_shift, n, T);
     return b2d::check_launch("u2c_embed");
 }
 

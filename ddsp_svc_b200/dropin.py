@@ -1,6 +1,6 @@
 """Drop-in wiring for an existing DDSP-SVC checkout.
 
-``patch_reference()`` rebinds the reference's synthesizer classes to the B200 ones so that its
+``patch_reference()`` rebinds the reference's synthesizer classes to this package's ones so that its
 unmodified entry points (main.py, flask_api.py, gui.py, enhancer.py, ...) run on the CUDA
 kernels:
 

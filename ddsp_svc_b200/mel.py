@@ -79,10 +79,10 @@ class STFT:
     def get_mel(self, y, keyshift=0, speed=1, center=False):
         """y [B, T] CUDA fp32 -> log-mel [B, n_mels, n_frames] (nvSTFT.py:73-117)."""
         if keyshift != 0 or speed != 1 or center:
-            raise NotImplementedError("the B200 mel kernel covers keyshift=0, speed=1, center=False (the inference call of "
+            raise NotImplementedError("the mel kernel covers keyshift=0, speed=1, center=False (the inference call of "
                                       "enhancer.py:113); got keyshift=%r speed=%r center=%r" % (keyshift, speed, center))
         if self.n_fft != 2048 or self.win_size != 2048 or self.n_mels > 128:
-            raise NotImplementedError("the B200 mel kernel is built for n_fft = win_size = 2048 and n_mels <= 128 "
+            raise NotImplementedError("the mel kernel is built for n_fft = win_size = 2048 and n_mels <= 128 "
                                       "(the 44.1 kHz NSF-HiFiGAN configuration); got %d / %d / %d" % (self.n_fft, self.win_size, self.n_mels))
         _need_cuda_f32("y", y)
         if y.dim() != 2:

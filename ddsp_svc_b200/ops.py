@@ -23,14 +23,14 @@ _tables_lock = threading.Lock()
 
 def set_fir_impl(impl):
     """'auto' (FFT-domain kernel for block size 512 and <= 1024 taps, else CUDA cores), 'cuda' (CUDA-core direct
-    form), 'tc' (tcgen05 3xTF32 kernel, block size 512), 'cuda8' (older scalar CUDA-core kernel) or 'fft'."""
+    form), 'tc' (wgmma 3xTF32 kernel, block size 512), 'cuda8' (older scalar CUDA-core kernel) or 'fft'."""
     global _fir_impl
     _lib.check(_lib.lib().b2d_set_fir_impl({"auto": 0, "cuda": 1, "tc": 2, "cuda8": 3, "fft": 4}[impl]), "b2d_set_fir_impl")
     _fir_impl = impl
 
 
 def set_ir_impl(impl):
-    """'auto' (tcgen05 when supported), 'cuda' (CUDA-core kernel) or 'tc' (tcgen05 3xTF32 kernel)."""
+    """'auto' (wgmma when supported), 'cuda' (CUDA-core kernel) or 'tc' (wgmma 3xTF32 kernel)."""
     _lib.check(_lib.lib().b2d_set_ir_impl({"auto": 0, "cuda": 1, "tc": 2}[impl]), "b2d_set_ir_impl")
 
 
@@ -53,7 +53,7 @@ def _ptr(t):
 
 def _need_cuda_f32(name, t, dtype=torch.float32, local=True):
     if not isinstance(t, torch.Tensor) or not t.is_cuda:
-        raise ValueError("%s must be a CUDA tensor (the B200 kernels have no CPU fallback)" % name)
+        raise ValueError("%s must be a CUDA tensor (the kernels have no CPU fallback)" % name)
     if t.dtype != dtype:
         raise ValueError("%s must be %s, got %s" % (name, dtype, t.dtype))
     if local and t.device.index != torch.cuda.current_device():
@@ -389,7 +389,7 @@ def source_module(f0, upp, sampling_rate, dim, rand_ini, linear_weight, linear_b
 
 
 def set_sinegen_impl(name):
-    """'auto' | 'v1' (one sample per thread) | 'v2' (four per thread) | 'v2p' (four per thread, packed f32x2) | 'v2r7' (v2
+    """'auto' | 'v1' (one sample per thread) | 'v2' (four per thread) | 'v2p' (four per thread, register pairs) | 'v2r7' (v2
     with Philox4x32-7 instead of -10 for the in-kernel noise)."""
     impl = {"auto": 0, "v1": 1, "v2": 2, "v2p": 3, "v2r7": 4}[name]
     _lib.check(_lib.lib().b2d_set_sinegen_impl(impl), "b2d_set_sinegen_impl")
@@ -420,7 +420,7 @@ def combsubfast_filter(comb, c_hm, c_hp, c_nm, block, noise_in=None, seed=0, utt
 
 
 def set_fft_arith(name):
-    """'packed' (default: f32x2 complex additions in the FFT kernels) | 'scalar'."""
+    """'packed' (default) | 'scalar': instantiations of the FFT kernels (identical scalar additions on Hopper)."""
     _lib.check(_lib.lib().b2d_set_fft_arith({"scalar": 0, "packed": 1}[name]), "b2d_set_fft_arith")
 
 

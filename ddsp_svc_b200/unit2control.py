@@ -181,9 +181,8 @@ class Unit2Control(nn.Module):
     gemm_precision = "3xtf32"
     #: PCmer: run the performer's linear attention (k-sum, context, normalised read-out) as ONE kernel per (utterance, head)
     #: (csrc/linear_attention.cu) instead of two batched library GEMMs + eager elementwise passes.  Off by default: correct
-    #: (same 1.4e-6 on the controls) but measured SLOWER on B200 at B = 32 x 861 frames (12.6 vs 10.5 ms for the whole
-    #: network): 256 CTAs of 9 warps, two per SM, single-buffered tiles -- it needs a split over frames and double buffering
-    #: to beat the batched SIMT GEMMs.
+    #: (same 1.4e-6 on the controls); 256 CTAs of 9 warps, two per SM, single-buffered tiles -- it needs a split over frames
+    #: and double buffering to compete with the batched SIMT GEMMs.
     fused_attention = False
 
     def __init__(self, input_channel, n_spk, output_splits, use_pitch_aug=False, pcmer_norm=False, use_naive_v2=False,

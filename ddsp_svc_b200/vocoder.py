@@ -1,6 +1,6 @@
 """Drop-in synthesizer modules: same constructor arguments, buffers (state-dict keys) and
 forward() contract as the reference's ddsp/vocoder.py classes, with the DSP executed by the
-sm_100a kernels of libb200ddsp.so.
+sm_90a kernels of libb200ddsp.so.
 
     signal, hidden, (harmonic, noise) = model(units_frames, f0_frames, volume_frames,
                                               spk_id=..., spk_mix_dict=..., initial_phase=..., infer=True)
@@ -22,7 +22,7 @@ from . import ops
 
 def _reference_unit2ctrl(n_unit, n_spk, split_map, **kw):
     """The control network: this package's own Unit2Control (same parameter tree as the reference's
-    ddsp/unit2control.py, so its checkpoints load strictly; fused B200 kernels + library GEMMs, inference only)."""
+    ddsp/unit2control.py, so its checkpoints load strictly; fused kernels + library GEMMs, inference only)."""
     from .unit2control import Unit2Control
     return Unit2Control(n_unit, n_spk, split_map, **kw)
 
@@ -36,7 +36,7 @@ def _check_shape(cls, ok, what):
     """Shapes the kernels do not cover fail when the model is BUILT (load_model / patch_reference time), not at the
     first forward after some kernels have already been launched."""
     if not ok:
-        raise ValueError("%s on B200: %s (every config the reference ships uses block_size 512)" % (cls, what))
+        raise ValueError("%s: %s (every config the reference ships uses block_size 512)" % (cls, what))
 
 
 class _SynthBase(torch.nn.Module):
@@ -57,7 +57,7 @@ class _SynthBase(torch.nn.Module):
     def _forward_only(ctrls):
         if torch.is_grad_enabled() and any(v.requires_grad for v in ctrls.values()):
             raise NotImplementedError(
-                "the B200 synthesis kernels are forward-only; call under torch.no_grad() "
+                "the synthesis kernels are forward-only; call under torch.no_grad() "
                 "(every inference caller of the reference does, e.g. main.py:250)")
 
 
@@ -179,7 +179,7 @@ class CombSubFast(_SynthBase):
     """Combtooth subtractive synthesiser with 2*block sqrt-Hann frames (the variant the diffusion / reflow vocoders
     embed) -- reference ddsp/vocoder.py:712-786.  Returns (signal, hidden, (signal, signal)) like the reference.
 
-    Parity on B200: 2e-8 RMS against the live-reference goldens (tests/test_gpu_combsubfast.py)."""
+    Parity: checked against the live-reference goldens (tests/test_gpu_combsubfast.py)."""
 
     def __init__(self, sampling_rate, block_size, n_unit=256, n_spk=1, use_pitch_aug=False, pcmer_norm=False,
                  unit2ctrl=None):

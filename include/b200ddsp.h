@@ -1,5 +1,5 @@
 /*
- * b200ddsp.h -- C ABI of libb200ddsp.so: the B200 (sm_100a) DDSP harmonic-plus-noise
+ * b200ddsp.h -- C ABI of libb200ddsp.so: the H100 (sm_90a) DDSP harmonic-plus-noise
  * synthesis kernels behind the reference's Sins / CombSub / CombSubSuperFast / SineGen
  * forward() calls (yxlllc/DDSP-SVC).
  *
@@ -90,7 +90,7 @@ int b2d_sins_bank(const float* f0_frames, const double* frame_phase, const float
  * b2d_dft_tables() (constant cos/sin matrices of the L-point inverse real DFT).
  * f0_frames is only read in mode B2D_IR_MAG_DYNAMIC (window half-width 1.5*sr/(f0+1e-3)).
  */
-/* Two implementations: tcgen05 tensor cores (3xTF32; default when the accumulators fit TMEM)
+/* Two implementations: wgmma tensor cores (3xTF32; default when the accumulators fit the registers)
  * and CUDA cores.  b2d_set_ir_impl: 0 = automatic, 1 = CUDA cores, 2 = tensor cores (test knob).
  * The table buffer (256-byte aligned) holds the constant matrices for both. */
 int    b2d_set_ir_impl(int impl);
@@ -121,10 +121,10 @@ int b2d_ltv_fir(const float* x1, const float* ir1, int taps1, float* y1,
 
 /* Kernel selection for b2d_ltv_fir and the synthesizer drivers.  0 = automatic: the FFT-domain kernel
  * (ltv_fir_fft.cu: per input hop one N-point FFT per signal, the impulse responses' spectra and one inverse FFT per
- * pair of hops; N = 1024 up to 512 taps, 2048 up to 1024 taps; ~4x fewer instructions than the direct form,
- * 0.37 ms against 1.18 ms on B200 for Sins' two 510-tap filters) when the block size is 512 and no filter has more than
+ * pair of hops; N = 1024 up to 512 taps, 2048 up to 1024 taps; ~4x fewer instructions than the direct form)
+ * when the block size is 512 and no filter has more than
  * 1024 taps, otherwise the CUDA-core direct form (block size multiple of 256).  1 = CUDA-core direct form
- * (16 outputs per thread, packed fma.rn.f32x2), 2 = tcgen05 tensor cores (3xTF32, block size 512; correct but
+ * (16 outputs per thread, register-pair FMAs), 2 = wgmma tensor cores (3xTF32, block size 512; correct but
  * operand-bandwidth bound and ~3x slower, see DESIGN.md), 3 = the older 8-outputs-per-thread scalar-FFMA direct form,
  * 4 = FFT-domain kernel wherever it applies.  B2D_FIR_AUTO=cuda in the environment makes 0 mean 1.
  * Process-wide test/diagnostic knob. */
@@ -235,10 +235,8 @@ int b2d_combsubfast_filter(const float* comb, const float* c_harmonic_magnitude,
                            uint64_t seed, int64_t utterance_offset, int B, int n_frames, int block,
                            float* signal, void* stream);
 
-/* Arithmetic of the shared-memory FFT kernels (ltv_fir_fft, superfast, combsubfast): 1 (default) = packed
- * add/sub.rn.f32x2 (one FADD2 per complex addition; 15 % / 7 % fewer instructions in the FIR / SuperFast main loops by SASS
- * count, measured 2.5 % / 1.2 % faster on B200; outputs within 5e-8 of the scalar instantiation), 0 = scalar complex
- * additions.  B2D_FFT_ARITH=scalar in the environment selects 0 as the initial value.  Process-wide test/diagnostic knob
+/* Arithmetic of the shared-memory FFT kernels (ltv_fir_fft, superfast, combsubfast): 1 (default) = the
+ * "packed" instantiations, 0 = the scalar ones; Hopper has no packed FP32 add, so both use scalar complex additions.  B2D_FFT_ARITH=scalar in the environment selects 0 as the initial value.  Process-wide test/diagnostic knob
  * (atomic, read once per call). */
 int b2d_set_fft_arith(int packed);
 
@@ -303,7 +301,7 @@ int b2d_mel_spectrogram(const float* audio, const float* window, const float* me
 
 /* b2d_sins_synth variants.  0 (default) = 1 = oscillator-bank kernel next to the impulse-response builds, then the FIR
  * kernel transforms the impulse responses itself.  2 = the bank is evaluated inside the FFT-domain FIR kernel (additionally <= 128 harmonics):
- * no [B, T] sinusoid tensor, one launch less -- measured 1.4 % slower on B200 (see api.cu), kept as a tested alternative.
+ * no [B, T] sinusoid tensor, one launch less, kept as a tested alternative (see api.cu).
  * 3 = spectrum path: a small kernel turns the impulse responses into packed 1024-point spectra once per frame (beside the
  * bank), the FIR kernel reads them: a quarter fewer transforms, 53 instead of 70 KB of shared memory (4 CTAs per SM); needs
  * block 512, both filters <= 512 taps, FIR selection 0/4; measured 4 % slower (the transform is only moved) -- the consumer
@@ -323,8 +321,7 @@ int b2d_set_overlap(int mode);
 
 /* Kernel selection for b2d_sinegen / b2d_source_module (measurement and A/B tests): 0 auto (= 4), 1 one sample per
  * thread (first kernel of round 1; also the only one for dim other than 1 or 9), 2 four samples per thread,
- * 3 four samples per thread with packed f32x2 arithmetic (3-5 % faster, but ptxas fuses its packed mul+add pairs, so
- * the sine argument is rounded once instead of twice: max error 3e-6 instead of 3e-8).  Impl 1 and 2/3 draw DIFFERENT in-kernel
+ * 3 four samples per thread with register-pair arithmetic.  Impl 1 and 2/3 draw DIFFERENT in-kernel
  * noise streams (both Philox4x32-10 keyed by seed / global utterance / position).
  * 4 = variant 2 with Philox4x32-7 instead of -10 for the in-kernel normals (7 rounds: the smallest count reported to
  * pass BigCrush; 11 % faster; Kolmogorov-Smirnov / correlation tests in tests/test_gpu_combsub_sinegen.py). */

@@ -1,35 +1,25 @@
-"""Import the live reference (yxlllc/DDSP-SVC) for oracle validation.
+"""Import the upstream reference (yxlllc/DDSP-SVC) for oracle validation.
 
 TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).  The reference is a Python /
 PyTorch program; its hot path (ddsp/vocoder.py, ddsp/core.py,
 nsf_hifigan/models.py) imports several third-party packages that are not
 installed here and are not used by the path.  They are replaced by empty stub
-modules before import.  /root/reference exists only in the build container; on the
-GPU box the staged copy under baseline/_ref/ (tools/stage_reference.py) is used when
-present, so callers must check ``available()`` first.
+modules before import.  The reference is not part of this repository: point
+DDSP_REFERENCE_ROOT at a checkout of it to use it (the golden generators under
+tests/golden/ need it); callers must check ``available()`` first.
 """
 import os
 import sys
 import types
 
-def _find_root():
-    """The live checkout in the build container, else the staged copy that travels to the GPU box
-    (baseline/_ref/, written by tools/stage_reference.py; git-ignored)."""
-    here = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    for cand in (os.environ.get("DDSP_REFERENCE_ROOT"), "/root/reference", os.path.join(here, "baseline", "_ref")):
-        if cand and os.path.isfile(os.path.join(cand, "ddsp", "vocoder.py")):
-            return cand
-    return "/root/reference"
-
-
-REFERENCE_ROOT = _find_root()
+REFERENCE_ROOT = os.environ.get("DDSP_REFERENCE_ROOT", "")
 
 _STUBS = ("pyworld", "parselmouth", "torchcrepe", "resampy", "fairseq", "gin",
           "local_attention")
 
 
 def available() -> bool:
-    return os.path.isfile(os.path.join(REFERENCE_ROOT, "ddsp", "vocoder.py"))
+    return bool(REFERENCE_ROOT) and os.path.isfile(os.path.join(REFERENCE_ROOT, "ddsp", "vocoder.py"))
 
 
 def _install_stubs():
@@ -57,8 +47,8 @@ def load():
     if "mods" in _cache:
         return _cache["mods"]
     if not available():
-        raise RuntimeError("live reference not present at %s" % REFERENCE_ROOT)
-    sys.dont_write_bytecode = True  # /root/reference is read-only
+        raise RuntimeError("reference not found: set DDSP_REFERENCE_ROOT to a DDSP-SVC checkout")
+    sys.dont_write_bytecode = True  # the reference checkout may be read-only
     _install_stubs()
     if REFERENCE_ROOT not in sys.path:
         sys.path.insert(0, REFERENCE_ROOT)

@@ -2,14 +2,14 @@
 
 TEST INFRASTRUCTURE ONLY (see oracle/__init__.py) -- never imported by the product.
 
-Why torch: the arithmetic of this path does not live in /root/reference at all, it
+Why torch: the arithmetic of this path does not live in the reference at all, it
 lives in PyTorch's CPU kernels (upsample_linear1d, cumsum with fp64 accumulation,
 sin, pocketfft rfft/irfft/stft/istft, col2im, mt19937).  PyTorch is an unpinned
 third-party dependency of the reference (requirements.txt lists no torch; README
 names 1.9.1 / 2.0.0); the build container and the GPU box both carry torch 2.11.0.
 Restating the algorithm on the same operators makes this port bit-identical to the
 live reference on CPU, which tests/test_oracle_vs_reference.py checks whenever
-/root/reference is present, and tests/test_oracle_golden.py checks against vectors
+the reference is importable, and tests/test_oracle_golden.py checks against vectors
 the live reference produced (tests/golden/make_golden.py).
 
 Every function returns the intermediate stage outputs as well, so the CUDA path can

@@ -9,12 +9,12 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (select with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
     """GPU tests never silently pass on a box without a GPU: they are skipped there
-    (the driver selects them with -m gpu on the B200 box, where they must run)."""
+    (select them with -m gpu on a machine with an H100, where they must run)."""
     try:
         import torch
         has_gpu = torch.cuda.is_available()

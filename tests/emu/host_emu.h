@@ -2,7 +2,7 @@
 //
 // One CTA = one group of std::threads; __syncthreads() is a std::barrier over the CTA; threadIdx / blockIdx are
 // thread-local; `extern __shared__` storage is a static buffer owned by the harness (CTAs run one after another).
-// Only what the emulated kernels use is provided (no warp intrinsics, no inline PTX, no TMA / tcgen05): it checks
+// Only what the emulated kernels use is provided (no warp intrinsics, no inline PTX, no TMA / wgmma): it checks
 // index arithmetic, barrier placement, shared-memory data flow and the numerical formulation -- not performance and
 // not the PTX-level features.  Kernels opt in with `#ifdef B2D_HOST_EMU` around their CUDA-only includes and launcher.
 #pragma once

@@ -1,6 +1,6 @@
 """Generate tests/golden/*.npz by running the LIVE reference (yxlllc/DDSP-SVC) on CPU.
 
-Run in the build container only (needs /root/reference):
+Needs a reference checkout (DDSP_REFERENCE_ROOT):
 
     python tests/golden/make_golden.py
 

@@ -1,15 +1,16 @@
-"""Collect measured parity errors into gpurun_out/parity_report.json (read back in the build
-container to calibrate tolerances and to quote in DESIGN.md / profiles)."""
+"""Collect measured parity errors into the JSON file named by B2D_PARITY_REPORT (to calibrate tolerances); nothing is
+written when it is unset."""
 import json
 import os
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-PATH = os.path.join(ROOT, "gpurun_out", "parity_report.json")
+PATH = os.environ.get("B2D_PARITY_REPORT")
 
 
 def record(test, **metrics):
+    if not PATH:
+        return
     try:
-        os.makedirs(os.path.dirname(PATH), exist_ok=True)
+        os.makedirs(os.path.dirname(os.path.abspath(PATH)), exist_ok=True)
         data = {}
         if os.path.isfile(PATH):
             try:

@@ -1,4 +1,4 @@
-"""CPU-side checks of the boundary: the C-ABI library builds for sm_100a, loads, and exports
+"""CPU-side checks of the boundary: the C-ABI library builds for sm_90a, loads, and exports
 every symbol include/b200ddsp.h declares; argument errors come back as codes, not crashes.
 No kernel is launched here."""
 import ctypes

@@ -1,9 +1,7 @@
-"""Packed f32x2 complex additions in the FFT kernels (ops.set_fft_arith("packed")) against the scalar default.
+"""The "packed" and "scalar" instantiations of the FFT kernels (ops.set_fft_arith) against each other.
 
-Per-lane add.rn.f32x2 / sub.rn.f32x2 round like the scalar FADDs, so the outputs are expected to be IDENTICAL unless
-ptxas re-associates or contracts differently around them (it does contract packed mul+add pairs, see sinegen.cu); the
-bound below allows for that.  Measured on B200 (round 2): Sins identical, SuperFast 4.5e-8 / CombSubFast 2.2e-8 max
-difference at 8e-3 signal RMS (fp32 round-off level); 2.5 % / 1.2 % faster kernels (profiles/r2_bench_call1_*)."""
+Hopper has no packed FP32 add, so both instantiations perform the same scalar complex additions and their outputs are
+identical: the test checks that."""
 import pytest
 import torch
 
@@ -51,4 +49,4 @@ def test_packed_matches_scalar(kind):
     scale = ref.pow(2).mean().sqrt().item()
     err = (got - ref).abs().max().item()
     report.record("fft_packed/" + kind, max_diff=err, ref_rms=scale, identical=bool(torch.equal(got, ref)))
-    assert err < 2e-7           # a few fp32 ulps of the largest samples (~0.03); the parity gate is 2e-6 RMS
+    assert torch.equal(got, ref), err

@@ -1,4 +1,4 @@
-"""The tcgen05 (tensor-core, 3xTF32) time-varying FIR against the CUDA-core kernel, the
+"""The wgmma (tensor-core, 3xTF32) time-varying FIR against the CUDA-core kernel, the
 one-thread-per-sample kernel and the oracle.  It is not the default dispatch (it is correct but
 operand-bandwidth bound, see ltv_fir_tc.cu); these tests keep it honest, including one full Sins
 forward through it."""
@@ -59,7 +59,7 @@ def test_tc_full_size_vs_generic_and_noise_modes():
     scale = y_g.pow(2).mean().sqrt().item()
     e = (y_tc - y_g).pow(2).mean().sqrt().item()
     report.record("fir_tc/full", rel_rms=e / scale, max=(y_tc - y_g).abs().max().item(), scale=scale)
-    assert e / scale < 2e-5     # the fp32 TMEM accumulator truncates: ~5e-6 after 390 accumulation steps
+    assert e / scale < 2e-5     # the fp32 tensor-core accumulator truncates: ~5e-6 after 390 accumulation steps
     # in-kernel noise: identical stream in both implementations (same Philox keying)
     ident = torch.zeros(2, 16, 510, device=DEV); ident[:, :, 255] = 1.0
     a = ops.ltv_fir(None, ident, P, seed=7)

@@ -1,4 +1,4 @@
-"""The tcgen05 (3xTF32) impulse-response builder against the CUDA-core kernel and the oracle, for
+"""The wgmma (3xTF32) impulse-response builder against the CUDA-core kernel and the oracle, for
 all three modes and several n_mag (including sizes that need column / K padding)."""
 import math
 

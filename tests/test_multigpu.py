@@ -4,7 +4,7 @@ per-chunk peer stores or copy-engine pushes on one or two compute streams, and t
 rank 0 exactly the single-GPU synthesis of the whole batch (bit for bit: the in-kernel noise is keyed by the global
 utterance index and the FFT-domain FIR is chunking-invariant).
 
-Run on a multi-GPU box:  gpurun --gpus 2 -- 'python -m pytest tests/test_multigpu.py -q'   (and --gpus 8)."""
+Run on a machine with two (and eight) GPUs:  python -m pytest tests/test_multigpu.py -q"""
 import os
 import socket
 

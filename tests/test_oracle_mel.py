@@ -40,12 +40,12 @@ def test_filterbank_agrees_with_torchaudio_and_with_the_product_host_code():
         assert (ours.sum(1) > 0).all()
 
 
-@pytest.mark.skipif(not ref_loader.available(), reason="live reference not present")
 def test_restatement_equals_the_live_reference_code():
-    ref = om.load_reference_stft()
+    """the reference's own STFT.get_mel on these inputs is stored in tests/golden/stft_live_reference.npz
+    (tests/golden/make_golden_reference.py)"""
+    gold = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "stft_live_reference.npz"))
     g = torch.Generator().manual_seed(9)
-    for T, hop in ((512 * 9 + 17, 512), (900, 512), (256 * 30, 256)):
+    for i, (T, hop) in enumerate(((512 * 9 + 17, 512), (900, 512), (256 * 30, 256))):
         y = 0.2 * torch.randn(2, T, generator=g)
-        st = ref.STFT(44100, 128, 2048, 2048, hop, 40, 16000)
         with torch.no_grad():
-            assert torch.equal(st.get_mel(y), om.get_mel(y, hop_length=hop))
+            assert np.array_equal(om.get_mel(y, hop_length=hop).numpy(), gold["mel_%d" % i])
