@@ -206,11 +206,92 @@ __device__ __forceinline__ float4 normals4(unsigned long long seed, unsigned lon
 }
 
 // shared-memory footprint (bytes): 2 x 17408 (bufA, bufS) + 16384 (src) + 12288 (ring) + 4112 (win)
-// + 1920 (tw2) + 2048 (tw3) = 71568  -> 3 CTAs per SM
+// + 1920 (tw2) + 2048 (tw3) = 71568  -> 3 CTAs per SM  (the backward kernel uses the same layout)
 constexpr int kWinLen = kHalf + 4;   // window stored for i in [0, 1024]; win[i] = win[2048 - i]
 constexpr size_t kSmemBytes = (size_t)2 * kPadN * sizeof(float2) + (size_t)kN * sizeof(float2) +
                               (size_t)kRingHops * kHop * sizeof(float) + (size_t)kWinLen * sizeof(float) +
                               (size_t)(15 * 16 + 256) * sizeof(float2);
+
+// one-time tables of both kernels: periodic Hann (first half), FFT pass twiddles; zeroed hop ring
+__device__ __forceinline__ void sf_tables(float* winh, float2* tw2, float2* tw3, float* ring, int tid) {
+    for (int i = tid; i <= kHalf; i += kThreads) winh[i] = 0.5f - 0.5f * cospif((float)i * (2.0f / kN));
+    for (int i = tid; i < 15 * 16; i += kThreads) {
+        const int r = i / 16 + 1, k = i % 16;
+        float sn, cs; sincospif(-2.0f * (float)(r * k) / 256.0f, &sn, &cs);
+        tw2[i] = make_float2(cs, sn);
+    }
+    for (int i = tid; i < 256; i += kThreads) {
+        float sn, cs; sincospif(-2.0f * (float)i / 2048.0f, &sn, &cs);
+        tw3[i] = make_float2(cs, sn);
+    }
+    for (int i = tid; i < kRingHops * kHop; i += kThreads) ring[i] = 0.f;
+}
+
+// The un-windowed source (comb, noise) of one utterance, as both kernels evaluate it.
+struct SfSource {
+    const float4* fpar;          // (s, ds, acc_prev) per frame of this utterance
+    const float* noise_row;      // explicit N(0,1) samples of this utterance or nullptr (in-kernel Philox)
+    unsigned long long seed, utt;
+    int T, P;
+    bool reflect;                // pad_mode (:672-675)
+};
+
+// source samples of absolute positions [mstart + i_lo, mstart + i_hi) -> src ring slots (i + off) & 2047
+__device__ __forceinline__ void sf_fill_src(float2* src, const SfSource& s, int mstart, int off, int i_lo, int i_hi,
+                                            int tid) {
+    const int T = s.T, P = s.P;
+    const float fP = (float)P;
+#pragma unroll 1
+    for (int i0 = i_lo + (tid << 2); i0 < i_hi; i0 += kThreads << 2) {
+        const int m0 = mstart + i0;
+        float cv[4], nv[4];
+        if (m0 >= 0 && m0 + 3 < T) {
+            float4 nz;
+            if (s.noise_row) nz = __ldg(reinterpret_cast<const float4*>(s.noise_row + m0));   // m0 % 4 == 0
+            else nz = normals4(s.seed, s.utt, (uint32_t)(m0 >> 2));
+            nv[0] = nz.x; nv[1] = nz.y; nv[2] = nz.z; nv[3] = nz.w;
+#pragma unroll
+            for (int e = 0; e < 4; ++e) cv[e] = comb_at(s.fpar, P, fP, m0 + e);
+        } else {
+#pragma unroll 1
+            for (int e = 0; e < 4; ++e) {
+                int m = m0 + e;
+                bool valid = true;
+                if (m < 0 || m >= T) {
+                    if (s.reflect) m = (m < 0) ? -m : 2 * (T - 1) - m;
+                    else valid = false;
+                }
+                cv[e] = 0.f; nv[e] = 0.f;
+                if (valid) {
+                    cv[e] = comb_at(s.fpar, P, fP, m);
+                    if (s.noise_row) nv[e] = s.noise_row[m];
+                    else {
+                        const float4 g = normals4(s.seed, s.utt, (uint32_t)(m >> 2));
+                        const int l = m & 3;
+                        nv[e] = l == 0 ? g.x : l == 1 ? g.y : l == 2 ? g.z : g.w;
+                    }
+                }
+            }
+        }
+#pragma unroll
+        for (int e = 0; e < 4; ++e) src[(i0 + e + off) & (kN - 1)] = make_float2(cv[e], nv[e]);
+    }
+}
+
+// OLA(win^2) of the iSTFT at sample i4 + e of hop h: the frames h-1 .. h+2 that exist (0 .. nF)
+__device__ __forceinline__ float sf_env(const float* winh, int h, int nF, int i) {
+    float env = 0.f;
+#pragma unroll
+    for (int d = -1; d <= 2; ++d) {
+        const int qq = h + d;
+        if (qq >= 0 && qq <= nF) {
+            const int k = i - d * kHop + kHalf;
+            const float w = winh[k <= kHalf ? k : kN - k];
+            env = fmaf(w, w, env);
+        }
+    }
+    return env;
+}
 
 // PK: the "packed" complex-addition policy of the FFT butterflies (fft_regs.cuh Ar<true>; scalar on Hopper)
 template <bool PK>
@@ -228,65 +309,17 @@ __global__ void __launch_bounds__(kThreads, 3) superfast_kernel(SfParams p) {
     const int b = blockIdx.y;
     const int nF = p.nF, P = p.P, T = nF * P;
     const int h0 = blockIdx.x * p.G, h1 = min(h0 + p.G, nF);
-    const float fP = (float)P;
-    const bool reflect = T > kHalf;                              // pad_mode (:672-675)
-    const float4* fpar = p.frame_par + (size_t)b * nF;
-    const float* noise_row = p.noise_in ? p.noise_in + (size_t)b * T : nullptr;
-    const unsigned long long utt = (unsigned long long)(p.utt_off + b);
+    SfSource sv;
+    sv.fpar = p.frame_par + (size_t)b * nF;
+    sv.noise_row = p.noise_in ? p.noise_in + (size_t)b * T : nullptr;
+    sv.seed = p.seed; sv.utt = (unsigned long long)(p.utt_off + b);
+    sv.T = T; sv.P = P; sv.reflect = T > kHalf;
 
     // ---- one-time tables ----
-    for (int i = tid; i <= kHalf; i += kThreads) winh[i] = 0.5f - 0.5f * cospif((float)i * (2.0f / kN));
-    for (int i = tid; i < 15 * 16; i += kThreads) {
-        const int r = i / 16 + 1, k = i % 16;
-        float sn, cs; sincospif(-2.0f * (float)(r * k) / 256.0f, &sn, &cs);
-        tw2[i] = make_float2(cs, sn);
-    }
-    for (int i = tid; i < 256; i += kThreads) {
-        float sn, cs; sincospif(-2.0f * (float)i / 2048.0f, &sn, &cs);
-        tw3[i] = make_float2(cs, sn);
-    }
-    for (int i = tid; i < kRingHops * kHop; i += kThreads) ring[i] = 0.f;
+    sf_tables(winh, tw2, tw3, ring, tid);
     __syncthreads();
     auto win_at = [&](int i) { return winh[i <= kHalf ? i : kN - i]; };
-
-    // source samples of absolute positions [mstart + i_lo, mstart + i_hi) -> src ring slots (i + off) & 2047
-    auto fill_src = [&](int mstart, int off, int i_lo, int i_hi) {
-#pragma unroll 1
-        for (int i0 = i_lo + (tid << 2); i0 < i_hi; i0 += kThreads << 2) {
-            const int m0 = mstart + i0;
-            float cv[4], nv[4];
-            if (m0 >= 0 && m0 + 3 < T) {
-                float4 nz;
-                if (noise_row) nz = __ldg(reinterpret_cast<const float4*>(noise_row + m0));   // m0 % 4 == 0
-                else nz = normals4(p.seed, utt, (uint32_t)(m0 >> 2));
-                nv[0] = nz.x; nv[1] = nz.y; nv[2] = nz.z; nv[3] = nz.w;
-#pragma unroll
-                for (int e = 0; e < 4; ++e) cv[e] = comb_at(fpar, P, fP, m0 + e);
-            } else {
-#pragma unroll 1
-                for (int e = 0; e < 4; ++e) {
-                    int m = m0 + e;
-                    bool valid = true;
-                    if (m < 0 || m >= T) {
-                        if (reflect) m = (m < 0) ? -m : 2 * (T - 1) - m;
-                        else valid = false;
-                    }
-                    cv[e] = 0.f; nv[e] = 0.f;
-                    if (valid) {
-                        cv[e] = comb_at(fpar, P, fP, m);
-                        if (noise_row) nv[e] = noise_row[m];
-                        else {
-                            const float4 g = normals4(p.seed, utt, (uint32_t)(m >> 2));
-                            const int l = m & 3;
-                            nv[e] = l == 0 ? g.x : l == 1 ? g.y : l == 2 ? g.z : g.w;
-                        }
-                    }
-                }
-            }
-#pragma unroll
-            for (int e = 0; e < 4; ++e) src[(i0 + e + off) & (kN - 1)] = make_float2(cv[e], nv[e]);
-        }
-    };
+    auto fill_src = [&](int mstart, int off, int i_lo, int i_hi) { sf_fill_src(src, sv, mstart, off, i_lo, i_hi, tid); };
 
     const int qs = max(h0 - 1, 0), qe = min(h1 + 1, nF);
     int off = 0;            // src ring offset of the current frame's sample 0
@@ -394,19 +427,176 @@ __global__ void __launch_bounds__(kThreads, 3) superfast_kernel(SfParams p) {
                 const int n = h * P + i4;
                 float v[4] = {acc.x, acc.y, acc.z, acc.w};
 #pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    float env = 0.f;     // OLA(win^2) over the frames that exist
-#pragma unroll
-                    for (int d = -1; d <= 2; ++d) {
-                        const int qq = h + d;
-                        if (qq >= 0 && qq <= nF) { const float w = win_at(i4 + e - d * kHop + kHalf); env = fmaf(w, w, env); }
-                    }
-                    v[e] = __fdiv_rn(v[e], env);
-                }
+                for (int e = 0; e < 4; ++e) v[e] = __fdiv_rn(v[e], sf_env(winh, h, nF, i4 + e));
                 b2d::st_global_v4(p.out + (size_t)b * T + n, make_float4(v[0], v[1], v[2], v[3]));
             }
         }
         __syncthreads();
+    }
+}
+
+// ---- backward: gradients of the four raw controls ----------------------------------------------------------
+// g = dL/dsignal.  For frame q (row min(q, nF-1)):
+//   r_q[i] = win[i] g[n] / env(n), n = qP + i - 1024 (0 outside [0, T))      cotangent of the windowed frame
+//   G_q    = adjoint of irfft applied to R_q = rfft(r_q): (2/N) R_q[k], and (1/N) Re R_q[k] at DC / Nyquist
+//   A      = X_q exp(m_h + j pi p_h)  (noise: N_q exp(m_n + j pi p_n) / 128), with X_q, N_q recomputed as the
+//            forward computes them (same source, same noise stream)
+//   dL/dm  = Re(conj(G) A),  dL/dp = -pi Im(conj(G) A)
+// One CTA owns the control rows [h0, h1) of one utterance and transforms exactly those frames (plus frame nF,
+// which the owner of row nF-1 adds into that row): no overlap, no atomics, deterministic.  Per frame one complex
+// FFT of win * (comb + j noise) as in the forward; per pair of frames one complex FFT of r_a + j r_b, split by
+// conjugate symmetry -> 1.5 FFTs per frame.  g / env is kept in a 6-hop shared-memory ring (the forward's OLA
+// ring), so each frame reads one new hop of g.
+struct SfBwdParams {
+    const float4* frame_par;   // [B, nF]
+    const float* c_hm; const float* c_hp; const float* c_nm; const float* c_np;
+    long long ctrl_stride;
+    const float* noise_in;     // [B, T] or nullptr
+    const float* grad;         // [B, T]  dL/dsignal
+    float* grad_ctrl;          // [B, nF, 4 * 1025]  harmonic_magnitude | harmonic_phase | noise_magnitude | noise_phase
+    int nF, P, G;
+    unsigned long long seed;
+    long long utt_off;
+};
+
+template <bool PK>
+__global__ void __launch_bounds__(kThreads, 3) superfast_bwd_kernel(SfBwdParams p) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    float2* bufA = reinterpret_cast<float2*>(smem_raw);          // [kPadN] windowed source frame -> its spectrum
+    float2* bufS = bufA + kPadN;                                 // [kPadN] cotangent pair r_a + j r_b -> spectrum
+    float2* src = bufS + kPadN;                                  // [kN]   un-windowed (comb, noise), ring-indexed
+    float2* tw2 = src + kN;
+    float2* tw3 = tw2 + 15 * 16;
+    float* ring = reinterpret_cast<float*>(tw3 + 256);           // [6][512]  g / env by hop
+    float* winh = ring + kRingHops * kHop;
+
+    const int tid = threadIdx.x;
+    const int b = blockIdx.y;
+    const int nF = p.nF, P = p.P, T = nF * P;
+    const int h0 = blockIdx.x * p.G, h1 = min(h0 + p.G, nF);
+    const int qe = (h1 == nF) ? nF : h1 - 1;                     // last frame of this CTA
+    constexpr int kBins = kHalf + 1;
+    SfSource sv;
+    sv.fpar = p.frame_par + (size_t)b * nF;
+    sv.noise_row = p.noise_in ? p.noise_in + (size_t)b * T : nullptr;
+    sv.seed = p.seed; sv.utt = (unsigned long long)(p.utt_off + b);
+    sv.T = T; sv.P = P; sv.reflect = T > kHalf;
+    const float* grow = p.grad + (size_t)b * T;
+
+    sf_tables(winh, tw2, tw3, ring, tid);
+    __syncthreads();
+    auto win_at = [&](int i) { return winh[i <= kHalf ? i : kN - i]; };
+
+    int off = 0;                // src ring offset of the current frame's sample 0
+    bool primed = false;
+    int loaded = h0 - 3;        // highest hop of g / env in the ring
+
+    for (int qa = h0; qa <= qe; qa += 2) {
+        const int qb = qa + 1;
+        const bool has_b = qb <= qe;
+        // ---- hops qa-2 .. qa+2 of g / env (zero outside the utterance: the part the iSTFT trims) ----
+        for (int h = max(loaded + 1, qa - 2); h <= qa + 2; ++h) {
+            const int i4 = tid << 2;
+            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (h >= 0 && h < nF) {
+                v = __ldg(reinterpret_cast<const float4*>(grow + (size_t)h * P + i4));
+                v.x = __fdiv_rn(v.x, sf_env(winh, h, nF, i4));
+                v.y = __fdiv_rn(v.y, sf_env(winh, h, nF, i4 + 1));
+                v.z = __fdiv_rn(v.z, sf_env(winh, h, nF, i4 + 2));
+                v.w = __fdiv_rn(v.w, sf_env(winh, h, nF, i4 + 3));
+            }
+            *reinterpret_cast<float4*>(ring + ((h + 6 * 1024) % kRingHops) * kHop + i4) = v;
+        }
+        loaded = qa + 2;
+        __syncthreads();
+        // ---- cotangent pair r_a + j r_b (frame q covers hops q-2 .. q+1) ----
+        int hslot[5];
+#pragma unroll
+        for (int t = 0; t < 5; ++t) hslot[t] = ((qa - 2 + t + 6 * 1024) % kRingHops) * kHop;
+#pragma unroll 4
+        for (int i = tid; i < kN; i += kThreads) {
+            const float w = win_at(i);
+            const int hi = i >> 9, lo = i & (kHop - 1);
+            const float ra = w * ring[hslot[hi] + lo];
+            const float rb = has_b ? w * ring[hslot[hi + 1] + lo] : 0.f;
+            bufS[padi(i)] = make_float2(ra, rb);
+        }
+        __syncthreads();
+        fft2048<PK>(bufS, tw2, tw3, tid);
+#pragma unroll 1
+        for (int which = 0; which < 2; ++which) {
+            if (which == 1 && !has_b) break;
+            const int q = which ? qb : qa;
+            const int mstart = q * P - kHalf;
+            if (!primed) { sf_fill_src(src, sv, mstart, off, 0, kN, tid); primed = true; }
+            else { off = (off + kHop) & (kN - 1); sf_fill_src(src, sv, mstart, off, kN - kHop, kN, tid); }
+            __syncthreads();
+#pragma unroll 4
+            for (int i = tid; i < kN; i += kThreads) {
+                const float2 v = src[(i + off) & (kN - 1)];
+                const float w = win_at(i);
+                bufA[padi(i)] = make_float2(w * v.x, w * v.y);
+            }
+            const int qc = min(q, nF - 1);
+            const size_t crow = ((size_t)b * nF + qc) * p.ctrl_stride;
+            float chm[9], chp[9], cnm[9], cnp[9];
+#pragma unroll
+            for (int it = 0; it < 8; ++it) {
+                const size_t o = crow + tid + it * kThreads;
+                chm[it] = __ldg(p.c_hm + o); chp[it] = __ldg(p.c_hp + o);
+                cnm[it] = __ldg(p.c_nm + o); cnp[it] = __ldg(p.c_np + o);
+            }
+            chm[8] = chp[8] = cnm[8] = cnp[8] = 0.f;
+            if (tid == 0) {
+                chm[8] = __ldg(p.c_hm + crow + kHalf); chp[8] = __ldg(p.c_hp + crow + kHalf);
+                cnm[8] = __ldg(p.c_nm + crow + kHalf); cnp[8] = __ldg(p.c_np + crow + kHalf);
+            }
+            __syncthreads();
+            fft2048<PK>(bufA, tw2, tw3, tid);
+            float* grow_out = p.grad_ctrl + ((size_t)b * nF + qc) * (4 * kBins);
+            const bool held = q == nF;                            // frame nF reuses row nF-1: add into it
+#pragma unroll
+            for (int it = 0; it < 9; ++it) {
+                const int bin = (it < 8) ? tid + it * kThreads : kHalf;
+                if (it == 8 && tid != 0) break;
+                const int mir = (kN - bin) & (kN - 1);
+                // source spectra X (comb) and Nz (noise) of this frame, as in the forward
+                const float2 za = bufA[padi(bin)];
+                float2 zb = bufA[padi(mir)];
+                zb.y = -zb.y;
+                const float2 X = make_float2(0.5f * (za.x + zb.x), 0.5f * (za.y + zb.y));
+                const float2 dz = csub(za, zb);
+                const float2 Nz = make_float2(0.5f * dz.y, -0.5f * dz.x);
+                // this frame's cotangent spectrum R from the pair spectrum (a: even part, b: odd part / j)
+                const float2 sa = bufS[padi(bin)];
+                float2 sb = bufS[padi(mir)];
+                sb.y = -sb.y;
+                float2 R;
+                if (which == 0) R = make_float2(0.5f * (sa.x + sb.x), 0.5f * (sa.y + sb.y));
+                else { const float2 ds = csub(sa, sb); R = make_float2(0.5f * ds.y, -0.5f * ds.x); }
+                // adjoint of irfft: the forward drops Im at DC and Nyquist
+                float2 Gc;
+                if (bin == 0 || bin == kHalf) Gc = make_float2(R.x * (1.0f / kN), 0.f);
+                else Gc = make_float2(R.x * (2.0f / kN), R.y * (2.0f / kN));
+                float sh, ch, sn, cn;
+                __sincosf(B2D_PI_F * chp[it], &sh, &ch);
+                __sincosf(B2D_PI_F * cnp[it], &sn, &cn);
+                const float eh = __expf(chm[it]), en = __expf(cnm[it]) * 0.0078125f;   // /128 (:668)
+                const float2 Ah = cmul(X, make_float2(eh * ch, eh * sh));
+                const float2 An = cmul(Nz, make_float2(en * cn, en * sn));
+                float dmh = fmaf(Gc.x, Ah.x, Gc.y * Ah.y);                           // Re(conj(G) A)
+                float dph = -B2D_PI_F * fmaf(Gc.x, Ah.y, -Gc.y * Ah.x);              // -pi Im(conj(G) A)
+                float dmn = fmaf(Gc.x, An.x, Gc.y * An.y);
+                float dpn = -B2D_PI_F * fmaf(Gc.x, An.y, -Gc.y * An.x);
+                if (held) {     // row nF-1 was stored by this thread for frame nF-1 (same bin -> same thread)
+                    dmh += grow_out[bin]; dph += grow_out[kBins + bin];
+                    dmn += grow_out[2 * kBins + bin]; dpn += grow_out[3 * kBins + bin];
+                }
+                grow_out[bin] = dmh; grow_out[kBins + bin] = dph;
+                grow_out[2 * kBins + bin] = dmn; grow_out[3 * kBins + bin] = dpn;
+            }
+            __syncthreads();
+        }
     }
 }
 
@@ -464,5 +654,47 @@ extern "C" int b2d_superfast_synth(const void* workspace, const float* c_harmoni
     const int rc = b2d::g_fft_packed.load(std::memory_order_relaxed) ? go(superfast_kernel<true>) : go(superfast_kernel<false>);
     if (rc) return rc;
     return b2d::check_launch("superfast_synth");
+}
+
+extern "C" int b2d_superfast_synth_backward(const void* workspace, const float* c_hm, const float* c_hp,
+                                            const float* c_nm, const float* c_np, int64_t ctrl_stride,
+                                            const float* noise_in, uint64_t seed, int64_t utterance_offset,
+                                            const float* grad_signal, int B, int n_frames, int block, int win_length,
+                                            float* grad_ctrl, void* stream) {
+    if (!workspace || !c_hm || !c_hp || !c_nm || !c_np || !grad_signal || !grad_ctrl)
+        return b2d::fail(B2D_ERR_NULL, "superfast_synth_backward: null pointer");
+    if (B <= 0 || n_frames <= 0 || block <= 0 || ctrl_stride < win_length / 2 + 1)
+        return b2d::fail(B2D_ERR_SHAPE, "superfast_synth_backward: bad shape");
+    if (win_length != kN || block != 512)
+        return b2d::fail(B2D_ERR_UNSUPPORTED, "superfast_synth_backward: only win_length=2048 / block_size=512 "
+                         "(configs/combsub.yaml) is implemented (got %d / %d)", win_length, block);
+    if (B > 65535) return b2d::fail(B2D_ERR_UNSUPPORTED, "superfast_synth_backward: batch %d > 65535", B);
+    if (!b2d::aligned16(grad_signal) || !b2d::aligned16(grad_ctrl) || !b2d::aligned16(workspace) ||
+        (noise_in && !b2d::aligned16(noise_in)))
+        return b2d::fail(B2D_ERR_ALIGN, "superfast_synth_backward: grad_signal / grad_ctrl / noise_in / workspace "
+                         "must be 16-byte aligned");
+    SfBwdParams p;
+    p.frame_par = static_cast<const float4*>(workspace);
+    p.c_hm = c_hm; p.c_hp = c_hp; p.c_nm = c_nm; p.c_np = c_np;
+    p.ctrl_stride = ctrl_stride; p.noise_in = noise_in; p.grad = grad_signal; p.grad_ctrl = grad_ctrl;
+    p.nF = n_frames; p.P = block;
+    // chunk length: every frame is transformed once whatever G is; a chunk only re-primes the source (4 hops)
+    // and the g ring, so shrink it until the grid keeps >= ~4 CTAs per SM
+    int G = 29;
+    while (G > 5 && (long long)B * ((n_frames + G - 1) / G) < 4 * b2d::num_sms()) G -= 4;
+    p.G = G;
+    p.seed = seed; p.utt_off = utterance_offset;
+    const size_t smem = kSmemBytes;
+    auto go = [&](auto kern) -> int {
+        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return b2d::fail((int)e, "superfast_synth_backward: smem attr: %s", cudaGetErrorString(e));
+        cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        kern<<<dim3((n_frames + G - 1) / G, B), kThreads, smem, (cudaStream_t)stream>>>(p);
+        return 0;
+    };
+    const int rc = b2d::g_fft_packed.load(std::memory_order_relaxed) ? go(superfast_bwd_kernel<true>)
+                                                                     : go(superfast_bwd_kernel<false>);
+    if (rc) return rc;
+    return b2d::check_launch("superfast_synth_backward");
 }
 #endif  // B2D_HOST_EMU

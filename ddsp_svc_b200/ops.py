@@ -334,19 +334,85 @@ def superfast_scan(f0_frames, block, sampling_rate):
 
 def superfast_synth(ws, c_hm, c_hp, c_nm, c_np, block, win_length, noise_in=None, seed=0, utterance_offset=0,
                     signal_out=None):
+    """CombSubSuperFast after the frame scan: raw controls [B, nF, win_length/2+1] -> signal [B, nF*block].
+    Differentiable with respect to the four controls when one of them requires grad (and grad mode is on):
+    the backward runs superfast_synth_backward with the same workspace, noise and seed."""
+    if torch.is_grad_enabled() and any(isinstance(c, torch.Tensor) and c.requires_grad for c in (c_hm, c_hp, c_nm, c_np)):
+        if signal_out is not None:
+            raise ValueError("signal_out cannot be used when the controls require grad (it may be peer-mapped memory "
+                             "that autograd does not own)")
+        if noise_in is not None:
+            noise_in = noise_in.detach()
+        return _SuperFastSynth.apply(ws, int(block), int(win_length), noise_in, int(seed), int(utterance_offset),
+                                     c_hm, c_hp, c_nm, c_np)
+    return _superfast_synth(ws, c_hm, c_hp, c_nm, c_np, block, win_length, noise_in, seed, utterance_offset,
+                            signal_out)
+
+
+def _superfast_args(ws, c_hm, c_hp, c_nm, c_np, block, win_length, noise_in):
+    """checked (ws, controls, frame stride, noise rows, B, nF) of a superfast call"""
     if c_hm.dim() != 3:
         raise ValueError("controls must be [B, n_frames, win_length/2+1]")
     B, nF = c_hm.shape[0], c_hm.shape[1]
     if not isinstance(ws, torch.Tensor) or not ws.is_cuda or ws.dtype != torch.uint8 or \
             ws.numel() < _lib.lib().b2d_superfast_workspace_bytes(B, nF):
         raise ValueError("ws must be the workspace superfast_scan returned for the same (B, n_frames) = (%d, %d)" % (B, nF))
-    (hm, hp, nm, npz), stride = _same_stride([("harmonic_magnitude", c_hm), ("harmonic_phase", c_hp),
-                                              ("noise_magnitude", c_nm), ("noise_phase", c_np)], B, nF)
-    if hm.shape[2] != win_length // 2 + 1:
+    ctrls, stride = _same_stride([("harmonic_magnitude", c_hm), ("harmonic_phase", c_hp),
+                                  ("noise_magnitude", c_nm), ("noise_phase", c_np)], B, nF)
+    if ctrls[0].shape[2] != win_length // 2 + 1:
         raise ValueError("controls must have win_length/2+1 = %d bins" % (win_length // 2 + 1))
-    T = nF * block
     if noise_in is not None:
-        noise_in = _noise_rows(noise_in, B, T)
+        noise_in = _noise_rows(noise_in, B, nF * block)
+    return ctrls, stride, noise_in, B, nF
+
+
+def superfast_synth_backward(ws, c_hm, c_hp, c_nm, c_np, grad_signal, block, win_length, noise_in=None, seed=0,
+                             utterance_offset=0):
+    """Gradient of superfast_synth with respect to the four raw controls, for dL/dsignal ``grad_signal`` [B, T].
+    ws / controls / noise_in / seed / utterance_offset must be those of the forward call (the kernel recomputes the
+    source spectra and regenerates the in-kernel noise).  -> dense [B, nF, 4*(win_length/2+1)]: harmonic_magnitude |
+    harmonic_phase | noise_magnitude | noise_phase along the last axis (the split_to_dict layout)."""
+    (hm, hp, nm, npz), stride, noise_in, B, nF = _superfast_args(ws, c_hm, c_hp, c_nm, c_np, block, win_length, noise_in)
+    _need_cuda_f32("grad_signal", grad_signal)
+    if tuple(grad_signal.shape) != (B, nF * block):
+        raise ValueError("grad_signal must be [B, n_frames*block] = [%d, %d], got %s"
+                         % (B, nF * block, tuple(grad_signal.shape)))
+    grad_signal = grad_signal.contiguous()
+    grad = torch.empty(B, nF, 4 * (win_length // 2 + 1), dtype=torch.float32, device=hm.device)
+    rc = _lib.lib().b2d_superfast_synth_backward(ws.data_ptr(), hm.data_ptr(), hp.data_ptr(), nm.data_ptr(),
+                                                 npz.data_ptr(), stride, _ptr(noise_in), int(seed), int(utterance_offset),
+                                                 grad_signal.data_ptr(), B, nF, int(block), int(win_length),
+                                                 grad.data_ptr(), _stream())
+    _lib.check(rc, "b2d_superfast_synth_backward")
+    _count(1)
+    return grad
+
+
+class _SuperFastSynth(torch.autograd.Function):
+    """superfast_synth with a CUDA backward.  Saves the scan workspace, the control views and the noise input (no
+    spectra): the backward kernel recomputes the source spectra and regenerates the in-kernel noise from seed."""
+
+    @staticmethod
+    def forward(ctx, ws, block, win_length, noise_in, seed, utterance_offset, c_hm, c_hp, c_nm, c_np):
+        signal = _superfast_synth(ws, c_hm, c_hp, c_nm, c_np, block, win_length, noise_in, seed, utterance_offset)
+        ctx.save_for_backward(ws, noise_in, c_hm, c_hp, c_nm, c_np)
+        ctx.cfg = (block, win_length, seed, utterance_offset)
+        return signal
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_signal):
+        ws, noise_in, c_hm, c_hp, c_nm, c_np = ctx.saved_tensors
+        block, win_length, seed, utterance_offset = ctx.cfg
+        grad = superfast_synth_backward(ws, c_hm, c_hp, c_nm, c_np, grad_signal, block, win_length, noise_in=noise_in,
+                                        seed=seed, utterance_offset=utterance_offset)
+        return (None,) * 6 + tuple(torch.split(grad, win_length // 2 + 1, dim=-1))
+
+
+def _superfast_synth(ws, c_hm, c_hp, c_nm, c_np, block, win_length, noise_in=None, seed=0, utterance_offset=0,
+                     signal_out=None):
+    (hm, hp, nm, npz), stride, noise_in, B, nF = _superfast_args(ws, c_hm, c_hp, c_nm, c_np, block, win_length, noise_in)
+    T = nF * block
     if signal_out is not None:
         _need_cuda_f32("signal_out", signal_out, local=False)        # may be peer-mapped memory of another GPU
         if tuple(signal_out.shape) != (B, T) or not signal_out.is_contiguous():

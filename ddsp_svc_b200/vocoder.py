@@ -162,12 +162,21 @@ class CombSubSuperFast(_SynthBase):
 
     def forward(self, units_frames, f0_frames, volume_frames, spk_id=None, spk_mix_dict=None, aug_shift=None,
                 initial_phase=None, infer=True, noise=None, utterance_offset=0, signal_out=None, **kwargs):
-        """``initial_phase`` is accepted and ignored, like the reference (ddsp/vocoder.py:653-661)."""
+        """``initial_phase`` is accepted and ignored, like the reference (ddsp/vocoder.py:653-661).
+
+        Trainable: when a control from ``unit2ctrl`` requires grad (and grad mode is on), ``signal`` is
+        differentiable with respect to the four controls (CUDA backward, ops.superfast_synth_backward).
+        f0 is data (reference train.py), so an f0 that requires grad is refused."""
         sr, block, win = self._scalars()
+        if torch.is_grad_enabled() and isinstance(f0_frames, torch.Tensor) and f0_frames.requires_grad:
+            raise NotImplementedError("CombSubSuperFast has no gradient with respect to f0_frames; pass f0 as data "
+                                      "(f0_frames.detach()), as the reference's train.py does")
         ws, phase_frames = ops.superfast_scan(f0_frames, block, sr)
         ctrls, hidden = self.unit2ctrl(units_frames, f0_frames, phase_frames, volume_frames, spk_id=spk_id,
                                        spk_mix_dict=spk_mix_dict, aug_shift=aug_shift)
-        self._forward_only(ctrls)
+        if signal_out is not None and torch.is_grad_enabled() and any(v.requires_grad for v in ctrls.values()):
+            raise ValueError("signal_out cannot be combined with controls that require grad; call under "
+                             "torch.no_grad() or drop signal_out")
         signal = ops.superfast_synth(ws, ctrls["harmonic_magnitude"], ctrls["harmonic_phase"],
                                      ctrls["noise_magnitude"], ctrls["noise_phase"], block, win, noise_in=noise,
                                      seed=0 if noise is not None else _host_seed(),

@@ -213,6 +213,17 @@ int    b2d_superfast_synth(const void* workspace, const float* c_harmonic_magnit
                            const float* c_noise_phase, int64_t ctrl_stride, const float* noise_in,
                            uint64_t seed, int64_t utterance_offset, int B, int n_frames, int block,
                            int win_length, float* signal, void* stream);
+/* Backward of b2d_superfast_synth with respect to the four raw controls (training; no gradient with respect to
+ * f0).  Same workspace, controls, noise_in / seed / utterance_offset as the forward call (the comb and noise
+ * spectra are recomputed, the in-kernel noise stream is regenerated); grad_signal = dL/dsignal [B, T] (T =
+ * n_frames*block).  grad_ctrl [B, n_frames, 4*(win_length/2+1)] receives dL/d(harmonic_magnitude |
+ * harmonic_phase | noise_magnitude | noise_phase) per frame; it is overwritten, deterministically (no atomics).
+ * grad_signal, grad_ctrl, noise_in and workspace must be 16-byte aligned. */
+int    b2d_superfast_synth_backward(const void* workspace, const float* c_hm, const float* c_hp,
+                                    const float* c_nm, const float* c_np, int64_t ctrl_stride,
+                                    const float* noise_in, uint64_t seed, int64_t utterance_offset,
+                                    const float* grad_signal, int B, int n_frames, int block, int win_length,
+                                    float* grad_ctrl, void* stream);
 
 /* SineGen fused with the tail of SourceModuleHnNSF.   replaces nsf_hifigan/models.py:201-204
  * (sine_merge = tanh(l_linear(sine_wavs))) on top of b2d_sinegen: merged [B, n_frames*upp] =
