@@ -30,7 +30,7 @@ def test_combsub_stages(name):
     e_comb = util.rms(comb - ref["comb"])
     ir_h = ops.ir_build(c["harmonic_magnitude"], ops.IR_MAG_DYNAMIC, SR, f0_frames=f0).cpu()
     e_irh = (ir_h - ref["ir_harmonic"]).abs().max().item()
-    # 1022-tap FIR (two tap segments) on the oracle's intermediate signal
+    # 1022-tap FIR on the oracle's intermediate signal ('auto' runs it on the FFT-domain kernel's 2048-point instance)
     y = ops.ltv_fir(ref["allpassed"].to(DEV), ref["ir_harmonic"].to(DEV).contiguous(), P).cpu()
     e_fir = util.rms(y - ref["harmonic"])
     report.record("combsub_stages/" + name, comb_rms=e_comb, comb_max=(comb - ref["comb"]).abs().max().item(),
