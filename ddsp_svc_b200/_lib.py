@@ -73,6 +73,10 @@ SIGNATURES = {
     "b2d_mel_frames": (ctypes.c_int, [ctypes.c_int] * 4),
     "b2d_mel_spectrogram": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                            ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, c_f32p, c_stream]),
+    "b2d_mel_spectrogram_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
+                                                    ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                                    ctypes.c_float, c_f32p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64,
+                                                    c_f32p, c_stream]),
     "b2d_volume_extract": (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p, c_stream]),
     "b2d_volume_mask": (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_float, c_f32p, c_stream]),
     "b2d_mask_apply": (ctypes.c_int, [c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,

@@ -4,7 +4,9 @@ and reflow/vocoder.py:125 (SURVEY 8f rank 4).
 
 ``STFT.get_mel(y)`` runs ONE kernel (csrc/mel.cu: padding + Hann frames + 2048-point FFT + magnitude + sparse mel
 projection + log) for the shape every shipped configuration uses -- keyshift 0, speed 1, n_fft = win_size = 2048.
-Other shapes raise NotImplementedError (there is no PyTorch fallback in this package).
+Other shapes raise NotImplementedError (there is no PyTorch fallback in this package).  When ``y`` requires grad (and
+grad mode is on), the result is differentiable with respect to ``y``: the backward runs ``mel_bwd_kernel`` (same file),
+which recomputes the spectra from ``y`` instead of storing them.
 
 The mel filterbank is librosa's (``librosa.filters.mel``, Slaney scale and normalisation: a third-party dependency of
 the reference, unpinned in requirements.txt and absent here); ``mel_filterbank`` restates its published algorithm.
@@ -55,6 +57,15 @@ def _support(basis):
     return np.stack([lo, hi], 1).astype(np.int32)
 
 
+def _bin_filters(basis):
+    """[n_bins, 2] int32: first and one-past-last filter that is non-zero at each bin (bins no filter covers -> 0, 0);
+    the rows of the transposed projection the backward kernel sums over."""
+    nz = basis.T != 0
+    lo = np.where(nz.any(1), nz.argmax(1), 0)
+    hi = np.where(nz.any(1), basis.shape[0] - nz[:, ::-1].argmax(1), 0)
+    return np.stack([lo, hi], 1).astype(np.int32)
+
+
 class STFT:
     def __init__(self, sr=22050, n_mels=80, n_fft=1024, win_size=1024, hop_length=256, fmin=20, fmax=11025, clip_val=1e-5):
         self.target_sr = sr
@@ -72,12 +83,13 @@ class STFT:
         key = str(self.fmax) + "_" + str(device)
         if key not in self.mel_basis:
             mel = mel_filterbank(self.target_sr, self.n_fft, self.n_mels, self.fmin, self.fmax)
-            self.mel_basis[key] = (torch.from_numpy(mel).to(device), torch.from_numpy(_support(mel)).to(device))
+            self.mel_basis[key] = (torch.from_numpy(mel).to(device), torch.from_numpy(_support(mel)).to(device),
+                                   torch.from_numpy(_bin_filters(mel)).to(device))
             self.hann_window[key] = torch.hann_window(self.win_size).to(device)
         return self.mel_basis[key] + (self.hann_window[key],)
 
-    def get_mel(self, y, keyshift=0, speed=1, center=False):
-        """y [B, T] CUDA fp32 -> log-mel [B, n_mels, n_frames] (nvSTFT.py:73-117)."""
+    def _checked(self, y, keyshift, speed, center):
+        """the checked (y, B, T, n_frames) of a get_mel call"""
         if keyshift != 0 or speed != 1 or center:
             raise NotImplementedError("the mel kernel covers keyshift=0, speed=1, center=False (the inference call of "
                                       "enhancer.py:113); got keyshift=%r speed=%r center=%r" % (keyshift, speed, center))
@@ -87,16 +99,65 @@ class STFT:
         _need_cuda_f32("y", y)
         if y.dim() != 2:
             raise ValueError("y must be [B, n_samples]")
-        y = y.contiguous()
         B, T = y.shape
-        L = _lib.lib()
-        n_frames = L.b2d_mel_frames(T, self.n_fft, self.win_size, int(self.hop_length))
+        n_frames = _lib.lib().b2d_mel_frames(T, self.n_fft, self.win_size, int(self.hop_length))
         if n_frames <= 0:
             raise ValueError("signal of %d samples is too short for one frame" % T)
-        basis, lohi, window = self._tables(y.device)
+        return y.contiguous(), B, T, n_frames
+
+    def get_mel(self, y, keyshift=0, speed=1, center=False):
+        """y [B, T] CUDA fp32 -> log-mel [B, n_mels, n_frames] (nvSTFT.py:73-117).
+        Differentiable with respect to y when y requires grad and grad mode is on (CUDA backward, get_mel_backward)."""
+        if torch.is_grad_enabled() and isinstance(y, torch.Tensor) and y.requires_grad:
+            self._checked(y, keyshift, speed, center)
+            return _GetMel.apply(self, y)
+        return self._forward(y, keyshift, speed, center)
+
+    def _forward(self, y, keyshift=0, speed=1, center=False):
+        y, B, T, n_frames = self._checked(y, keyshift, speed, center)
+        L = _lib.lib()
+        basis, lohi, _, window = self._tables(y.device)
         out = torch.empty(B, self.n_mels, n_frames, dtype=torch.float32, device=y.device)
         _lib.check(L.b2d_mel_spectrogram(y.data_ptr(), window.data_ptr(), basis.data_ptr(), lohi.data_ptr(), B, T, self.n_fft,
                                          self.win_size, int(self.hop_length), self.n_mels, float(self.clip_val), out.data_ptr(),
                                          _stream()), "b2d_mel_spectrogram")
         _count(1)
         return out
+
+    def get_mel_backward(self, y, grad_mel):
+        """Gradient of get_mel(y) with respect to y for dL/dmel ``grad_mel`` [B, n_mels, n_frames] -> [B, n_samples].
+        grad_mel may be any strided view (e.g. the transpose of a [B, n_frames, n_mels] tensor): it is read through its
+        strides, not copied.  The spectra are recomputed from y, so y must be the forward's input."""
+        y, B, T, n_frames = self._checked(y.detach(), 0, 1, False)
+        _need_cuda_f32("grad_mel", grad_mel)
+        if tuple(grad_mel.shape) != (B, self.n_mels, n_frames):
+            raise ValueError("grad_mel must be [B, n_mels, n_frames] = [%d, %d, %d], got %s"
+                             % (B, self.n_mels, n_frames, tuple(grad_mel.shape)))
+        if grad_mel.device != y.device:
+            raise ValueError("grad_mel lives on %s, y on %s" % (grad_mel.device, y.device))
+        basis, lohi, bins, window = self._tables(y.device)
+        grad = torch.empty(B, T, dtype=torch.float32, device=y.device)
+        sb, sm, sf = grad_mel.stride()
+        _lib.check(_lib.lib().b2d_mel_spectrogram_backward(
+            y.data_ptr(), window.data_ptr(), basis.data_ptr(), lohi.data_ptr(), bins.data_ptr(), B, T, self.n_fft,
+            self.win_size, int(self.hop_length), self.n_mels, float(self.clip_val), grad_mel.data_ptr(), sb, sm, sf,
+            grad.data_ptr(), _stream()), "b2d_mel_spectrogram_backward")
+        _count(1)
+        return grad
+
+
+class _GetMel(torch.autograd.Function):
+    """STFT.get_mel with a CUDA backward.  Saves only y: the backward kernel recomputes the spectra and the mel values
+    (bit-identical to the forward's, so it takes the same clamp decisions)."""
+
+    @staticmethod
+    def forward(ctx, stft, y):
+        ctx.stft = stft
+        ctx.save_for_backward(y)
+        return stft._forward(y)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_mel):
+        (y,) = ctx.saved_tensors
+        return None, ctx.stft.get_mel_backward(y, grad_mel)

@@ -309,6 +309,16 @@ int b2d_u2c_linear_attention(const float* q_features, const float* k_features, c
 int b2d_mel_frames(int n_samples, int n_fft, int win_size, int hop);
 int b2d_mel_spectrogram(const float* audio, const float* window, const float* mel_basis, const int* filter_lohi, int B,
                         int n_samples, int n_fft, int win_size, int hop, int n_mels, float clip_val, float* mel, void* stream);
+/* Backward of b2d_mel_spectrogram with respect to audio (training).  Same audio / tables / shape arguments as the
+ * forward; bin_filter_range [n_fft/2 + 1, 2] (int32, device): first and one-past-last filter that is non-zero at each
+ * bin.  grad_mel = dL/dmel, element (b, mel, frame) at grad_mel[b*grad_stride_b + mel*grad_stride_mel +
+ * frame*grad_stride_frame] (elements), so the transposed [B, n_frames, n_mels] layout is read without a copy.
+ * grad_audio [B, n_samples] is overwritten, deterministically (no atomics).  The mel values are recomputed bit for bit
+ * as the forward computes them, so the clamp (gradient passed where mel_basis @ mag >= clip_val) matches the forward. */
+int b2d_mel_spectrogram_backward(const float* audio, const float* window, const float* mel_basis, const int* filter_lohi,
+                                 const int* bin_filter_range, int B, int n_samples, int n_fft, int win_size, int hop,
+                                 int n_mels, float clip_val, const float* grad_mel, int64_t grad_stride_b,
+                                 int64_t grad_stride_mel, int64_t grad_stride_frame, float* grad_audio, void* stream);
 
 /* b2d_sins_synth variants.  0 (default) = 1 = oscillator-bank kernel next to the impulse-response builds, then the FIR
  * kernel transforms the impulse responses itself.  2 = the bank is evaluated inside the FFT-domain FIR kernel (additionally <= 128 harmonics):
