@@ -102,6 +102,15 @@ SIGNATURES = {
     "b2d_superfast_synth_backward": (ctypes.c_int, [ctypes.c_void_p, c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int64,
                                                     c_f32p, ctypes.c_uint64, ctypes.c_int64, c_f32p, ctypes.c_int,
                                                     ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p, c_stream]),
+    "b2d_rss_table_floats": (ctypes.c_int, [ctypes.c_int]),
+    "b2d_rss_frames": (ctypes.c_int, [ctypes.c_int, ctypes.c_int]),
+    "b2d_rss_loss_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
+    "b2d_rss_loss_forward": (ctypes.c_int, [c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                            ctypes.c_void_p, ctypes.c_float, ctypes.c_float, ctypes.c_void_p,
+                                            ctypes.c_size_t, c_f64p, c_f32p, c_stream]),
+    "b2d_rss_loss_backward": (ctypes.c_int, [c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                             ctypes.c_void_p, ctypes.c_float, ctypes.c_float, c_f64p, c_f32p, c_f32p,
+                                             c_stream]),
 }
 
 _lock = threading.Lock()

@@ -35,6 +35,17 @@ template <int R, int K> __device__ __forceinline__ float2 twid(float2 o) {  // o
     if (4 * K == R) return mul_mj(o);
     if (8 * K == R) return make_float2(0.70710678118654752f * (o.x + o.y), 0.70710678118654752f * (o.y - o.x));
     if (8 * K == 3 * R) return make_float2(0.70710678118654752f * (o.y - o.x), -0.70710678118654752f * (o.x + o.y));
+    if constexpr (R == 32) {
+        // even K: the R = 16 twiddle of K / 2; odd K: (c - j s) * o with c, s = cos, sin(pi K / 16)
+        if constexpr (K % 2 == 0) return twid<16, K / 2>(o);
+        const float c1 = 0.98078528040323044f, s1 = 0.19509032201612826f, c3 = 0.83146961230254524f,
+                    s3 = 0.55557023301960218f;
+        const float c = (K == 1) ? c1 : (K == 3) ? c3 : (K == 5) ? s3 : (K == 7) ? s1 : (K == 9) ? -s1
+                      : (K == 11) ? -s3 : (K == 13) ? -c3 : -c1;
+        const float s = (K == 1) ? s1 : (K == 3) ? s3 : (K == 5) ? c3 : (K == 7) ? c1 : (K == 9) ? c1
+                      : (K == 11) ? c3 : (K == 13) ? s3 : s1;
+        return make_float2(fmaf(o.x, c, o.y * s), fmaf(o.y, c, -o.x * s));
+    }
     // remaining cases: R = 16, K in {1,3,5,7}
     const float c1 = 0.92387953251128674f, s1 = 0.38268343236508977f;
     const float c = (K == 1) ? c1 : (K == 3) ? s1 : (K == 5) ? -s1 : -c1;

@@ -1,6 +1,7 @@
-// N-point complex FFT (N = 1024 or 2048) in shared memory for a 128-thread CTA: three in-place Stockham passes
+// N-point complex FFT (N = 1024, 2048 or 4096) in shared memory for a 128-thread CTA: three in-place Stockham passes
 // (radix 16, R2, 8 with R2 = N/128) over NBATCH independent transforms stored back to back, data padded by one slot
-// per 16 so every pass is bank-conflict free.  Used by combsubfast.cu (N = 1024) and ltv_fir_fft.cu (both sizes).
+// per 16 so every pass is bank-conflict free.  Used by combsubfast.cu (N = 1024), ltv_fir_fft.cu, superfast.cu and
+// mel.cu (1024 / 2048) and rss_loss.cu (all three: the Bluestein transforms).
 // Index formulas pinned by tests/test_csfast_math.py and by the host emulation of both kernels (tests/emu/).
 #pragma once
 #include "fft_regs.cuh"
@@ -13,10 +14,10 @@ constexpr int kThreads = 128;
 __device__ __forceinline__ int padi(int i) { return i + (i >> 4); }   // one pad slot per 16: conflict-free passes
 
 template <int N> struct Plan {
-    static_assert(N == 1024 || N == 2048, "supported sizes");
+    static_assert(N == 1024 || N == 2048 || N == 4096, "supported sizes");
     static constexpr int kN = N;
     static constexpr int kPad = N + N / 16;          // complex slots of one padded FFT buffer
-    static constexpr int kR2 = N / 128;              // radix of the middle pass: 8 (N = 1024) or 16 (N = 2048)
+    static constexpr int kR2 = N / 128;              // radix of the middle pass: 8, 16 or 32 (N = 1024, 2048, 4096)
     static constexpr int kTw2 = (kR2 - 1) * 16;      // exp(-2 pi i r k / (16 R2)), r = 1..R2-1, k < 16
     static constexpr int kTw3 = N / 8;               // exp(-2 pi i k / N), k < N/8
 };

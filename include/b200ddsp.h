@@ -320,6 +320,29 @@ int b2d_mel_spectrogram_backward(const float* audio, const float* window, const 
                                  int n_mels, float clip_val, const float* grad_mel, int64_t grad_stride_b,
                                  int64_t grad_stride_mel, int64_t grad_stride_frame, float* grad_audio, void* stream);
 
+/* ---- random-scale spectral loss (RSSLoss, ddsp/loss.py:9-54; the loss of configs/combsub.yaml and sins.yaml) ------------
+ * Per scale n = n_ffts[s] (host array, 256 <= n <= 2047, n <= n_samples): frames of n samples at hop n (no overlap,
+ * no centering), periodic Hann window w, S = |rfft(w frame)| / sqrt(sum w^2) + eps, and
+ *   loss = sum_s [ mean_b ||S_t - S_p||_F / ||S_t + S_p||_F + alpha mean |log S_t - log S_p| ] / n_scale.
+ * tables: host array of n_scale device pointers, each to the b2d_rss_table_floats(n) floats of that scale (8-byte
+ * aligned; layout in csrc/rss_loss.cu: sqrt(sum w^2), the window, the Bluestein chirp and chirp-filter spectrum, built
+ * in float64 by ddsp_svc_b200.loss.table_host).  b2d_rss_frames(n_samples, n) = 1 + (n_samples - n) / n (0 if none).
+ * Forward: loss [1] fp32 and norms [n_scale, B, 2] float64 (||S_t - S_p||, ||S_t + S_p|| per scale and row) on the
+ * device, through a caller-owned workspace of b2d_rss_loss_workspace_bytes (8-byte aligned); no host synchronisation,
+ * no atomics, the same bits for any launch geometry.  Backward: grad_pred [B, n_samples] = grad_loss[0] * dloss/dx_pred
+ * (overwritten; zero past each scale's last frame) from the forward's norms; the spectra are recomputed from x_pred and
+ * x_true.  Argument errors (null pointers, misalignment, n outside [256, 2047], n_samples < n, B > 65535,
+ * n_scale > 64) return B2D_ERR_* before any device call. */
+int b2d_rss_table_floats(int n);
+int b2d_rss_frames(int n_samples, int n);
+size_t b2d_rss_loss_workspace_bytes(int B, int n_samples, int n_scale, const int* n_ffts);
+int b2d_rss_loss_forward(const float* x_pred, const float* x_true, int B, int n_samples, int n_scale, const int* n_ffts,
+                         const float* const* tables, float alpha, float eps, void* workspace, size_t workspace_bytes,
+                         double* norms, float* loss, void* stream);
+int b2d_rss_loss_backward(const float* x_pred, const float* x_true, int B, int n_samples, int n_scale, const int* n_ffts,
+                          const float* const* tables, float alpha, float eps, const double* norms, const float* grad_loss,
+                          float* grad_pred, void* stream);
+
 /* b2d_sins_synth variants.  0 (default) = 1 = oscillator-bank kernel next to the impulse-response builds, then the FIR
  * kernel transforms the impulse responses itself.  2 = the bank is evaluated inside the FFT-domain FIR kernel (additionally <= 128 harmonics):
  * no [B, T] sinusoid tensor, one launch less, kept as a tested alternative (see api.cu).
