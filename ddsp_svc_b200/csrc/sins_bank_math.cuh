@@ -2,7 +2,9 @@
 // into the FFT-domain FIR kernel): harmonic factoring h = a + 16 b, paired (register-pair) accumulation.  See sins_bank.cu for the
 // derivation; reference ddsp/vocoder.py:580,585-594.
 #pragma once
+#ifndef B2D_HOST_EMU               // tests/emu/ runs sins_bwd.cu on the CPU: only the asm-free helpers below exist there
 #include "b2d_common.cuh"
+#endif
 
 // 1 (default): even anchors by double-angle chains (halves the SFU
 // work of the anchors); 0: every anchor by __sincosf (round-1 code)
@@ -35,6 +37,7 @@ __device__ __forceinline__ int slot_of(int hh) {
     return (g << 7) + ((r & (kNA - 1)) * kNBmax) + (r / kNA);
 }
 
+#ifndef B2D_HOST_EMU
 typedef unsigned long long u64;
 __device__ __forceinline__ u64 pack2(float lo, float hi) { u64 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
 __device__ __forceinline__ void unpack2(u64 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
@@ -138,6 +141,7 @@ __device__ __forceinline__ void bank_group(const float* __restrict__ arow, const
         }
     }
 }
+#endif  // B2D_HOST_EMU
 
 
 // activated amplitude of 0-based harmonic hh at a frame with pitch f0:  exp(c)/128 * (1[f0 (hh+1) < sr/2] + 1e-7)

@@ -191,12 +191,135 @@ def ltv_fir(x, ir, block, seed=0, utterance_offset=0, generic=False):
     return y
 
 
+SINS_GRAD_MAX_MAG, SINS_GRAD_MAX_HARMONICS = 257, 512
+
+
+def sins_grad_unsupported(block, n_harmonics, n_mag_allpass, n_mag_noise):
+    """None if sins_synth_backward covers the shape, else why not."""
+    if int(block) != 512:
+        return "block size %d (the backward is built for 512)" % block
+    if max(n_mag_allpass, n_mag_noise) > SINS_GRAD_MAX_MAG:
+        return "n_mag %d / %d (the backward is built for <= %d)" % (n_mag_allpass, n_mag_noise, SINS_GRAD_MAX_MAG)
+    if n_harmonics > SINS_GRAD_MAX_HARMONICS:
+        return "%d harmonics (the backward is built for <= %d)" % (n_harmonics, SINS_GRAD_MAX_HARMONICS)
+    return None
+
+
 def sins_synth(f0_frames, frame_phase, c_amp, c_group_delay, c_noise, block, sampling_rate, noise_in=None,
                seed=0, utterance_offset=0, infer=True, want_parts=True, signal_out=None):
     """Whole Sins DSP after Unit2Control -> (signal, harmonic, noise) [B, T] each.
     ``signal_out``: optional preallocated [B, T] fp32 CUDA tensor for the mixed signal; it may live in
     another GPU's memory (peer-mapped, see sharding.PeerGather): the FIR kernel then writes the
-    waveform straight over NVLink."""
+    waveform straight over NVLink.
+
+    Differentiable with respect to the three controls when one of them requires grad (and grad mode is on), in the
+    training phase (``infer=False``, frame_phase from phase_scan(..., infer=False)): the backward runs
+    sins_synth_backward with the forward's workspace, noise and seed.  All three outputs are differentiable."""
+    ctrls = (c_amp, c_group_delay, c_noise)
+    if torch.is_grad_enabled() and any(isinstance(c, torch.Tensor) and c.requires_grad for c in ctrls):
+        if signal_out is not None:
+            raise ValueError("signal_out cannot be used when the controls require grad (it may be peer-mapped memory "
+                             "that autograd does not own)")
+        if infer:
+            raise NotImplementedError("the Sins backward covers the training phase only: call with infer=False (what "
+                                      "the reference's solver.py does), or under torch.no_grad() for inference")
+        if isinstance(f0_frames, torch.Tensor) and f0_frames.requires_grad:
+            raise NotImplementedError("Sins has no gradient with respect to f0_frames; pass f0 as data")
+        why = sins_grad_unsupported(block, c_amp.shape[-1], c_group_delay.shape[-1], c_noise.shape[-1])
+        if why is not None:
+            raise NotImplementedError("the Sins backward does not cover " + why)
+        if noise_in is not None:
+            noise_in = noise_in.detach()
+        return _SinsSynth.apply(f0_frames.detach(), frame_phase, int(block), float(sampling_rate), noise_in, int(seed),
+                                int(utterance_offset), c_amp, c_group_delay, c_noise)
+    return _sins_synth(f0_frames, frame_phase, c_amp, c_group_delay, c_noise, block, sampling_rate, noise_in, seed,
+                       utterance_offset, infer, want_parts, signal_out)[:3]
+
+
+def _sins_args(f0_frames, frame_phase, c_amp, c_group_delay, c_noise, block, noise_in):
+    """checked (f0 [B, nF], controls sharing one frame stride, the stride, noise rows) of a Sins call"""
+    f0 = _frames_2d(f0_frames)
+    B, nF = f0.shape
+    _need_frame_phase(frame_phase, B, nF)
+    ca, s0 = _ctrl_view("amplitudes", c_amp, B, nF)
+    cg, s1 = _ctrl_view("group_delay", c_group_delay, B, nF)
+    cn, s2 = _ctrl_view("noise_magnitude", c_noise, B, nF)
+    if not (s0 == s1 == s2):  # views of different tensors: densify so one stride describes all
+        ca, cg, cn = ca.contiguous(), cg.contiguous(), cn.contiguous()
+        dense = torch.cat((ca, cg, cn), dim=-1)
+        ca, cg, cn = torch.split(dense, [ca.shape[2], cg.shape[2], cn.shape[2]], dim=-1)
+        s0 = dense.stride(1)
+    if noise_in is not None:
+        noise_in = _noise_rows(noise_in, B, nF * int(block))
+    return f0, ca, cg, cn, s0, noise_in
+
+
+def sins_synth_backward(f0_frames, frame_phase, c_amp, c_group_delay, c_noise, ws, grad_signal, block, sampling_rate,
+                        grad_harmonic=None, grad_noise=None, noise_in=None, seed=0, utterance_offset=0,
+                        ws_has_sinusoids=True):
+    """Gradient of sins_synth (infer=False) with respect to the three raw controls, for the cotangents of signal,
+    harmonic and noise [B, T] (None = zero).  f0 / frame_phase / controls / noise_in / seed / utterance_offset must be
+    those of the forward call and ``ws`` the workspace it filled (its impulse responses, and its sinusoids unless
+    ``ws_has_sinusoids`` is False: the 'fused' variant does not store them and the bank is rerun).
+    -> dense [B, nF, H + Ma + Mn]: amplitudes | group_delay | noise_magnitude (the split_to_dict layout)."""
+    f0, ca, cg, cn, stride, noise_in = _sins_args(f0_frames, frame_phase, c_amp, c_group_delay, c_noise, block, noise_in)
+    B, nF = f0.shape
+    H, Ma, Mn = ca.shape[2], cg.shape[2], cn.shape[2]
+    T = nF * int(block)
+    L = _lib.lib()
+    if not isinstance(ws, torch.Tensor) or not ws.is_cuda or ws.dtype != torch.uint8 or \
+            ws.numel() < L.b2d_sins_workspace_bytes(B, nF, int(block), Ma, Mn):
+        raise ValueError("ws must be the workspace sins_synth filled for the same shapes")
+    cots = []
+    for name, g in (("grad_signal", grad_signal), ("grad_harmonic", grad_harmonic), ("grad_noise", grad_noise)):
+        if g is not None:
+            _need_cuda_f32(name, g)
+            if tuple(g.shape) != (B, T):
+                raise ValueError("%s must be [B, n_frames*block] = [%d, %d], got %s" % (name, B, T, tuple(g.shape)))
+            g = g.contiguous()
+        cots.append(g)
+    grad = torch.empty(B, nF, H + Ma + Mn, dtype=torch.float32, device=f0.device)
+    bws_bytes = L.b2d_sins_synth_backward_workspace_bytes(B, nF, int(block))
+    bws = torch.empty(bws_bytes, dtype=torch.uint8, device=f0.device)
+    rc = L.b2d_sins_synth_backward(f0.data_ptr(), frame_phase.data_ptr(), ca.data_ptr(), cg.data_ptr(), cn.data_ptr(),
+                                   stride, _ptr(noise_in), int(seed), int(utterance_offset), ws.data_ptr(),
+                                   1 if ws_has_sinusoids else 0, _ptr(cots[0]), _ptr(cots[1]), _ptr(cots[2]), B, nF,
+                                   int(block), H, Ma, Mn, float(sampling_rate), grad.data_ptr(), bws.data_ptr(),
+                                   bws_bytes, _stream())
+    _lib.check(rc, "b2d_sins_synth_backward")
+    _count(2 if ws_has_sinusoids else 3)
+    return grad
+
+
+class _SinsSynth(torch.autograd.Function):
+    """sins_synth (infer=False) with a CUDA backward.  Saves the forward's workspace (sinusoids | impulse responses),
+    f0, frame_phase, the control views and the noise input; the backward regenerates the in-kernel noise from seed."""
+
+    @staticmethod
+    def forward(ctx, f0, frame_phase, block, sampling_rate, noise_in, seed, utterance_offset, c_amp, c_gd, c_nm):
+        signal, harmonic, noise, ws = _sins_synth(f0, frame_phase, c_amp, c_gd, c_nm, block, sampling_rate, noise_in,
+                                                  seed, utterance_offset, False, True, None)
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(ws, f0, frame_phase, noise_in, c_amp, c_gd, c_nm)
+        # the 'fused' variant evaluates the bank inside its FIR kernel and leaves the sinusoid slot unwritten
+        ctx.cfg = (block, sampling_rate, seed, utterance_offset, _sins_impl != "fused")
+        return signal, harmonic, noise
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_signal, grad_harmonic, grad_noise):
+        ws, f0, frame_phase, noise_in, c_amp, c_gd, c_nm = ctx.saved_tensors
+        block, sampling_rate, seed, utterance_offset, has_sinusoids = ctx.cfg
+        grad = sins_synth_backward(f0, frame_phase, c_amp, c_gd, c_nm, ws, grad_signal, block, sampling_rate,
+                                   grad_harmonic=grad_harmonic, grad_noise=grad_noise, noise_in=noise_in, seed=seed,
+                                   utterance_offset=utterance_offset, ws_has_sinusoids=has_sinusoids)
+        parts = torch.split(grad, [c_amp.shape[-1], c_gd.shape[-1], c_nm.shape[-1]], dim=-1)
+        return (None,) * 7 + tuple(parts)
+
+
+def _sins_synth(f0_frames, frame_phase, c_amp, c_group_delay, c_noise, block, sampling_rate, noise_in=None,
+                seed=0, utterance_offset=0, infer=True, want_parts=True, signal_out=None):
+    """-> (signal, harmonic, noise, workspace)"""
     f0 = _frames_2d(f0_frames)
     B, nF = f0.shape
     _need_frame_phase(frame_phase, B, nF)
@@ -236,7 +359,7 @@ def sins_synth(f0_frames, frame_phase, c_amp, c_group_delay, c_noise, block, sam
     spectrum = _sins_impl == "spectrum" and fft_ok
     nsplit = max(1, min(abs(_overlap_mode), B)) if abs(_overlap_mode) >= 2 else 1
     _count(3 if fused else 5 if spectrum else 2 + nsplit * (2 if Ma == Mn else 3))
-    return signal, harmonic, noise
+    return signal, harmonic, noise, ws
 
 
 def sinegen(f0, upp, sampling_rate, dim, rand_ini, sine_amp=0.1, noise_std=0.003, voiced_threshold=0.0,

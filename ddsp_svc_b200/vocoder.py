@@ -84,12 +84,31 @@ class Sins(_SynthBase):
                 infer=True, max_upsample_dim=32, noise=None, utterance_offset=0, signal_out=None):
         """units_frames B x n_frames x n_unit; f0_frames B x n_frames x 1; volume_frames B x n_frames x 1.
         ``max_upsample_dim`` only chunks the reference's temporaries and has no effect here.
-        ``signal_out``: optional preallocated [B, T] destination of ``signal`` (may be peer-mapped memory)."""
+        ``signal_out``: optional preallocated [B, T] destination of ``signal`` (may be peer-mapped memory).
+
+        Trainable in the training phase: with ``infer=False`` (what the reference's solver.py calls) and a control
+        from ``unit2ctrl`` that requires grad (grad mode on), signal, harmonic and noise are differentiable with
+        respect to the three controls (CUDA backward, ops.sins_synth_backward) for block 512, n_mag <= 257 and up
+        to 512 harmonics.  f0 is data, as in the reference's train.py: an f0 that requires grad is refused."""
         sr, block = self._scalars()
+        if torch.is_grad_enabled() and isinstance(f0_frames, torch.Tensor) and f0_frames.requires_grad:
+            raise NotImplementedError("Sins has no gradient with respect to f0_frames; pass f0 as data "
+                                      "(f0_frames.detach()), as the reference's train.py does")
         frame_phase, phase_frames = ops.phase_scan(f0_frames, block, sr, initial_phase, infer)
         ctrls, hidden = self.unit2ctrl(units_frames, f0_frames, phase_frames, volume_frames, spk_id=spk_id,
                                        spk_mix_dict=spk_mix_dict)
-        self._forward_only(ctrls)
+        if torch.is_grad_enabled() and any(v.requires_grad for v in ctrls.values()):
+            if infer:
+                raise NotImplementedError(
+                    "Sins is differentiable in the training phase only: call it with infer=False (what the "
+                    "reference's solver.py does), or under torch.no_grad() for inference (main.py:250)")
+            if signal_out is not None:
+                raise ValueError("signal_out cannot be combined with controls that require grad; call under "
+                                 "torch.no_grad() or drop signal_out")
+            why = ops.sins_grad_unsupported(block, ctrls["amplitudes"].shape[-1], ctrls["group_delay"].shape[-1],
+                                            ctrls["noise_magnitude"].shape[-1])
+            if why is not None:
+                raise NotImplementedError("the Sins backward does not cover " + why)
         signal, harmonic, noise_out = ops.sins_synth(
             f0_frames, frame_phase, ctrls["amplitudes"], ctrls["group_delay"], ctrls["noise_magnitude"], block, sr,
             noise_in=noise, seed=0 if noise is not None else _host_seed(), utterance_offset=utterance_offset,

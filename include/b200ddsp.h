@@ -153,8 +153,30 @@ int    b2d_sins_synth(const float* f0_frames, const double* frame_phase,
                       float* signal, float* harmonic, float* noise_out,
                       void* workspace, size_t workspace_bytes, void* stream);
 
+/* Backward of b2d_sins_synth in the training phase (round_fp32 = 1, infer=False) with respect to
+ * the three raw controls.                            ddsp/vocoder.py:580-611 under autograd
+ * grad_ctrl: dense [B, n_frames, H + Ma + Mn] = amplitudes | group_delay | noise_magnitude (the
+ * split_to_dict layout), every element written.  grad_signal / grad_harmonic / grad_noise: [B, T]
+ * cotangents of the three outputs, NULL = zero.  forward_workspace: what b2d_sins_synth filled
+ * for the same arguments (its impulse responses, and its sinusoids unless
+ * forward_has_sinusoids = 0: the fused variant, b2d_set_sins_impl(2), does not store them and the
+ * bank is rerun into `workspace`).  f0_frames, frame_phase, controls, noise_in, seed and
+ * utterance_offset: those of the forward call (the in-kernel noise is regenerated).  Built for
+ * block 512, 2 <= n_mag <= 257, H <= 512.  Deterministic: no atomics; the result depends neither
+ * on the grid nor on b2d_set_overlap / b2d_set_sins_impl. */
+size_t b2d_sins_synth_backward_workspace_bytes(int B, int n_frames, int block);
+int    b2d_sins_synth_backward(const float* f0_frames, const double* frame_phase, const float* c_amp,
+                               const float* c_group_delay, const float* c_noise, int64_t ctrl_stride,
+                               const float* noise_in, uint64_t seed, int64_t utterance_offset,
+                               const void* forward_workspace, int forward_has_sinusoids,
+                               const float* grad_signal, const float* grad_harmonic,
+                               const float* grad_noise, int B, int n_frames, int block,
+                               int n_harmonics, int n_mag_allpass, int n_mag_noise,
+                               double sampling_rate, float* grad_ctrl, void* workspace,
+                               size_t workspace_bytes, void* stream);
+
 /* ---------------------------------------------------------------------------------------
- * NSF-HiFiGAN SineGen f0 excitation.                 replaces nsf_hifigan/models.py:134-165
+ * NSF-HiFiGAN SineGen f0 excitation.                replaces nsf_hifigan/models.py:134-165
  * (SineGen._f02sine + forward).  f0 [B, n_frames] (Hz, 0 = unvoiced), piecewise constant per
  * frame of `upp` samples; out [B, n_frames*upp, dim], dim = harmonic_num + 1 <= 16.
  * rand_ini [dim]: the random initial phases in cycles (element 0 = 0), drawn by the caller
