@@ -23,6 +23,9 @@ constexpr int kLaD = 64;                 // dim_head of the reference's SelfAtte
 constexpr int kLaJmax = 272;             // features padded to a multiple of 8 (266 = int(64 ln 64))
 constexpr int kLaTT = 16;                // frames per tile
 constexpr int kLaThreads = 288;          // 272 compute threads of phase A (34 feature groups x 8 channel groups) + 16 loaders
+// phase A sums 64 frames in registers, then adds them to the totals in shared memory: one fp32 chain over all T frames
+// had 7x the error of the library path (kf.sum + fp32 GEMM) at T = 5168, J = 8; two chains of about sqrt(T) do not
+constexpr int kLaFlushTiles = 4;
 
 struct LinAttnParams {
     const float* qf;       // [BH, T, J]
@@ -56,7 +59,15 @@ __global__ void __launch_bounds__(kLaThreads, 2) u2c_linear_attention_kernel(Lin
 #pragma unroll
         for (int c = 0; c < 8; ++c) acc[a][c] = 0.f;
     }
-    for (int t0 = 0; t0 < T; t0 += kLaTT) {
+    if (tid < 272) {                                        // each thread owns its 8 x 8 block of the totals
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) ctx[(8 * jg + i) * kLaD + 8 * dg + k] = 0.f;
+            if (dg == 0) ksum[8 * jg + i] = 0.f;
+        }
+    }
+    for (int t0 = 0, tile = 1; t0 < T; t0 += kLaTT, ++tile) {
         for (int i = tid; i < kLaTT * kLaJmax; i += kLaThreads) {
             const int tt = i / kLaJmax, j = i - tt * kLaJmax;
             ftile[i] = (t0 + tt < T && j < J) ? kf[(size_t)(t0 + tt) * J + j] : 0.f;
@@ -79,18 +90,18 @@ __global__ void __launch_bounds__(kLaThreads, 2) u2c_linear_attention_kernel(Lin
                     for (int k = 0; k < 8; ++k) acc[i][k] = fmaf(a[i], c[k], acc[i][k]);
                 }
             }
+            if (tile % kLaFlushTiles == 0 || t0 + kLaTT >= T) {
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+#pragma unroll
+                    for (int k = 0; k < 8; ++k) { ctx[(8 * jg + i) * kLaD + 8 * dg + k] += acc[i][k]; acc[i][k] = 0.f; }
+                    if (dg == 0) ksum[8 * jg + i] += ks[i];
+                    ks[i] = 0.f;
+                }
+            }
         }
         __syncthreads();
     }
-    if (tid < 272) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-#pragma unroll
-            for (int k = 0; k < 8; ++k) ctx[(8 * jg + i) * kLaD + 8 * dg + k] = acc[i][k];
-            if (dg == 0) ksum[8 * jg + i] = ks[i];
-        }
-    }
-    __syncthreads();
 
     // ---- phase B: out[t] = (q'[t] . context) / (q'[t] . k_sum + eps) ----
     const int b = bh / p.H, h = bh - b * p.H;

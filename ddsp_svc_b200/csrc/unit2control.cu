@@ -68,11 +68,13 @@ __global__ void __launch_bounds__(256) u2c_gn_apply_kernel(float* __restrict__ x
     const double n = (double)cpg * (double)T;
     const double mean = stats[((size_t)b * G + g) * 2] / n;
     const double var = fmax(stats[((size_t)b * G + g) * 2 + 1] / n - mean * mean, 0.0);
-    const float rstd = (float)(1.0 / sqrt(var + (double)eps)), mu = (float)mean;
+    // the mean as an unevaluated fp32 pair: rounding it to one float would shift a group whose mean is large against its
+    // spread by up to half an ulp of the mean (mean / std = 1e3: 3e-5 std)
+    const float rstd = (float)(1.0 / sqrt(var + (double)eps)), mu = (float)mean, mu_lo = (float)(mean - (double)mu);
     const float ga = gamma[c], be = beta[c];
     for (int t = blockIdx.x; t < T; t += gridDim.x) {
         const size_t i = ((size_t)b * T + t) * C + c;
-        float v = (x[i] - mu) * rstd * ga + be;
+        float v = ((x[i] - mu) - mu_lo) * rstd * ga + be;
         x[i] = v >= 0.f ? v : v * slope;
     }
 }
@@ -164,10 +166,18 @@ __global__ void __launch_bounds__(256) u2c_softmax_feat_kernel(float* __restrict
 
 // ---- fp32 -> (tf32 hi, tf32 lo) split for 3xTF32 library GEMMs: x = hi + lo + O(2^-22 |x|), both parts exactly
 // representable in TF32 (10-bit mantissa, round to nearest even on the dropped 13 bits) ----
+// A NaN becomes the TF32 quiet NaN 0x7FFFE000: the rounding add would carry the low payload bits of a NaN into the
+// exponent and sign (the canonical NaN 0x7FFFFFFF that device arithmetic produces came out as -0).  +-inf split into
+// (+-inf, +0).  Finite values above the largest TF32 value round to hi = +-inf, lo = -+inf.
 __device__ __forceinline__ float tf32_rn(float x) {
     uint32_t u = __float_as_uint(x);
+    if ((u & 0x7FFFFFFFu) > 0x7F800000u) return __uint_as_float(0x7FFFE000u);
     u += 0x00000FFFu + ((u >> 13) & 1u);
     return __uint_as_float(u & 0xFFFFE000u);
+}
+__device__ __forceinline__ void tf32_split(float v, float& h, float& l) {
+    h = tf32_rn(v);
+    l = tf32_rn(v == h ? 0.f : v - h);              // v == h also for +-inf, where v - h would be NaN
 }
 __global__ void __launch_bounds__(256) u2c_split_tf32_kernel(const float4* __restrict__ x, float4* __restrict__ hi, float4* __restrict__ lo,
                                                              size_t n4, const float* __restrict__ xt, float* __restrict__ hit,
@@ -175,13 +185,13 @@ __global__ void __launch_bounds__(256) u2c_split_tf32_kernel(const float4* __res
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
         const float4 v = x[i];
         float4 h, l;
-        h.x = tf32_rn(v.x); h.y = tf32_rn(v.y); h.z = tf32_rn(v.z); h.w = tf32_rn(v.w);
-        l.x = tf32_rn(v.x - h.x); l.y = tf32_rn(v.y - h.y); l.z = tf32_rn(v.z - h.z); l.w = tf32_rn(v.w - h.w);
+        tf32_split(v.x, h.x, l.x); tf32_split(v.y, h.y, l.y); tf32_split(v.z, h.z, l.z); tf32_split(v.w, h.w, l.w);
         hi[i] = h; lo[i] = l;
     }
     if (blockIdx.x == 0 && (int)threadIdx.x < tail) {
-        const float v = xt[threadIdx.x], h = tf32_rn(v);
-        hit[threadIdx.x] = h; lot[threadIdx.x] = tf32_rn(v - h);
+        float h, l;
+        tf32_split(xt[threadIdx.x], h, l);
+        hit[threadIdx.x] = h; lot[threadIdx.x] = l;
     }
 }
 

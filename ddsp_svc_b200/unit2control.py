@@ -131,11 +131,13 @@ class _Gemm:
     """The library GEMMs of the control network at one of three precisions.
 
     * ``"3xtf32"`` (default): every product runs as THREE tensor-core GEMMs on TF32-exact operand halves, a_hi b_hi +
-      a_lo b_hi + a_hi b_lo with fp32 accumulation -- fp32-grade results (measured 5e-7 relative on the controls, like the
-      SIMT fp32 GEMM) at tensor-core speed; the halves come from b2d_split_tf32 (weights: once per checkpoint).
+      a_lo b_hi + a_hi b_lo with fp32 accumulation -- near-fp32 results at tensor-core speed (against float64: up to
+      2.2e-6 relative RMS on the controls, the SIMT fp32 GEMMs 4.6e-7; the tensor cores' accumulators truncate; measured
+      on an H100 SXM at 700 W); the halves come from b2d_split_tf32 (weights: once per checkpoint).
     * ``"fp32"``: cuBLAS SIMT fp32 GEMMs (what the reference's Linear layers run on a GPU).
-    * ``"tf32"``: one TF32 pass (1e-3 relative per product, 3e-4 on the controls; the reference's cuDNN convolutions do
-      this under torch's defaults and land at 1.4e-4).
+    * ``"tf32"``: one TF32 pass (1e-3 relative per product, under 4e-4 relative RMS on the controls: 3.0e-4 to 3.4e-4
+      measured on an H100 SXM at 700 W; the reference's cuDNN convolutions do this under torch's defaults and land at
+      1.4e-4).  A single token (B T = 1) runs as matrix-vector products without TF32.
     The TF32 modes flip torch.backends.cuda.matmul.allow_tf32 around their own calls only."""
 
     def __init__(self, mode):

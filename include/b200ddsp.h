@@ -305,7 +305,9 @@ int b2d_cross_fade(const float* a, int64_t len_a, const float* b, int64_t len_b,
  *   [rows, n_features] with data [rows, dim_head]: query rows ratio (exp(p - diag - rowmax) + eps), key rows
  *   ratio exp(p - diag + eps), diag = |data|^2 / (2 sqrt(d)), ratio = n_features^-1/2. */
 /* x [n] -> hi, lo [n]: x = hi + lo up to 2^-22 |x| with both parts exactly representable in TF32 (round to nearest even);
- * the operand preparation of 3xTF32 GEMMs (hi hi + lo hi + hi lo on the tensor cores = fp32-grade products). */
+ * the operand preparation of 3xTF32 GEMMs (hi hi + lo hi + hi lo on the tensor cores = fp32-grade products).
+ * A NaN gives the TF32 quiet NaN in both parts, +-inf gives (+-inf, +0); finite values at or above (2 - 2^-11) 2^127
+ * round to hi = +-inf, lo = -+inf. */
 int b2d_split_tf32(const float* x, float* hi, float* lo, size_t n, void* stream);
 int b2d_u2c_embed(float* x, const float* f0, const float* phase, const float* volume, const float* embed_table,
                   const float* spk, int spk_rows, const float* aug_shift, int B, int T, void* stream);

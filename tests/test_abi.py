@@ -54,6 +54,20 @@ def test_argument_errors_do_not_touch_the_device(lib):
     assert lib.b2d_dft_tables_bytes(256) == 2 * 256 * 128 * 4 + 16 * 8 * 128 * 8 * 4   # CUDA-core tables + tensor-core image
     assert lib.b2d_sins_synth(16, 16, 16, 16, 16, 640, 0, 0, 0, 16, 16, 1, 1, 512, 128, 256, 256, 44100.0, 0,
                               16, 16, 16, 256, 10, 0) == -5                                  # workspace too small
+    # the control network's kernels (unit2control.cu, linear_attention.cu); p: a non-null, 16-byte aligned address
+    p = 16
+    for C in (0, 33, 1056):                                                                  # C % 32, C > 1024
+        assert lib.b2d_u2c_layernorm(p, p, 4, C, p, p, 1e-5, 0) == -2
+    for B, C, groups in ((1, 128, 4), (1, 256, 3), (65536, 256, 4)):                         # C != 256, C % groups, grid.y
+        assert lib.b2d_u2c_groupnorm_lrelu(p, B, 8, C, groups, p, p, 1e-5, 0.01, p, 0) == -2
+    for B, inner, k in ((1, 256, 29), (1, 100, 31), (65536, 256, 31)):                       # k != 31, inner % 128, grid.z
+        assert lib.b2d_u2c_glu_dwconv_silu(p, p, p, p, B, 8, inner, k, 0) == -2
+    assert lib.b2d_u2c_softmax_features(p, p, 0, 266, 64, 1, 1e-4, 0) == -2
+    assert lib.b2d_u2c_linear_attention(p, p, p, p, 1, 8, 16, 266, 32, 1e-8, 0) == -4         # dim_head != 64
+    assert lib.b2d_u2c_linear_attention(p, p, p, p, 1, 8, 16, 273, 64, 1e-8, 0) == -4         # > 272 features
+    assert lib.b2d_split_tf32(p + 4, p, p, 8, 0) == -3                                        # misaligned x
+    assert lib.b2d_split_tf32(p, p, p, 0, 0) == 0                                             # nothing to do
+    assert lib.b2d_u2c_embed(p, p, p, p, p, p, 2, 0, 3, 10, 0) == -2                          # spk_rows not 1 or B
 
 
 def test_ops_refuse_cpu_tensors():
