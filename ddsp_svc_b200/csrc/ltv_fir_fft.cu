@@ -14,7 +14,7 @@
 //     Y_g + j Y_{g+1} returns both.  Only signals of the SAME job are ever paired in one transform, so the fp32
 //     round-off of a loud channel (harmonic) never leaks into a quiet one (filtered noise);
 //   * all forward transforms of a pair (2 inputs + 1 impulse-response pair per job) run as one batch through the
-//     shared-memory Stockham passes of fft_smem.cuh, then all inverse transforms as a second batch;
+//     in-place passes below (three block barriers per batch), then all inverse transforms as a second batch;
 //   * every 1021-sample output segment is overlap-added into a 4-hop ring per job at its delay-compensated position;
 //     a hop is complete once the segment of the FOLLOWING input hop has been added and is then written exactly once
 //     (y1, y2 and mix = y1 + y2 (+ addend)) with 128-bit stores -- deterministic, no atomics.
@@ -72,12 +72,156 @@ struct FftFirParams {
 };
 
 constexpr int kBankRow = 128;            // harmonics per activated amplitude row of the BANK variant (H <= 128)
+// ---- the kernel's N-point transform: in-place mixed radix (16, N/128, 8) over a batch of padded buffers ----
+// Forward = decimation in frequency: natural order in, bin k out at position binpos(k) (digit-reversed).  The transposed
+// network (passes in reverse order, twiddles before the butterflies) is again a forward DFT, one that reads that order
+// and writes natural order, so the pointwise step runs in place between the two and nothing is ever permuted.  Every
+// butterfly writes back the slots it read, so each pass needs ONE block barrier, whatever the batch size (the
+// Stockham passes of fft_smem.cuh need one per stage of one or two transforms), and only one butterfly is live per
+// thread.  Buffers keep the padding of fft_smem.cuh (slot padi(n)): the slots of a butterfly are the slot of its first
+// element plus constants (immediate offsets, no per-element index registers), and with the block order of pass 2 and
+// the bin ownership of the pointwise step (own_pos) every half warp hits 16 different bank pairs.
+template <int N> struct Ct {
+    static_assert(N == 1024 || N == 2048, "supported sizes");
+    static constexpr int kM = N / 16;                // span of pass 1
+    static constexpr int kR2 = N / 128;              // radix of pass 2 (span 8)
+    static constexpr int kTw1 = 8 * kM;              // W_N^(j q) at [(q-1) kM + j], q = 1..8, j < kM (q > 8: times W_N^(8 j))
+    static constexpr int kTw2 = 8 * (kR2 - 1);       // W_kM^(j q) at [(q-1) 8 + j], q = 1..kR2-1, j < 8
+};
+// position of bin k = q + 16 q2 + (N/8) m3 after the forward transform, and its inverse
+template <int N> __device__ __forceinline__ int binpos(int k) {
+    return (N / 16) * (k & 15) + 8 * ((k >> 4) & (N / 128 - 1)) + k / (N / 8);
+}
+template <int N> __device__ __forceinline__ int bin_at(int pos) {
+    return pos / (N / 16) + 16 * ((pos >> 3) & (N / 128 - 1)) + (N / 8) * (pos & 7);
+}
+// bins of the pointwise step owned by thread tid: positions 8 (tid + 128 v) + u, u < 4 -- exactly the bins below N/2
+// (m3 < 4), consecutive slots across a half warp
+__device__ __forceinline__ int own_pos(int tid, int i) { return 8 * (tid + kThreads * (i >> 2)) + (i & 3); }
+
+template <int N> __device__ __forceinline__ void ct_twiddles(float2* tw1, float2* tw2, int tid) {
+    constexpr int M = Ct<N>::kM;
+    for (int i = tid; i < Ct<N>::kTw1; i += kThreads) {
+        const int q = i / M + 1, j = i % M;
+        float sn, cs; sincospif(-2.0f * (float)(j * q) / (float)N, &sn, &cs);
+        tw1[i] = make_float2(cs, sn);
+    }
+    for (int i = tid; i < Ct<N>::kTw2; i += kThreads) {
+        const int q = i / 8 + 1, j = i % 8;
+        float sn, cs; sincospif(-2.0f * (float)(j * q) / (float)M, &sn, &cs);
+        tw2[i] = make_float2(cs, sn);
+    }
+}
+
+// W_N^(j q), q = 1..15, of pass 1 (w = tw1 + j)
+template <int N> __device__ __forceinline__ float2 tw_pass1(const float2* w, int q) {
+    constexpr int M = Ct<N>::kM;
+    return q <= 8 ? w[(q - 1) * M] : cmul(w[(q - 9) * M], w[7 * M]);
+}
+
+// pass 1: radix 16 over {j + M r}.  FWD: butterfly, then output q times W_N^(j q); transposed: input r times W_N^(j r),
+// then butterfly.  ZU (forward only): the upper half of every transform is zero and is not read.
+template <int N, int NB, bool FWD, bool ZU, bool PK>
+__device__ __forceinline__ void ct_pass1(float2* F, const float2* tw1, int tid) {
+    constexpr int M = Ct<N>::kM, TPJ = kThreads / M, kPad = Plan<N>::kPad;   // TPJ transforms side by side
+    const int j = tid % M;
+    const float2* w = tw1 + j;
+#pragma unroll 1
+    for (int u = 0; u < (NB + TPJ - 1) / TPJ; ++u) {
+        const int t = tid / M + TPJ * u;
+        if (t >= NB) break;
+        float2* x = F + t * kPad + padi(j);                     // element r at x[r (M + M/16)]
+        float2 v[16];
+        if (FWD) {
+#pragma unroll
+            for (int r = 0; r < (ZU ? 8 : 16); ++r) v[r] = x[r * (M + M / 16)];
+            if (ZU) Dft16ZeroUpper<PK>::run(v);
+            else Dft<16, PK>::run(v);
+#pragma unroll
+            for (int q = 1; q < 16; ++q) v[q] = cmul(v[q], tw_pass1<N>(w, q));
+        } else {
+            v[0] = x[0];
+#pragma unroll
+            for (int r = 1; r < 16; ++r) v[r] = cmul(x[r * (M + M / 16)], tw_pass1<N>(w, r));
+            Dft<16, PK>::run(v);
+        }
+#pragma unroll
+        for (int q = 0; q < 16; ++q) x[q * (M + M / 16)] = v[q];
+    }
+}
+
+// pass 2: radix R2 over {M q + j + 8 r} inside each of the 16 blocks of pass 1, twiddles W_M^(j r).  For N = 1024 the
+// two 8-lane groups of a half warp take blocks two apart (bits 0 and 1 of the block index swapped): their slots are
+// then 8 banks pairs apart, as they are for neighbouring blocks when N = 2048.
+template <int N, int NB, bool FWD, bool PK>
+__device__ __forceinline__ void ct_pass2(float2* F, const float2* tw2, int tid) {
+    constexpr int M = Ct<N>::kM, R2 = Ct<N>::kR2, kPad = Plan<N>::kPad;
+    const int j = tid & 7, b = tid >> 3;
+    const int q = N == 1024 ? ((b & ~3) | ((b & 1) << 1) | ((b >> 1) & 1)) : b;
+    const float2* w = tw2 + j;
+#pragma unroll 1
+    for (int t = 0; t < NB; ++t) {
+        float2* x = F + t * kPad + padi(M * q + j);            // element r at x[8 r + r / 2]
+        float2 v[R2];
+        v[0] = x[0];
+#pragma unroll
+        for (int r = 1; r < R2; ++r) {
+            v[r] = x[8 * r + r / 2];
+            if (!FWD) v[r] = cmul(v[r], w[(r - 1) * 8]);
+        }
+        Dft<R2, PK>::run(v);
+        if (FWD) {
+#pragma unroll
+            for (int r = 1; r < R2; ++r) v[r] = cmul(v[r], w[(r - 1) * 8]);
+        }
+#pragma unroll
+        for (int r = 0; r < R2; ++r) x[8 * r + r / 2] = v[r];
+    }
+}
+
+// pass 3: radix 8 over 8 consecutive positions, no twiddles (its own transpose)
+template <int N, int NB, bool PK>
+__device__ __forceinline__ void ct_pass3(float2* F, int tid) {
+    constexpr int kPad = Plan<N>::kPad;
+#pragma unroll 1
+    for (int i = tid; i < NB * (N / 8); i += kThreads) {
+        float2* x = F + (i / (N / 8)) * kPad + padi(8 * (i % (N / 8)));
+        float2 v[8];
+#pragma unroll
+        for (int r = 0; r < 8; ++r) v[r] = x[r];
+        Dft<8, PK>::run(v);
+#pragma unroll
+        for (int r = 0; r < 8; ++r) x[r] = v[r];
+    }
+}
+
+// NB transforms at F, F + kPad, ...: natural order -> bin k at position binpos(k) (ct_forward) and back
+// (ct_transposed); both end with a barrier
+template <int N, int NB, bool PK, bool ZU = false>
+__device__ __forceinline__ void ct_forward(float2* F, const float2* tw1, const float2* tw2, int tid) {
+    ct_pass1<N, NB, true, ZU, PK>(F, tw1, tid);
+    __syncthreads();
+    ct_pass2<N, NB, true, PK>(F, tw2, tid);
+    __syncthreads();
+    ct_pass3<N, NB, PK>(F, tid);
+    __syncthreads();
+}
+template <int N, int NB, bool PK>
+__device__ __forceinline__ void ct_transposed(float2* F, const float2* tw1, const float2* tw2, int tid) {
+    ct_pass3<N, NB, PK>(F, tid);
+    __syncthreads();
+    ct_pass2<N, NB, false, PK>(F, tw2, tid);
+    __syncthreads();
+    ct_pass1<N, NB, false, false, PK>(F, tw1, tid);
+    __syncthreads();
+}
+
 // SPEC variant: the spectra of the impulse responses are read from memory (ir_spectrum_kernel made them once per frame),
-// so the HH buffers and a quarter of the transforms disappear: 2 NJ buffers -> 53.4 KB for N = 1024, NJ = 2 -> 4 CTAs per SM
+// so the HH buffers and a quarter of the transforms disappear: 2 NJ buffers -> 54.4 KB for N = 1024, NJ = 2 -> 4 CTAs per SM
 template <int N, int NJ, int NBANK = 0, bool SPEC = false> constexpr size_t fir_fft_smem() {
-    return (size_t)(SPEC ? 2 : 3) * NJ * Plan<N>::kPad * sizeof(float2) + (size_t)(Plan<N>::kTw2 + Plan<N>::kTw3) * sizeof(float2) +
+    return (size_t)(SPEC ? 2 : 3) * NJ * Plan<N>::kPad * sizeof(float2) + (size_t)(Ct<N>::kTw1 + Ct<N>::kTw2) * sizeof(float2) +
            (size_t)NJ * kRing * sizeof(float) + (NBANK ? (size_t)5 * kBankRow * sizeof(float) : 0);
-}   // N = 1024: NJ = 2 -> 70528 B (3 CTAs per SM), NJ = 1 -> 36224 B;  N = 2048: NJ = 1 -> 64384 B, NJ = 2 -> 124800 B
+}   // N = 1024: NJ = 2 -> 73152 B (3 CTAs per SM), NJ = 1 -> 38848 B;  N = 2048: NJ = 1 -> 69568 B, NJ = 2 -> 129984 B
 
 // spectra of two real sequences a, c from Z = FFT(a + j c):  A[k] = (Z[k] + conj Z[N-k]) / 2,  C[k] = (Z[k] - conj Z[N-k]) / 2j
 __device__ __forceinline__ void split2(float2 zk, float2 zm, float2& A, float2& C) {
@@ -90,15 +234,16 @@ __device__ __forceinline__ void split2(float2 zk, float2 zm, float2& A, float2& 
 // SPEC: job[j].ir holds the packed 1024-point spectra of the impulse responses instead of the taps
 template <int N, int NJ, bool PK, int NBANK = 0, bool SPEC = false>
 __global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ? 4 : 3)) ltv_fir_fft_kernel(FftFirParams p) {
-    constexpr int kN = N, kPad = Plan<N>::kPad, kTw2 = Plan<N>::kTw2, kTw3 = Plan<N>::kTw3;
-    constexpr int kBins = N / 2 / kThreads;          // bins k = tid + 128 u per thread (DC.. N/2-1); Nyquist on thread 0
+    constexpr int kN = N, kPad = Plan<N>::kPad;
+    constexpr int kBins = N / 2 / kThreads;          // bins per thread (own_pos: DC .. N/2-1); Nyquist on thread 0
     extern __shared__ __align__(16) unsigned char smem_raw[];
     // buffer b of the batch lives at F + b * kPad:  XA(j) = j  (hop g; later the paired output of job j),
-    // XB(j) = NJ + j (hop g+1),  HH(j) = 2 NJ + j (impulse responses of frames g+1 and g+2)
+    // XB(j) = NJ + j (hop g+1),  HH(j) = 2 NJ + j (impulse responses of frames g+1 and g+2).  Sample n of a buffer is at
+    // slot padi(n), bin k of a forward-transformed one at slot at(k).
     float2* F = reinterpret_cast<float2*>(smem_raw);
-    float2* tw2 = F + (SPEC ? 2 : 3) * NJ * kPad;
-    float2* tw3 = tw2 + kTw2;
-    float* ring = reinterpret_cast<float*>(tw3 + kTw3);          // [NJ][kRing]
+    float2* tw1 = F + (SPEC ? 2 : 3) * NJ * kPad;
+    float2* tw2 = tw1 + Ct<N>::kTw1;
+    float* ring = reinterpret_cast<float*>(tw2 + Ct<N>::kTw2);   // [NJ][kRing]
     float* bank_act = ring + NJ * kRing;                         // BANK: [3][128] activated amplitudes of frames g, g+1, g+2
     float* bank_dlt = bank_act + 3 * kBankRow;                   //       [2][128] their differences
 
@@ -109,8 +254,10 @@ __global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ?
     const int t_lo = h0 * kHop, t_hi = h1 * kHop;
     const unsigned long long utt = (unsigned long long)(p.utt_off + b);
 
-    init_twiddles<N>(tw2, tw3, tid);
+    ct_twiddles<N>(tw1, tw2, tid);
     for (int i = tid; i < NJ * kRing; i += kThreads) ring[i] = 0.f;
+    auto at = [](int k) { return padi(binpos<N>(k)); };
+    const auto own_bin = [&](int u) { return bin_at<N>(own_pos(tid, u)); };
 
     // (h_j[fa], h_j[fb]) as one complex sequence, zero-padded to 1024; frame indices clamp (h_{nF} := h_{nF-1})
     auto load_ir_pair = [&](int j, int fa, int fb, bool with_b) {
@@ -210,7 +357,7 @@ __global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ?
     };
 #endif
 
-    // spectrum of frame g per job: bins k = tid + 128 u; thread 0 additionally holds DC (u = 0) and Nyquist (real)
+    // spectrum of frame g per job at the bins own_bin(u); thread 0 additionally holds DC (u = 0) and Nyquist (real)
     float2 Hp[NJ][kBins];
     float HpN[NJ];
     // Input hops are always transformed in the SAME pairs (2m-1, 2m), whatever the chunking: G is even, so the first hop
@@ -231,7 +378,7 @@ __global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ?
             const float2* row = spec_row(j, gs);
 #pragma unroll
             for (int u = 0; u < kBins; ++u) {
-                const int k = tid + u * kThreads;
+                const int k = own_bin(u);
                 const float2 h = __ldg(row + k);
                 Hp[j][u] = k == 0 ? make_float2(h.x, 0.f) : h;
                 if (k == 0) HpN[j] = h.y;
@@ -242,18 +389,18 @@ __global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ?
 #pragma unroll
         for (int j = 0; j < NJ; ++j) load_ir_pair(j, gs - 1, gs, true);    // exactly the (h_{g+1}, h_{g+2}) pair of hops gs-2, gs-1
         __syncthreads();
-        fft_forward<N, NJ, PK, true>(F + 2 * NJ * kPad, tw2, tw3, tid);
+        ct_forward<N, NJ, PK, true>(F + 2 * NJ * kPad, tw1, tw2, tid);
 #pragma unroll
         for (int j = 0; j < NJ; ++j) {
             const float2* H = F + (2 * NJ + j) * kPad;
 #pragma unroll
             for (int u = 0; u < kBins; ++u) {
-                const int k = tid + u * kThreads;
+                const int k = own_bin(u);
                 float2 unused;
-                if (k == 0) Hp[j][u] = make_float2(H[padi(0)].y, 0.f);
-                else split2(H[padi(k)], H[padi(kN - k)], unused, Hp[j][u]);
+                if (k == 0) Hp[j][u] = make_float2(H[at(0)].y, 0.f);
+                else split2(H[padi(own_pos(tid, u))], H[at(kN - k)], unused, Hp[j][u]);
             }
-            HpN[j] = H[padi(kN / 2)].y;                                 // only thread 0 uses it
+            HpN[j] = H[at(kN / 2)].y;                                 // only thread 0 uses it
         }
         __syncthreads();
     }
@@ -321,8 +468,7 @@ __global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ?
             if (!SPEC) put_ir_pair(j, pf);
         }
         __syncthreads();
-        if (g + 2 <= ge) fetch(g + 2, pf);                 // next pair's loads fly during this pair's transforms
-        fft_forward<N, (SPEC ? 2 : 3) * NJ, PK, true>(F, tw2, tw3, tid);   // all have zero upper halves: pruned first pass
+        ct_forward<N, (SPEC ? 2 : 3) * NJ, PK, true>(F, tw1, tw2, tid);   // all have zero upper halves: pruned first pass
 
         // ---- Y_g = X_g H_g + XU_g (H_{g+1} - H_g),  Y_{g+1} = X_{g+1} H_{g+1} + XU_{g+1} (H_{g+2} - H_{g+1});
         //      paired as Y_g + j Y_{g+1} (Hermitian extension), stored re/im-swapped over XA(j) ----
@@ -336,13 +482,13 @@ __global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ?
             float2 HaR[kBins], HbR[kBins];
             if (SPEC) {
 #pragma unroll
-                for (int u = 0; u < kBins; ++u) { HaR[u] = __ldg(rowA + tid + u * kThreads); HbR[u] = __ldg(rowB + tid + u * kThreads); }
+                for (int u = 0; u < kBins; ++u) { HaR[u] = __ldg(rowA + own_bin(u)); HbR[u] = __ldg(rowB + own_bin(u)); }
             }
 #pragma unroll
             for (int u = 0; u < kBins; ++u) {
-                const int k = tid + u * kThreads;
+                const int k = own_bin(u);
                 if (k == 0) continue;
-                const int ik = padi(k), im = padi(kN - k);
+                const int ik = padi(own_pos(tid, u)), im = at(kN - k);
                 float2 Xa, XUa, Xb, XUb, Ha, Hb;
                 split2(XA[ik], XA[im], Xa, XUa);
                 split2(XB[ik], XB[im], Xb, XUb);
@@ -356,24 +502,27 @@ __global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ?
                 Hp[j][u] = Hb;
             }
             if (tid == 0) {      // DC and Nyquist: every spectrum involved is real there
-                const float2 a0 = XA[padi(0)], b0 = XB[padi(0)];                              // (X, XU), (X, XU)
-                const float2 aN = XA[padi(kN / 2)], bN = XB[padi(kN / 2)];
+                const float2 a0 = XA[at(0)], b0 = XB[at(0)];                              // (X, XU), (X, XU)
+                const float2 aN = XA[at(kN / 2)], bN = XB[at(kN / 2)];
                 // (H_{g+1}, H_{g+2}) at DC and at Nyquist
-                const float2 z0 = SPEC ? make_float2(HaR[0].x, HbR[0].x) : HH[padi(0)];
-                const float2 zN = SPEC ? make_float2(HaR[0].y, HbR[0].y) : HH[padi(kN / 2)];
+                const float2 z0 = SPEC ? make_float2(HaR[0].x, HbR[0].x) : HH[at(0)];
+                const float2 zN = SPEC ? make_float2(HaR[0].y, HbR[0].y) : HH[at(kN / 2)];
                 const float hp0 = Hp[j][0].x, hpN = HpN[j];
                 const float ya0 = fmaf(a0.y, z0.x - hp0, a0.x * hp0), yb0 = fmaf(b0.y, z0.y - z0.x, b0.x * z0.x);
                 const float yaN = fmaf(aN.y, zN.x - hpN, aN.x * hpN), ybN = fmaf(bN.y, zN.y - zN.x, bN.x * zN.x);
-                XA[padi(0)] = make_float2(yb0, ya0);
-                XA[padi(kN / 2)] = make_float2(ybN, yaN);
+                XA[at(0)] = make_float2(yb0, ya0);
+                XA[at(kN / 2)] = make_float2(ybN, yaN);
                 Hp[j][0] = make_float2(z0.y, 0.f);
                 HpN[j] = zN.y;
             }
         }
         __syncthreads();
+        // the next pair's loads fly during the inverse transforms and the overlap-add (issued here, not earlier: the
+        // registers they land in would otherwise be held through the forward batch and the pointwise step)
+        if (g + 2 <= ge) fetch(g + 2, pf);
 
         // ---- inverse of the pairs (batch over jobs): hop g = stored .y / N, hop g+1 = stored .x / N ----
-        fft_forward<N, NJ, PK>(F, tw2, tw3, tid);
+        ct_transposed<N, NJ, PK>(F, tw1, tw2, tid);
 
         // ---- overlap-add at the delay-compensated positions t = gP - L/2 + n (hop g) and + P (hop g+1), kept to this
         //      CTA's hops.  Slots hit twice (n and n - P) belong to the same thread: no race. ----
@@ -475,22 +624,55 @@ bool ltv_fir_fft_supported(int P, int taps1, int taps2, int njobs) {
     return P == kHop && taps1 > 0 && (njobs == 1 || taps2 > 0) && tmax <= 1024;
 }
 
+// Hops per CTA, G (even).  A CTA walks its G + 2 input hops serially, so a launch takes about
+// (waves of CTAs at the kernel's occupancy) x (G + 2) hop times: G = 32 on B = 32 x 10 s gives 864 CTAs for 396 resident
+// slots, 2.18 waves, and the third wave runs 18 % full.  Pick the G that minimises that product (the largest on a tie:
+// least recomputation); it also shrinks G for small launches -- one utterance of a real-time caller, one chunk of the
+// host pipeline -- until they spread over the GPU.  The output does not depend on G (hops are always paired the same way).
+// `occ` caches the occupancy per device: the query costs host time that a small (real-time) launch would notice.
+static int fir_fft_hops_per_cta(const void* kernel, size_t smem, std::atomic<int>* occ, int B, int nF) {
+    constexpr int kMaxHops = 64;
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) { cudaGetLastError(); dev = -1; }
+    int per_sm = dev >= 0 ? occ[dev].load(std::memory_order_relaxed) : 0;
+    if (per_sm <= 0) {
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, smem) != cudaSuccess || per_sm < 1) {
+            cudaGetLastError();
+            per_sm = 1;
+        }
+        if (dev >= 0) occ[dev].store(per_sm, std::memory_order_relaxed);
+    }
+    const long long slots = (long long)per_sm * b2d::num_sms();
+    int best = 2;
+    long long best_cost = -1;
+    for (int G = kMaxHops; G >= 2; G -= 2) {
+        const long long ctas = (long long)B * ((nF + G - 1) / G);
+        const long long cost = (ctas + slots - 1) / slots * (G + 2);
+        if (best_cost < 0 || cost < best_cost) { best_cost = cost; best = G; }
+    }
+    return best;
+}
+
 template <int N, int NJ, bool PK, int NBANK = 0, bool SPEC = false>
-static int launch_fir_fft_as(const FftFirParams& p, dim3 grid, cudaStream_t st) {
+static int launch_fir_fft_as(FftFirParams p, int B, cudaStream_t st) {
+    const auto kernel = ltv_fir_fft_kernel<N, NJ, PK, NBANK, SPEC>;
     constexpr size_t smem = fir_fft_smem<N, NJ, NBANK, SPEC>();
     // per launch, like the direct-form kernels: function attributes are per device and this costs ~1 us
     if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(ltv_fir_fft_kernel<N, NJ, PK, NBANK, SPEC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return fail((int)e, "ltv_fir(fft): smem attr: %s", cudaGetErrorString(e));
     }
-    cudaFuncSetAttribute(ltv_fir_fft_kernel<N, NJ, PK, NBANK, SPEC>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    ltv_fir_fft_kernel<N, NJ, PK, NBANK, SPEC><<<grid, kThreads, smem, st>>>(p);
+    cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    static std::atomic<int> occ[64];
+    p.G = fir_fft_hops_per_cta(reinterpret_cast<const void*>(kernel), smem, occ, B, p.nF);
+    const dim3 grid((unsigned)((p.nF + p.G - 1) / p.G), B);
+    kernel<<<grid, kThreads, smem, st>>>(p);
     return check_launch("ltv_fir(fft)");
 }
 
 template <int N, int NJ>
-static int launch_fir_fft(const FftFirParams& p, dim3 grid, cudaStream_t st) {
-    return g_fft_packed.load(std::memory_order_relaxed) ? launch_fir_fft_as<N, NJ, true>(p, grid, st) : launch_fir_fft_as<N, NJ, false>(p, grid, st);
+static int launch_fir_fft(const FftFirParams& p, int B, cudaStream_t st) {
+    return g_fft_packed.load(std::memory_order_relaxed) ? launch_fir_fft_as<N, NJ, true>(p, B, st) : launch_fir_fft_as<N, NJ, false>(p, B, st);
 }
 
 int ltv_fir_fft_launch(const float* x1, const float* ir1, int taps1, float* y1, const float* x2, const float* ir2,
@@ -503,17 +685,9 @@ int ltv_fir_fft_launch(const float* x1, const float* ir1, int taps1, float* y1, 
     p.job[0] = {x1, ir1, y1, taps1};
     p.job[1] = {x2, ir2, y2, njobs == 2 ? taps2 : taps1};
     p.addend = addend; p.mix = mix; p.seed = seed; p.utt_off = utt_off; p.nF = nF;
-    // Hops per CTA.  A CTA walks its G + 2 input hops serially (~5.5 us per hop), so G = 32 is right when the grid fills
-    // the GPU (B = 32 x 10 s: 864 CTAs for 444 resident slots) but makes small launches -- one utterance of a real-time
-    // caller, one chunk of the host pipeline -- latency-bound; halve G (25 % / 50 % / 100 % recomputation at 8 / 4 / 2)
-    // until there are at least two CTAs per SM.
-    int G = 32;
-    while (G > 2 && (long long)B * ((nF + G - 1) / G) < (long long)b2d::num_sms() * 2) G >>= 1;
-    p.G = G;
-    const dim3 grid((unsigned)((nF + p.G - 1) / p.G), B);
     const int tmax = njobs == 2 ? (taps1 > taps2 ? taps1 : taps2) : taps1;
-    if (tmax <= kHop) return njobs == 2 ? launch_fir_fft<1024, 2>(p, grid, st) : launch_fir_fft<1024, 1>(p, grid, st);
-    return njobs == 2 ? launch_fir_fft<2048, 2>(p, grid, st) : launch_fir_fft<2048, 1>(p, grid, st);
+    if (tmax <= kHop) return njobs == 2 ? launch_fir_fft<1024, 2>(p, B, st) : launch_fir_fft<1024, 1>(p, B, st);
+    return njobs == 2 ? launch_fir_fft<2048, 2>(p, B, st) : launch_fir_fft<2048, 1>(p, B, st);
 }
 
 // Sins fused: harmonic = allpass(bank(f0, amplitudes)), noise = filter(white noise), signal = harmonic + noise in ONE
@@ -540,13 +714,9 @@ int sins_fused_launch(const float* f0, const double* frame_phase, const float* c
     p.bank.f0 = f0; p.bank.frame_phase = frame_phase; p.bank.c_amp = c_amp; p.bank.ctrl_stride = ctrl_stride;
     p.bank.H = H; p.bank.inv_sr = 1.0 / sampling_rate; p.bank.nyquist = (float)(sampling_rate / 2.0);
     p.bank.round_fp32 = round_fp32;
-    int G = 32;
-    while (G > 2 && (long long)B * ((nF + G - 1) / G) < (long long)b2d::num_sms() * 2) G >>= 1;
-    p.G = G;
-    const dim3 grid((unsigned)((nF + p.G - 1) / p.G), B);
     const bool pk = g_fft_packed.load(std::memory_order_relaxed) != 0;
-    if (H <= 64) return pk ? launch_fir_fft_as<1024, 2, true, 4>(p, grid, st) : launch_fir_fft_as<1024, 2, false, 4>(p, grid, st);
-    return pk ? launch_fir_fft_as<1024, 2, true, 8>(p, grid, st) : launch_fir_fft_as<1024, 2, false, 8>(p, grid, st);
+    if (H <= 64) return pk ? launch_fir_fft_as<1024, 2, true, 4>(p, B, st) : launch_fir_fft_as<1024, 2, false, 4>(p, B, st);
+    return pk ? launch_fir_fft_as<1024, 2, true, 8>(p, B, st) : launch_fir_fft_as<1024, 2, false, 8>(p, B, st);
 }
 
 // ---- spectrum path (Sins): ir_spectrum_kernel once per call, then the SPEC variant of the FIR kernel ----
@@ -581,12 +751,8 @@ int ltv_fir_fft_spec_launch(const float* x1, const float* spec1, int taps1, floa
     p.job[0] = {x1, spec1, y1, taps1};
     p.job[1] = {x2, spec2, y2, taps2};
     p.addend = nullptr; p.mix = mix; p.seed = seed; p.utt_off = utt_off; p.nF = nF;
-    int G = 32;
-    while (G > 2 && (long long)B * ((nF + G - 1) / G) < (long long)b2d::num_sms() * 2) G >>= 1;
-    p.G = G;
-    const dim3 grid((unsigned)((nF + p.G - 1) / p.G), B);
-    return g_fft_packed.load(std::memory_order_relaxed) ? launch_fir_fft_as<1024, 2, true, 0, true>(p, grid, st)
-                                                        : launch_fir_fft_as<1024, 2, false, 0, true>(p, grid, st);
+    return g_fft_packed.load(std::memory_order_relaxed) ? launch_fir_fft_as<1024, 2, true, 0, true>(p, B, st)
+                                                        : launch_fir_fft_as<1024, 2, false, 0, true>(p, B, st);
 }
 
 }  // namespace b2d
