@@ -91,6 +91,9 @@ SIGNATURES = {
     "b2d_set_sins_impl": (ctypes.c_int, [ctypes.c_int]),
     "b2d_combsubfast_filter": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int64, c_f32p, ctypes.c_uint64,
                                               ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p, c_stream]),
+    "b2d_combsubfast_filter_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int64, c_f32p,
+                                                       ctypes.c_uint64, ctypes.c_int64, c_f32p, ctypes.c_int,
+                                                       ctypes.c_int, ctypes.c_int, c_f32p, c_stream]),
     "b2d_comb_source": (ctypes.c_int, [c_f32p, c_f64p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double,
                                        ctypes.c_int, c_f32p, c_stream]),
     "b2d_combsub_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int] * 6),

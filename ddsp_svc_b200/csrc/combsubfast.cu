@@ -213,6 +213,183 @@ __global__ void __launch_bounds__(kThreads, 4) combsubfast_kernel(CfParams p) {
     }
 }
 
+// ---- backward: gradients of the three raw controls ----------------------------------------------------------------
+// g = dL/dsignal.  For frame q (control row min(q, nF-1)), with C_q, Z_q the comb / noise spectra of the forward:
+//   rho_q[i] = w[i] g[(q-1)P + i]  (zero outside [0, T))             cotangent of the windowed irfft output
+//   G_q      = (2/N) rfft(rho_q)[k] for 0 < k < N/2;  (1/N) Re rfft(rho_q)[k] at k = 0, N/2 (C2R drops Im there)
+//   A_q      = C_q exp(m_h + j pi p_h),  B_q = Z_q exp(m_n) / 128
+//   dL/dm_h  = Re(conj(G) A),  dL/dp_h = -pi Im(conj(G) A),  dL/dm_n = Re(conj(G) B)
+// Row nF-1 receives frames nF-1 and nF.  One CTA owns the control rows [h0, h1) of one utterance and transforms
+// exactly the frames of those rows (plus frame nF in the CTA of row nF-1): every gradient element has one owning
+// thread, no atomics.  Per pair of frames (2m, 2m+1) one batched transform of three buffers: w (comb + j noise) of
+// each frame, as the forward's load_frame builds it, and rho_a + j rho_b, split by conjugate symmetry -> 1.5 FFTs per
+// frame.  The pairs are fixed (G even), so the gradient is bit-identical for any chunking or batch split.
+struct CfBwdParams {
+    const float* comb;         // [B, T]  the forward's comb source
+    const float* noise_in;     // [B, T] or nullptr (in-kernel Philox, as the forward)
+    const float* c_hm; const float* c_hp; const float* c_nm;   // [B, nF, P+1] views, frame stride ctrl_stride
+    long long ctrl_stride;
+    const float* grad;         // [B, T]  dL/dsignal
+    float* grad_ctrl;          // [B, nF, 3 (P+1)]  harmonic_magnitude | harmonic_phase | noise_magnitude
+    int nF, G;
+    unsigned long long seed;
+    long long utt_off;
+};
+
+constexpr size_t kBwdSmemBytes = (size_t)3 * kPad * sizeof(float2) + (size_t)(kTw2 + kTw3) * sizeof(float2) +
+                                 (size_t)kN * sizeof(float);   // 52224 + 1920 + 4096 = 58240 B -> 3 CTAs per SM
+
+// windowed (comb + j noise) of frame q, built exactly as the forward's load_frame
+__device__ __forceinline__ void bwd_source_frame(const CfBwdParams& p, const float* comb_row, const float* noise_row,
+                                                 unsigned long long utt, int T, int q, const float* win, float2* buf,
+                                                 int tid) {
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+        const int i0 = (tid << 2) + u * (kThreads << 2);
+        const int m0 = (q - 1) * kP + i0;
+        float4 c = make_float4(0.f, 0.f, 0.f, 0.f), z = c;
+        if (m0 >= 0 && m0 < T) {
+            c = __ldg(reinterpret_cast<const float4*>(comb_row + m0));
+            z = noise_row ? __ldg(reinterpret_cast<const float4*>(noise_row + m0))
+                          : b2d::philox_uniform_pm1(p.seed, utt, (uint32_t)(m0 >> 2));
+        }
+        const float4 w = *reinterpret_cast<const float4*>(win + i0);
+        buf[padi(i0 + 0)] = make_float2(w.x * c.x, w.x * z.x);
+        buf[padi(i0 + 1)] = make_float2(w.y * c.y, w.y * z.y);
+        buf[padi(i0 + 2)] = make_float2(w.z * c.z, w.z * z.z);
+        buf[padi(i0 + 3)] = make_float2(w.w * c.w, w.w * z.w);
+    }
+}
+
+// rho_a + j rho_b of frames q, q+1 (rho_b = 0 without frame q+1)
+__device__ __forceinline__ void bwd_cotangent_pair(const float* g_row, int T, int q, bool has_b, const float* win,
+                                                   float2* buf, int tid) {
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+        const int i0 = (tid << 2) + u * (kThreads << 2);
+        const int ma = (q - 1) * kP + i0, mb = ma + kP;
+        float4 ga = make_float4(0.f, 0.f, 0.f, 0.f), gb = ga;
+        if (ma >= 0 && ma < T) ga = __ldg(reinterpret_cast<const float4*>(g_row + ma));
+        if (has_b && mb < T) gb = __ldg(reinterpret_cast<const float4*>(g_row + mb));   // mb >= 0
+        const float4 w = *reinterpret_cast<const float4*>(win + i0);
+        buf[padi(i0 + 0)] = make_float2(w.x * ga.x, w.x * gb.x);
+        buf[padi(i0 + 1)] = make_float2(w.y * ga.y, w.y * gb.y);
+        buf[padi(i0 + 2)] = make_float2(w.z * ga.z, w.z * gb.z);
+        buf[padi(i0 + 3)] = make_float2(w.w * ga.w, w.w * gb.w);
+    }
+}
+
+// (dL/dm_h, dL/dp_h, dL/dm_n) of one bin from the cotangent spectrum G, the comb spectrum C and the noise spectrum Z
+struct BinGrad { float hm, hp, nm; };
+__device__ __forceinline__ BinGrad bin_grad(float2 G, float2 C, float2 Z, const BinFilter& f) {
+    const float2 A = cmul(C, f.hs);
+    BinGrad d;
+    d.hm = fmaf(G.x, A.x, G.y * A.y);                                  // Re(conj(G) A)
+    d.hp = -B2D_PI_F * fmaf(G.x, A.y, -G.y * A.x);                     // -pi Im(conj(G) A)
+    d.nm = fmaf(G.x, Z.x, G.y * Z.y) * f.hn;                           // Re(conj(G) Z) exp(m_n) / 128
+    return d;
+}
+
+template <bool PK>
+__global__ void __launch_bounds__(kThreads, 3) combsubfast_bwd_kernel(CfBwdParams p) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    float2* bufA = reinterpret_cast<float2*>(smem_raw);          // source of frame a -> its spectrum
+    float2* bufB = bufA + kPad;                                  // source of frame b -> its spectrum
+    float2* bufC = bufB + kPad;                                  // rho_a + j rho_b -> pair spectrum (batched after bufB)
+    float2* tw2 = bufC + kPad;
+    float2* tw3 = tw2 + kTw2;
+    float* win = reinterpret_cast<float*>(tw3 + kTw3);           // sqrt(Hann_N), periodic
+
+    const int tid = threadIdx.x;
+    const int b = blockIdx.y;
+    const int nF = p.nF, T = nF * kP;
+    const int h0 = blockIdx.x * p.G, h1 = min(h0 + p.G, nF);
+    const int qe = (h1 == nF) ? nF : h1 - 1;                     // last frame of this CTA
+    const float* comb_row = p.comb + (size_t)b * T;
+    const float* noise_row = p.noise_in ? p.noise_in + (size_t)b * T : nullptr;
+    const float* g_row = p.grad + (size_t)b * T;
+    const unsigned long long utt = (unsigned long long)(p.utt_off + b);
+    constexpr int kBins = kP + 1;
+    constexpr float kScale = 1.0f / kN;                          // (2/N) x the 1/2 of the conjugate-symmetry split
+
+    for (int i = tid; i < kN; i += kThreads) win[i] = sqrtf(0.5f - 0.5f * cospif((float)i * (2.0f / kN)));
+    b2d_fft_smem::init_twiddles<kN>(tw2, tw3, tid);
+    __syncthreads();
+
+#pragma unroll 1
+    for (int qa = h0; qa <= qe; qa += 2) {
+        const int qb = qa + 1;
+        const bool has_b = qb <= qe;
+        const int row_a = min(qa, nF - 1), row_b = min(qb, nF - 1);
+        float hm_a[4], hp_a[4], nm_a[4], hm_b[4], hp_b[4], nm_b[4];
+        const size_t off_a = ((size_t)b * nF + row_a) * (size_t)p.ctrl_stride;
+        const size_t off_b = ((size_t)b * nF + row_b) * (size_t)p.ctrl_stride;
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+            const int k = tid + u * kThreads;
+            hm_a[u] = __ldg(p.c_hm + off_a + k); hp_a[u] = __ldg(p.c_hp + off_a + k); nm_a[u] = __ldg(p.c_nm + off_a + k);
+            hm_b[u] = __ldg(p.c_hm + off_b + k); hp_b[u] = __ldg(p.c_hp + off_b + k); nm_b[u] = __ldg(p.c_nm + off_b + k);
+        }
+        float ny_a[3] = {0.f, 0.f, 0.f}, ny_b[3] = {0.f, 0.f, 0.f};               // Nyquist bin, thread 0 only
+        if (tid == 0) {
+            ny_a[0] = __ldg(p.c_hm + off_a + kP); ny_a[1] = __ldg(p.c_hp + off_a + kP); ny_a[2] = __ldg(p.c_nm + off_a + kP);
+            ny_b[0] = __ldg(p.c_hm + off_b + kP); ny_b[1] = __ldg(p.c_hp + off_b + kP); ny_b[2] = __ldg(p.c_nm + off_b + kP);
+        }
+
+        bwd_source_frame(p, comb_row, noise_row, utt, T, qa, win, bufA, tid);
+        if (has_b) bwd_source_frame(p, comb_row, noise_row, utt, T, qb, win, bufB, tid);
+        else {
+            for (int i = tid; i < kPad; i += kThreads) bufB[i] = make_float2(0.f, 0.f);
+        }
+        bwd_cotangent_pair(g_row, T, qa, has_b, win, bufC, tid);
+        __syncthreads();
+        b2d_fft_smem::fft_forward<1024, 3, PK>(bufA, tw2, tw3, tid);
+
+        // the gradient of frame a goes to row_a; frame nF shares row nF-1 with frame nF-1 and is added to it
+        float* out_a = p.grad_ctrl + ((size_t)b * nF + row_a) * (3 * kBins);
+        float* out_b = p.grad_ctrl + ((size_t)b * nF + row_b) * (3 * kBins);
+        const bool merge = has_b && qb == nF;                      // frames nF-1, nF in this pair: one store of a + b
+        const bool held = qa == nF;                                // frame nF alone: add to the stored row nF-1
+        auto store = [&](int k, BinGrad da, BinGrad db) {
+            if (merge) { da.hm += db.hm; da.hp += db.hp; da.nm += db.nm; }
+            else if (held) { da.hm += out_a[k]; da.hp += out_a[kBins + k]; da.nm += out_a[2 * kBins + k]; }
+            out_a[k] = da.hm; out_a[kBins + k] = da.hp; out_a[2 * kBins + k] = da.nm;
+            if (has_b && !merge) { out_b[k] = db.hm; out_b[kBins + k] = db.hp; out_b[2 * kBins + k] = db.nm; }
+        };
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+            const int k = tid + u * kThreads;
+            if (k == 0) continue;                                                 // DC / Nyquist handled below
+            const int ik = padi(k), im = padi(kN - k);
+            const float2 za = bufA[ik], zam = bufA[im], zb = bufB[ik], zbm = bufB[im];
+            const float2 y = bufC[ik], ym = bufC[im];
+            // spectra of each real sequence from the spectrum of x + j y: X = (Z[k] + conj Z[N-k]) / 2,
+            // Y = (Z[k] - conj Z[N-k]) / (2j); the cotangent's 1/2 is folded into kScale
+            const float2 Ca = make_float2(0.5f * (za.x + zam.x), 0.5f * (za.y - zam.y));
+            const float2 Za = make_float2(0.5f * (za.y + zam.y), 0.5f * (zam.x - za.x));
+            const float2 Cb = make_float2(0.5f * (zb.x + zbm.x), 0.5f * (zb.y - zbm.y));
+            const float2 Zb = make_float2(0.5f * (zb.y + zbm.y), 0.5f * (zbm.x - zb.x));
+            const float2 Ga = make_float2(kScale * (y.x + ym.x), kScale * (y.y - ym.y));
+            const float2 Gb = make_float2(kScale * (y.y + ym.y), kScale * (ym.x - y.x));
+            store(k, bin_grad(Ga, Ca, Za, make_filter(hm_a[u], hp_a[u], nm_a[u])),
+                  bin_grad(Gb, Cb, Zb, make_filter(hm_b[u], hp_b[u], nm_b[u])));
+        }
+        if (tid == 0) {
+            // k = 0 and k = N/2: every spectrum is its own partner (C = Re Z, noise = Im Z); G = (1/N) Re rfft(rho)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int k = e ? kP : 0;
+                const float2 za = bufA[padi(k)], zb = bufB[padi(k)], y = bufC[padi(k)];
+                const BinFilter fa = e ? make_filter(ny_a[0], ny_a[1], ny_a[2]) : make_filter(hm_a[0], hp_a[0], nm_a[0]);
+                const BinFilter fb = e ? make_filter(ny_b[0], ny_b[1], ny_b[2]) : make_filter(hm_b[0], hp_b[0], nm_b[0]);
+                store(k, bin_grad(make_float2(y.x * kScale, 0.f), make_float2(za.x, 0.f), make_float2(za.y, 0.f), fa),
+                      bin_grad(make_float2(y.y * kScale, 0.f), make_float2(zb.x, 0.f), make_float2(zb.y, 0.f), fb));
+            }
+        }
+        __syncthreads();                                                          // the buffers are rewritten next pair
+    }
+}
+
 }  // namespace
 
 #ifndef B2D_HOST_EMU
@@ -240,5 +417,41 @@ extern "C" int b2d_combsubfast_filter(const float* comb, const float* c_harmonic
     if (b2d::g_fft_packed.load(std::memory_order_relaxed)) combsubfast_kernel<true><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(p);
     else combsubfast_kernel<false><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(p);
     return b2d::check_launch("combsubfast");
+}
+
+extern "C" int b2d_combsubfast_filter_backward(const float* comb, const float* c_hm, const float* c_hp, const float* c_nm,
+                                               int64_t ctrl_stride, const float* noise_in, uint64_t seed,
+                                               int64_t utterance_offset, const float* grad_signal, int B, int n_frames,
+                                               int block, float* grad_ctrl, void* stream) {
+    if (!comb || !c_hm || !c_hp || !c_nm || !grad_signal || !grad_ctrl)
+        return b2d::fail(B2D_ERR_NULL, "combsubfast_backward: null pointer");
+    if (B <= 0 || n_frames <= 0) return b2d::fail(B2D_ERR_SHAPE, "combsubfast_backward: bad shape");
+    if (block != kP) return b2d::fail(B2D_ERR_UNSUPPORTED, "combsubfast_backward: block size %d (this build: %d)", block, kP);
+    if (ctrl_stride < kP + 1)
+        return b2d::fail(B2D_ERR_SHAPE, "combsubfast_backward: control stride %lld < %d", (long long)ctrl_stride, kP + 1);
+    if (B > 65535) return b2d::fail(B2D_ERR_UNSUPPORTED, "combsubfast_backward: batch %d > 65535", B);
+    if (!b2d::aligned16(comb) || !b2d::aligned16(grad_signal) || !b2d::aligned16(grad_ctrl) ||
+        (noise_in && !b2d::aligned16(noise_in)))
+        return b2d::fail(B2D_ERR_ALIGN, "combsubfast_backward: comb / noise_in / grad_signal / grad_ctrl must be "
+                         "16-byte aligned");
+    CfBwdParams p;
+    p.comb = comb; p.noise_in = noise_in;
+    p.c_hm = c_hm; p.c_hp = c_hp; p.c_nm = c_nm; p.ctrl_stride = ctrl_stride;
+    p.grad = grad_signal; p.grad_ctrl = grad_ctrl; p.nF = n_frames;
+    int G = 32;            // rows per CTA (even: fixed frame pairs); shorter chunks when the launch would not fill the GPU
+    while (G > 2 && (long long)B * ((n_frames + G - 1) / G) < (long long)b2d::num_sms() * 2) G >>= 1;
+    p.G = G;
+    p.seed = seed; p.utt_off = utterance_offset;
+    const dim3 grid((unsigned)((n_frames + G - 1) / G), B);
+    auto go = [&](auto kern) -> int {
+        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBwdSmemBytes);
+        if (e != cudaSuccess) return b2d::fail((int)e, "combsubfast_backward: smem attr: %s", cudaGetErrorString(e));
+        kern<<<grid, kThreads, kBwdSmemBytes, (cudaStream_t)stream>>>(p);
+        return 0;
+    };
+    const int rc = b2d::g_fft_packed.load(std::memory_order_relaxed) ? go(combsubfast_bwd_kernel<true>)
+                                                                     : go(combsubfast_bwd_kernel<false>);
+    if (rc) return rc;
+    return b2d::check_launch("combsubfast_backward");
 }
 #endif  // B2D_HOST_EMU

@@ -586,20 +586,78 @@ def set_sinegen_impl(name):
 
 def combsubfast_filter(comb, c_hm, c_hp, c_nm, block, noise_in=None, seed=0, utterance_offset=0):
     """CombSubFast after the source: comb [B, T] + raw controls [B, nF, block+1] -> signal [B, T]
-    (reference ddsp/vocoder.py:758-784)."""
+    (reference ddsp/vocoder.py:758-784).
+    Differentiable with respect to the three controls when one of them requires grad (and grad mode is on): the
+    backward runs combsubfast_filter_backward with the same comb, noise and seed.  comb is data (no gradient)."""
+    if torch.is_grad_enabled() and any(isinstance(c, torch.Tensor) and c.requires_grad for c in (c_hm, c_hp, c_nm)):
+        if isinstance(comb, torch.Tensor) and comb.requires_grad:
+            raise NotImplementedError("combsubfast_filter has no gradient with respect to comb; pass comb.detach()")
+        if noise_in is not None:
+            noise_in = noise_in.detach()
+        return _CombSubFastFilter.apply(comb, noise_in, int(block), int(seed), int(utterance_offset), c_hm, c_hp, c_nm)
+    return _combsubfast_filter(comb, c_hm, c_hp, c_nm, block, noise_in, seed, utterance_offset)
+
+
+def combsubfast_filter_backward(comb, c_hm, c_hp, c_nm, grad_signal, block, noise_in=None, seed=0, utterance_offset=0):
+    """Gradient of combsubfast_filter with respect to the three raw controls, for dL/dsignal ``grad_signal`` [B, T].
+    comb / controls / noise_in / seed / utterance_offset must be those of the forward call (the kernel recomputes the
+    source spectra and regenerates the in-kernel noise).  -> dense [B, nF, 3*(block+1)]: harmonic_magnitude |
+    harmonic_phase | noise_magnitude along the last axis (the split_to_dict layout)."""
+    comb, (hm, hp, nm), stride, noise_in, B, nF = _combsubfast_args(comb, c_hm, c_hp, c_nm, block, noise_in)
+    _need_cuda_f32("grad_signal", grad_signal)
+    if tuple(grad_signal.shape) != (B, nF * block):
+        raise ValueError("grad_signal must be [B, n_frames*block] = [%d, %d], got %s"
+                         % (B, nF * block, tuple(grad_signal.shape)))
+    grad_signal = grad_signal.contiguous()
+    grad = torch.empty(B, nF, 3 * (block + 1), dtype=torch.float32, device=comb.device)
+    rc = _lib.lib().b2d_combsubfast_filter_backward(comb.data_ptr(), hm.data_ptr(), hp.data_ptr(), nm.data_ptr(), stride,
+                                                    _ptr(noise_in), int(seed), int(utterance_offset),
+                                                    grad_signal.data_ptr(), B, nF, int(block), grad.data_ptr(), _stream())
+    _lib.check(rc, "b2d_combsubfast_filter_backward")
+    _count(1)
+    return grad
+
+
+class _CombSubFastFilter(torch.autograd.Function):
+    """combsubfast_filter with a CUDA backward.  Saves the comb, the noise input and the control views (no spectra):
+    the backward kernel recomputes the source spectra and regenerates the in-kernel noise from seed."""
+
+    @staticmethod
+    def forward(ctx, comb, noise_in, block, seed, utterance_offset, c_hm, c_hp, c_nm):
+        signal = _combsubfast_filter(comb, c_hm, c_hp, c_nm, block, noise_in, seed, utterance_offset)
+        ctx.save_for_backward(comb, noise_in, c_hm, c_hp, c_nm)
+        ctx.cfg = (block, seed, utterance_offset)
+        return signal
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_signal):
+        comb, noise_in, c_hm, c_hp, c_nm = ctx.saved_tensors
+        block, seed, utterance_offset = ctx.cfg
+        grad = combsubfast_filter_backward(comb, c_hm, c_hp, c_nm, grad_signal, block, noise_in=noise_in, seed=seed,
+                                           utterance_offset=utterance_offset)
+        return (None,) * 5 + tuple(torch.split(grad, block + 1, dim=-1))
+
+
+def _combsubfast_args(comb, c_hm, c_hp, c_nm, block, noise_in):
+    """checked (comb, controls, frame stride, noise rows, B, nF) of a combsubfast call"""
     _need_cuda_f32("comb", comb)
     if comb.dim() != 2 or comb.shape[1] % int(block) != 0:
         raise ValueError("comb must be [B, n_frames*block] with block=%d, got %s" % (block, tuple(comb.shape)))
     B, T = comb.shape
     nF = T // block
-    (hm, hp, nm), stride = _same_stride([("harmonic_magnitude", c_hm), ("harmonic_phase", c_hp),
-                                         ("noise_magnitude", c_nm)], B, nF)
-    if hm.shape[2] != block + 1:
+    ctrls, stride = _same_stride([("harmonic_magnitude", c_hm), ("harmonic_phase", c_hp),
+                                  ("noise_magnitude", c_nm)], B, nF)
+    if ctrls[0].shape[2] != block + 1:
         raise ValueError("controls must have block_size+1 = %d bins" % (block + 1))
-    comb = comb.contiguous()
     if noise_in is not None:
         noise_in = _noise_rows(noise_in, B, T)
-    signal = torch.empty(B, T, dtype=torch.float32, device=comb.device)
+    return comb.contiguous(), ctrls, stride, noise_in, B, nF
+
+
+def _combsubfast_filter(comb, c_hm, c_hp, c_nm, block, noise_in=None, seed=0, utterance_offset=0):
+    comb, (hm, hp, nm), stride, noise_in, B, nF = _combsubfast_args(comb, c_hm, c_hp, c_nm, block, noise_in)
+    signal = torch.empty(B, nF * block, dtype=torch.float32, device=comb.device)
     rc = _lib.lib().b2d_combsubfast_filter(comb.data_ptr(), hm.data_ptr(), hp.data_ptr(), nm.data_ptr(), stride,
                                            _ptr(noise_in), int(seed), int(utterance_offset), B, nF, int(block),
                                            signal.data_ptr(), _stream())

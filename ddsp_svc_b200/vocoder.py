@@ -226,11 +226,22 @@ class CombSubFast(_SynthBase):
 
     def forward(self, units_frames, f0_frames, volume_frames, spk_id=None, spk_mix_dict=None, aug_shift=None,
                 initial_phase=None, infer=True, noise=None, utterance_offset=0, **kwargs):
+        """Trainable in the training phase: with ``infer=False`` (what the reference's diffusion/solver_new.py
+        passes through vocoder.Unit2Wav) and a control from ``unit2ctrl`` that requires grad (grad mode on),
+        ``signal`` is differentiable with respect to the three controls (CUDA backward,
+        ops.combsubfast_filter_backward).  Under grad, ``infer=True`` is refused.  f0 is data, as in the
+        reference's training loop: an f0 that requires grad is refused."""
         sr, block = self._scalars()
+        if torch.is_grad_enabled() and isinstance(f0_frames, torch.Tensor) and f0_frames.requires_grad:
+            raise NotImplementedError("CombSubFast has no gradient with respect to f0_frames; pass f0 as data "
+                                      "(f0_frames.detach()), as the reference's training loop does")
         frame_phase, phase_frames = ops.phase_scan(f0_frames, block, sr, initial_phase, infer)
         ctrls, hidden = self.unit2ctrl(units_frames, f0_frames, phase_frames, volume_frames, spk_id=spk_id,
                                        spk_mix_dict=spk_mix_dict, aug_shift=aug_shift)
-        self._forward_only(ctrls)
+        if infer and torch.is_grad_enabled() and any(v.requires_grad for v in ctrls.values()):
+            raise NotImplementedError(
+                "CombSubFast is differentiable in the training phase only: call it with infer=False (what the "
+                "reference's diffusion/solver_new.py does), or under torch.no_grad() for inference")
         comb = ops.comb_source(f0_frames, frame_phase, block, sr, infer)
         signal = ops.combsubfast_filter(comb, ctrls["harmonic_magnitude"], ctrls["harmonic_phase"],
                                         ctrls["noise_magnitude"], block, noise_in=noise,

@@ -267,6 +267,16 @@ int b2d_combsubfast_filter(const float* comb, const float* c_harmonic_magnitude,
                            const float* c_noise_magnitude, int64_t ctrl_stride, const float* noise_in,
                            uint64_t seed, int64_t utterance_offset, int B, int n_frames, int block,
                            float* signal, void* stream);
+/* Backward of b2d_combsubfast_filter with respect to the three raw controls (training; no gradient with respect to
+ * comb).  Same comb, controls, noise_in / seed / utterance_offset as the forward call (the source spectra are
+ * recomputed, the in-kernel noise stream is regenerated); grad_signal = dL/dsignal [B, T] (T = n_frames*block).
+ * grad_ctrl [B, n_frames, 3*(block+1)] receives dL/d(harmonic_magnitude | harmonic_phase | noise_magnitude) per
+ * frame; it is overwritten, deterministically (no atomics), bit-identically for any batch split.
+ * comb, grad_signal, grad_ctrl and noise_in must be 16-byte aligned.  block must be 512. */
+int b2d_combsubfast_filter_backward(const float* comb, const float* c_hm, const float* c_hp, const float* c_nm,
+                                    int64_t ctrl_stride, const float* noise_in, uint64_t seed,
+                                    int64_t utterance_offset, const float* grad_signal, int B, int n_frames,
+                                    int block, float* grad_ctrl, void* stream);
 
 /* Arithmetic of the shared-memory FFT kernels (ltv_fir_fft, superfast, combsubfast): 1 (default) = the
  * "packed" instantiations, 0 = the scalar ones; Hopper has no packed FP32 add, so both use scalar complex additions.  B2D_FFT_ARITH=scalar in the environment selects 0 as the initial value.  Process-wide test/diagnostic knob
