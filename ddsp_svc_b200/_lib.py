@@ -102,6 +102,12 @@ SIGNATURES = {
                                          ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                          ctypes.c_double, ctypes.c_int, c_f32p, c_f32p, c_f32p, ctypes.c_void_p,
                                          ctypes.c_size_t, c_stream]),
+    "b2d_combsub_synth_backward_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int] * 3),
+    "b2d_combsub_synth_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int64, c_f32p,
+                                                  ctypes.c_uint64, ctypes.c_int64, ctypes.c_void_p, c_f32p, c_f32p,
+                                                  c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                                  ctypes.c_int, ctypes.c_int, ctypes.c_double, c_f32p,
+                                                  ctypes.c_void_p, ctypes.c_size_t, c_stream]),
     "b2d_superfast_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int, ctypes.c_int]),
     "b2d_superfast_scan": (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double,
                                           ctypes.c_void_p, c_f32p, c_stream]),

@@ -20,6 +20,7 @@
 #ifndef B2D_HOST_EMU               // tests/emu/ runs these kernels' source on the CPU (host_emu.h provides the shims)
 #include "b2d_common.cuh"
 #endif
+#include "fir_adjoint.cuh"
 #include "sins_bank_math.cuh"
 
 namespace {
@@ -61,39 +62,6 @@ struct FirSmem {
     double cum[kMaxBins + 3];
     double part[2 * kThreads];
 };
-
-// inclusive prefix (reverse = false) or suffix (reverse = true) sums of val[0, n) in fp64 into out, n <= 3 kThreads.
-// Thread t owns scan positions [t per, (t + 1) per); the chunk totals are combined by a Hillis-Steele scan.  The
-// summation order depends only on n.  Ends with a barrier.
-__device__ void block_scan(const float* val, double* out, int n, bool reverse, double* part) {
-    const int tid = threadIdx.x;
-    const int per = (n + kThreads - 1) / kThreads;
-    double run = 0.0;
-    for (int q = 0; q < per; ++q) {
-        const int pos = tid * per + q;
-        if (pos < n) {
-            const int i = reverse ? n - 1 - pos : pos;
-            run += (double)val[i];
-            out[i] = run;
-        }
-    }
-    part[tid] = run;
-    __syncthreads();
-    int src = 0;
-    for (int off = 1; off < kThreads; off <<= 1) {
-        double s = part[src * kThreads + tid];
-        if (tid >= off) s += part[src * kThreads + tid - off];
-        part[(1 - src) * kThreads + tid] = s;
-        __syncthreads();
-        src = 1 - src;
-    }
-    const double before = tid > 0 ? part[src * kThreads + tid - 1] : 0.0;
-    for (int q = 0; q < per; ++q) {
-        const int pos = tid * per + q;
-        if (pos < n) out[reverse ? n - 1 - pos : pos] += before;
-    }
-    __syncthreads();
-}
 
 __global__ void __launch_bounds__(kThreads) sins_fir_bwd_kernel(FirBwdParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -162,24 +130,7 @@ __global__ void __launch_bounds__(kThreads) sins_fir_bwd_kernel(FirBwdParams p) 
         // ---- dh: thread owns taps 4 tid .. 4 tid + 3; an 8-float register window slides along the cotangent ----
         {
             float acc[4] = {0.f, 0.f, 0.f, 0.f};
-            if (4 * tid < L) {
-                const float4* g4 = reinterpret_cast<const float4*>(s.gw);
-                const float4* v4 = reinterpret_cast<const float4*>(s.v);
-                float4 cur = g4[tid];
-                for (int q = 0; q < 2 * kP / 4; ++q) {
-                    const float4 nx = g4[q + tid + 1];
-                    const float4 vv = v4[q];
-                    const float w[8] = {cur.x, cur.y, cur.z, cur.w, nx.x, nx.y, nx.z, nx.w};
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        acc[k] = fmaf(vv.x, w[k], acc[k]);
-                        acc[k] = fmaf(vv.y, w[k + 1], acc[k]);
-                        acc[k] = fmaf(vv.z, w[k + 2], acc[k]);
-                        acc[k] = fmaf(vv.w, w[k + 3], acc[k]);
-                    }
-                    cur = nx;
-                }
-            }
+            if (4 * tid < L) b2d_firadj::corr4(s.gw, s.v, tid, 2 * kP / 4, acc);
 #pragma unroll
             for (int k = 0; k < 4; ++k)
                 if (4 * tid + k < L) s.dh[4 * tid + k] = acc[k];
@@ -217,7 +168,7 @@ __global__ void __launch_bounds__(kThreads) sins_fir_bwd_kernel(FirBwdParams p) 
             }
             *reinterpret_cast<float4*>(p.dx + row + (size_t)f * kP + 4 * tid) = make_float4(o[0], o[1], o[2], o[3]);
         }
-        if (harm) block_scan(s.tmp, s.cum, M, false, s.part);    // forward phase phi_j = cumsum(pi tanh c) (barrier)
+        if (harm) b2d_firadj::block_scan<kThreads>(s.tmp, s.cum, M, false, s.part);    // forward phase phi_j = cumsum(pi tanh c) (barrier)
         else __syncthreads();
 
         // ---- un-roll the causal form: dr[n] = dh[(n + L/2) mod L] (noise: times the Hann window of that tap) ----
@@ -283,7 +234,7 @@ __global__ void __launch_bounds__(kThreads) sins_fir_bwd_kernel(FirBwdParams p) 
         }
         if (harm) {
             __syncthreads();
-            block_scan(s.tmp, s.cum, M, true, s.part);          // reverse cumsum: d(pi tanh c)_j = sum_{i >= j} dphi_i
+            b2d_firadj::block_scan<kThreads>(s.tmp, s.cum, M, true, s.part);          // reverse cumsum: d(pi tanh c)_j = sum_{i >= j} dphi_i
             for (int j = tid; j < M; j += kThreads) {
                 const float th = tanhf(crow[j]);
                 grow[p.H + j] = ((float)s.cum[j] * B2D_PI_F) * (1.0f - th * th);

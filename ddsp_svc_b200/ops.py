@@ -410,9 +410,50 @@ def _same_stride(named, B, nF):
     return list(parts), dense.stride(1)
 
 
+COMBSUB_GRAD_MAX_MAG = 513
+
+
+def combsub_grad_unsupported(block, n_mag_allpass, n_mag_harmonic, n_mag_noise):
+    """None if combsub_synth_backward covers the shape, else why not."""
+    if int(block) != 512:
+        return "block size %d (the backward is built for 512)" % block
+    if max(n_mag_allpass, n_mag_harmonic, n_mag_noise) > COMBSUB_GRAD_MAX_MAG:
+        return "n_mag %d / %d / %d (the backward is built for <= %d)" % (n_mag_allpass, n_mag_harmonic, n_mag_noise,
+                                                                        COMBSUB_GRAD_MAX_MAG)
+    return None
+
+
 def combsub_synth(f0_frames, frame_phase, c_group_delay, c_harmonic, c_noise, block, sampling_rate, noise_in=None,
                   seed=0, utterance_offset=0, infer=True, signal_out=None):
-    """Whole old-CombSub DSP after Unit2Control -> (signal, harmonic, noise) [B, T] each."""
+    """Whole old-CombSub DSP after Unit2Control -> (signal, harmonic, noise) [B, T] each.
+
+    Differentiable with respect to the three controls when one of them requires grad (and grad mode is on), in the
+    training phase (``infer=False``, frame_phase from phase_scan(..., infer=False)): the backward runs
+    combsub_synth_backward with the forward's workspace, noise and seed.  All three outputs are differentiable."""
+    ctrls = (c_group_delay, c_harmonic, c_noise)
+    if torch.is_grad_enabled() and any(isinstance(c, torch.Tensor) and c.requires_grad for c in ctrls):
+        if signal_out is not None:
+            raise ValueError("signal_out cannot be used when the controls require grad (it may be peer-mapped memory "
+                             "that autograd does not own)")
+        if infer:
+            raise NotImplementedError("the CombSub backward covers the training phase only: call with infer=False "
+                                      "(what the reference's solver.py does), or under torch.no_grad() for inference")
+        if isinstance(f0_frames, torch.Tensor) and f0_frames.requires_grad:
+            raise NotImplementedError("CombSub has no gradient with respect to f0_frames; pass f0 as data")
+        why = combsub_grad_unsupported(block, c_group_delay.shape[-1], c_harmonic.shape[-1], c_noise.shape[-1])
+        if why is not None:
+            raise NotImplementedError("the CombSub backward does not cover " + why)
+        if noise_in is not None:
+            noise_in = noise_in.detach()
+        return _CombSubSynth.apply(f0_frames.detach(), frame_phase, int(block), float(sampling_rate), noise_in,
+                                   int(seed), int(utterance_offset), c_group_delay, c_harmonic, c_noise)
+    return _combsub_synth(f0_frames, frame_phase, c_group_delay, c_harmonic, c_noise, block, sampling_rate, noise_in,
+                          seed, utterance_offset, infer, signal_out)[:3]
+
+
+def _combsub_synth(f0_frames, frame_phase, c_group_delay, c_harmonic, c_noise, block, sampling_rate, noise_in=None,
+                   seed=0, utterance_offset=0, infer=True, signal_out=None):
+    """-> (signal, harmonic, noise, workspace)"""
     f0 = _frames_2d(f0_frames)
     B, nF = f0.shape
     _need_frame_phase(frame_phase, B, nF)
@@ -438,7 +479,71 @@ def combsub_synth(f0_frames, frame_phase, c_group_delay, c_harmonic, c_noise, bl
                              noise.data_ptr(), ws.data_ptr(), ws_bytes, _stream())
     _lib.check(rc, "b2d_combsub_synth")
     _count(6 if Ma == Mn else 7)
-    return signal, harmonic, noise
+    return signal, harmonic, noise, ws
+
+
+def combsub_synth_backward(f0_frames, c_group_delay, c_harmonic, c_noise, ws, grad_signal, block, sampling_rate,
+                           grad_harmonic=None, grad_noise=None, noise_in=None, seed=0, utterance_offset=0):
+    """Gradient of combsub_synth (infer=False) with respect to the three raw controls, for the cotangents of signal,
+    harmonic and noise [B, T] (None = zero).  f0 / controls / noise_in / seed / utterance_offset must be those of the
+    forward call and ``ws`` the workspace it filled (its comb, all-passed comb and impulse responses).
+    -> dense [B, nF, Ma + Mh + Mn]: group_delay | harmonic_magnitude | noise_magnitude (the split_to_dict layout)."""
+    f0 = _frames_2d(f0_frames)
+    B, nF = f0.shape
+    (cg, ch, cn), stride = _same_stride([("group_delay", c_group_delay), ("harmonic_magnitude", c_harmonic),
+                                         ("noise_magnitude", c_noise)], B, nF)
+    Ma, Mh, Mn = cg.shape[2], ch.shape[2], cn.shape[2]
+    T = nF * int(block)
+    if noise_in is not None:
+        noise_in = _noise_rows(noise_in, B, T)
+    L = _lib.lib()
+    if not isinstance(ws, torch.Tensor) or not ws.is_cuda or ws.dtype != torch.uint8 or \
+            ws.numel() < L.b2d_combsub_workspace_bytes(B, nF, int(block), Ma, Mh, Mn):
+        raise ValueError("ws must be the workspace combsub_synth filled for the same shapes")
+    cots = []
+    for name, g in (("grad_signal", grad_signal), ("grad_harmonic", grad_harmonic), ("grad_noise", grad_noise)):
+        if g is not None:
+            _need_cuda_f32(name, g)
+            if tuple(g.shape) != (B, T):
+                raise ValueError("%s must be [B, n_frames*block] = [%d, %d], got %s" % (name, B, T, tuple(g.shape)))
+            g = g.contiguous()
+        cots.append(g)
+    grad = torch.empty(B, nF, Ma + Mh + Mn, dtype=torch.float32, device=f0.device)
+    bws_bytes = L.b2d_combsub_synth_backward_workspace_bytes(B, nF, int(block))
+    bws = torch.empty(bws_bytes, dtype=torch.uint8, device=f0.device)
+    rc = L.b2d_combsub_synth_backward(f0.data_ptr(), cg.data_ptr(), ch.data_ptr(), cn.data_ptr(), stride,
+                                      _ptr(noise_in), int(seed), int(utterance_offset), ws.data_ptr(), _ptr(cots[0]),
+                                      _ptr(cots[1]), _ptr(cots[2]), B, nF, int(block), Ma, Mh, Mn,
+                                      float(sampling_rate), grad.data_ptr(), bws.data_ptr(), bws_bytes, _stream())
+    _lib.check(rc, "b2d_combsub_synth_backward")
+    _count(2)
+    return grad
+
+
+class _CombSubSynth(torch.autograd.Function):
+    """combsub_synth (infer=False) with a CUDA backward.  Saves the forward's workspace (comb | all-passed comb | noise
+    | impulse responses), f0, the control views and the noise input; the backward regenerates the in-kernel noise from
+    seed."""
+
+    @staticmethod
+    def forward(ctx, f0, frame_phase, block, sampling_rate, noise_in, seed, utterance_offset, c_gd, c_hm, c_nm):
+        signal, harmonic, noise, ws = _combsub_synth(f0, frame_phase, c_gd, c_hm, c_nm, block, sampling_rate, noise_in,
+                                                     seed, utterance_offset, False, None)
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(ws, f0, noise_in, c_gd, c_hm, c_nm)
+        ctx.cfg = (block, sampling_rate, seed, utterance_offset)
+        return signal, harmonic, noise
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_signal, grad_harmonic, grad_noise):
+        ws, f0, noise_in, c_gd, c_hm, c_nm = ctx.saved_tensors
+        block, sampling_rate, seed, utterance_offset = ctx.cfg
+        grad = combsub_synth_backward(f0, c_gd, c_hm, c_nm, ws, grad_signal, block, sampling_rate,
+                                      grad_harmonic=grad_harmonic, grad_noise=grad_noise, noise_in=noise_in, seed=seed,
+                                      utterance_offset=utterance_offset)
+        parts = torch.split(grad, [c_gd.shape[-1], c_hm.shape[-1], c_nm.shape[-1]], dim=-1)
+        return (None,) * 7 + tuple(parts)
 
 
 def superfast_scan(f0_frames, block, sampling_rate):

@@ -53,13 +53,6 @@ class _SynthBase(torch.nn.Module):
         super()._load_from_state_dict(*a, **k)
         self.__dict__["_scalar_cache"] = None
 
-    @staticmethod
-    def _forward_only(ctrls):
-        if torch.is_grad_enabled() and any(v.requires_grad for v in ctrls.values()):
-            raise NotImplementedError(
-                "the synthesis kernels are forward-only; call under torch.no_grad() "
-                "(every inference caller of the reference does, e.g. main.py:250)")
-
 
 class Sins(_SynthBase):
     """Sinusoids additive synthesiser -- reference ddsp/vocoder.py:532-611."""
@@ -137,11 +130,33 @@ class CombSub(_SynthBase):
 
     def forward(self, units_frames, f0_frames, volume_frames, spk_id=None, spk_mix_dict=None, initial_phase=None,
                 infer=True, noise=None, utterance_offset=0, signal_out=None, **kwargs):
+        """units_frames B x n_frames x n_unit; f0_frames B x n_frames x 1; volume_frames B x n_frames x 1.
+        ``signal_out``: optional preallocated [B, T] destination of ``signal`` (may be peer-mapped memory).
+
+        Trainable in the training phase: with ``infer=False`` (what the reference's solver.py calls) and a control
+        from ``unit2ctrl`` that requires grad (grad mode on), signal, harmonic and noise are differentiable with
+        respect to the three controls (CUDA backward, ops.combsub_synth_backward) for block 512 and n_mag <= 513.
+        f0 is data, as in the reference's train.py: an f0 that requires grad is refused."""
         sr, block = self._scalars()
+        if torch.is_grad_enabled() and isinstance(f0_frames, torch.Tensor) and f0_frames.requires_grad:
+            raise NotImplementedError("CombSub has no gradient with respect to f0_frames; pass f0 as data "
+                                      "(f0_frames.detach()), as the reference's train.py does")
         frame_phase, phase_frames = ops.phase_scan(f0_frames, block, sr, initial_phase, infer)
         ctrls, hidden = self.unit2ctrl(units_frames, f0_frames, phase_frames, volume_frames, spk_id=spk_id,
                                        spk_mix_dict=spk_mix_dict)
-        self._forward_only(ctrls)
+        if torch.is_grad_enabled() and any(v.requires_grad for v in ctrls.values()):
+            if infer:
+                raise NotImplementedError(
+                    "CombSub is differentiable in the training phase only: call it with infer=False (what the "
+                    "reference's solver.py does), or under torch.no_grad() for inference (main.py:250)")
+            if signal_out is not None:
+                raise ValueError("signal_out cannot be combined with controls that require grad; call under "
+                                 "torch.no_grad() or drop signal_out")
+            why = ops.combsub_grad_unsupported(block, ctrls["group_delay"].shape[-1],
+                                               ctrls["harmonic_magnitude"].shape[-1],
+                                               ctrls["noise_magnitude"].shape[-1])
+            if why is not None:
+                raise NotImplementedError("the CombSub backward does not cover " + why)
         signal, harmonic, noise_out = ops.combsub_synth(
             f0_frames, frame_phase, ctrls["group_delay"], ctrls["harmonic_magnitude"], ctrls["noise_magnitude"],
             block, sr, noise_in=noise, seed=0 if noise is not None else _host_seed(),

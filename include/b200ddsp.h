@@ -214,6 +214,26 @@ int    b2d_combsub_synth(const float* f0_frames, const double* frame_phase,
                          float* signal, float* harmonic, float* noise_out,
                          void* workspace, size_t workspace_bytes, void* stream);
 
+/* Backward of b2d_combsub_synth in the training phase (round_fp32 = 1, infer=False) with respect
+ * to the three raw controls.                         ddsp/vocoder.py:834-862 under autograd
+ * grad_ctrl: dense [B, n_frames, Ma + Mh + Mn] = group_delay | harmonic_magnitude |
+ * noise_magnitude (the split_to_dict layout), every element written.  grad_signal /
+ * grad_harmonic / grad_noise: [B, T] cotangents of the three outputs, NULL = zero.
+ * forward_workspace: what b2d_combsub_synth filled for the same arguments (its comb, all-passed
+ * comb and impulse responses).  f0_frames, controls, noise_in, seed and utterance_offset: those of
+ * the forward call (the in-kernel noise is regenerated).  workspace: dL/d(all-passed comb), [B, T].
+ * Built for block 512, 2 <= n_mag <= 513 (up to 1024 taps).  Deterministic: no atomics; the
+ * result depends neither on the grid nor on b2d_set_overlap. */
+size_t b2d_combsub_synth_backward_workspace_bytes(int B, int n_frames, int block);
+int    b2d_combsub_synth_backward(const float* f0_frames, const float* c_group_delay,
+                                  const float* c_harmonic, const float* c_noise, int64_t ctrl_stride,
+                                  const float* noise_in, uint64_t seed, int64_t utterance_offset,
+                                  const void* forward_workspace, const float* grad_signal,
+                                  const float* grad_harmonic, const float* grad_noise, int B,
+                                  int n_frames, int block, int n_mag_allpass, int n_mag_harmonic,
+                                  int n_mag_noise, double sampling_rate, float* grad_ctrl,
+                                  void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * CombSubSuperFast (what configs/combsub.yaml selects).   replaces ddsp/vocoder.py:639-710
  * Two steps around Unit2Control, like the reference:
