@@ -22,14 +22,10 @@
 
 namespace {
 
-constexpr int kP = 512;                      // block size the backward is built for
+using b2d_firadj::kP;                        // block size the backward is built for
+using b2d_firadj::kThreads;
 constexpr int kMaxTaps = 1024;               // 2 (n_mag - 1), n_mag <= 513
 constexpr int kMaxBins = kMaxTaps / 2 + 1;
-constexpr int kThreads = 128;
-constexpr int kWin = 2 * kP + kMaxTaps + 4;  // cotangent window of one frame (+ the register window's overhang)
-using b2d_firadj::kSub;
-
-enum Filter { kAllpass = 0, kHarmonic = 1, kNoise = 2 };
 
 struct CsBwdParams {
     const float* comb;        // [B, T] the forward's comb source
@@ -52,166 +48,30 @@ struct CsBwdParams {
     float* grad;              // dense [B, nF, Ma + Mh + Mn]
 };
 
-struct CsSmem {
-    float gw[kWin];                    // cotangent window, origin at sample (f-1)P - L/2
-    float v[2 * kP];                   // weighted filter input of hops f-1, f
-    float hA[kMaxTaps], hB[kMaxTaps];  // h_f, h_{f+1} of the harmonic filter, zero-padded
-    float dh[kMaxTaps];
-    float cosT[kMaxTaps], sinT[kMaxTaps];   // cos / sin(2 pi t / N)
-    float2 eo[kMaxTaps / 2];           // (dr[n] + dr[N-n], dr[n] - dr[N-n]) for 1 <= n < N/2, zero elsewhere
-    float d0, dN;                      // dr[0], dr[N/2]
-    float tmp[kMaxBins + 3];
-    double cum[kMaxBins + 3];
-    double part[2 * kThreads];
-};
-
-__device__ void filter_bwd(const CsBwdParams& p, CsSmem& s, Filter which) {
-    const int f = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
-    const int nF = p.nF;
-    const long long T = (long long)nF * kP;
-    const size_t row = (size_t)b * (size_t)T;
-    const size_t frow = (size_t)b * nF + f;
-    float* grow = p.grad + frow * (size_t)(p.Ma + p.Mh + p.Mn);
-    const bool ap = which == kAllpass, harm = which == kHarmonic;
-    const int M = ap ? p.Ma : harm ? p.Mh : p.Mn, L = 2 * (M - 1), N = L, half = L / 2;
-    const float* g1 = ap ? p.da : p.g;
-    const float* g2 = ap ? nullptr : harm ? p.g_harm : p.g_noise;
-    const float* crow = (ap ? p.c_gd : harm ? p.c_hm : p.c_nm) + frow * (size_t)p.ctrl_stride;
-    const long long n0 = (long long)(f - 1) * kP - half;
-
-    // ---- stage: cotangent window, weighted input, filter rows, DFT table, raw activations ----
-    for (int i = tid; i < kWin; i += kThreads) {
-        const long long n = n0 + i;
-        float v = 0.f;
-        if (i < 2 * kP + L - 1 && n >= 0 && n < T) {
-            if (g1) v = g1[row + n];
-            if (g2) v += g2[row + n];
-        }
-        s.gw[i] = v;
-    }
-    for (int q = tid; q < 2 * kP / 4; q += kThreads) {
-        const int i = 4 * q;
-        const long long m = (long long)(f - 1) * kP + i;
-        float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (m >= 0 && m < T) {          // whole quads: m and T are multiples of 4
-            if (ap) x = *reinterpret_cast<const float4*>(p.comb + row + m);
-            else if (harm) x = *reinterpret_cast<const float4*>(p.allpassed + row + m);
-            else if (p.noise_in) x = *reinterpret_cast<const float4*>(p.noise_in + row + m);
-            else x = b2d::philox_uniform_pm1(p.seed, (unsigned long long)(p.utt_off + b), (uint32_t)(m >> 2));
-        }
-        const float xs[4] = {x.x, x.y, x.z, x.w};
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const int ii = i + k;
-            float w;
-            if (ii < kP) w = (float)ii * (1.0f / kP);                                  // hop f-1: phi
-            else w = (f == nF - 1) ? 1.0f : 1.0f - (float)(ii - kP) * (1.0f / kP);    // hop f: 1 - phi (+ held row)
-            s.v[ii] = w * xs[k];
-        }
-    }
-    if (harm) {
-        const float* ir = p.ir_h + (size_t)b * nF * L;
-        const int f1 = min(f + 1, nF - 1);
-        for (int t = tid; t < kMaxTaps; t += kThreads) {
-            s.hA[t] = t < L ? ir[(size_t)f * L + t] : 0.f;
-            s.hB[t] = t < L ? ir[(size_t)f1 * L + t] : 0.f;
-        }
-    }
-    for (int t = tid; t < N; t += kThreads) {
-        double sd, cd;
-        sincospi(2.0 * (double)t / (double)N, &sd, &cd);
-        s.cosT[t] = (float)cd;
-        s.sinT[t] = (float)sd;
-    }
-    if (ap)
-        for (int j = tid; j < M; j += kThreads) s.tmp[j] = B2D_PI_F * tanhf(crow[j]);   // the forward's pi tanh(c)
-    __syncthreads();
-
-    // ---- dh: thread owns taps 4 t4 .. 4 t4 + 3 for t4 = tid, tid + 128 ----
-#pragma unroll 1
-    for (int grp = 0; grp < kMaxTaps / (4 * kThreads); ++grp) {
-        const int t4 = tid + grp * kThreads;
-        float acc[4] = {0.f, 0.f, 0.f, 0.f};
-        if (4 * t4 < L) b2d_firadj::corr4(s.gw, s.v, t4, 2 * kP / 4, acc);
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-            if (4 * t4 + k < L) s.dh[4 * t4 + k] = acc[k];
-    }
-    // ---- da of hop f (harmonic filter only): thread owns samples 4 tid .. 4 tid + 3 ----
-    if (harm) {
-        float a[4] = {0.f, 0.f, 0.f, 0.f}, c[4] = {0.f, 0.f, 0.f, 0.f};
-        b2d_firadj::fir_t4(s.gw + kP, s.hA, s.hB, tid, (L + 3) / 4, a, c);
-        float o[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const float ph = (float)(4 * tid + k) * (1.0f / kP);
-            o[k] = fmaf(1.0f - ph, a[k], ph * c[k]);
-        }
-        *reinterpret_cast<float4*>(p.da + row + (size_t)f * kP + 4 * tid) = make_float4(o[0], o[1], o[2], o[3]);
-    }
-    if (ap) b2d_firadj::block_scan<kThreads>(s.tmp, s.cum, M, false, s.part);   // forward phase phi_j (barrier)
-    else __syncthreads();
-
-    // ---- un-roll the causal form: dr[n] = dh[(n + L/2) mod L] times the window of that tap ----
-    const float hw = harm ? p.hw_num / (p.f0[frow] + 1e-3f) : 1.f;
-    auto dr = [&](int n) -> float {
-        int t = n + half;
-        if (t >= L) t -= L;
-        const float v = s.dh[t];
-        if (ap) return v;
-        if (!harm) return v * (0.5f - 0.5f * s.cosT[t]);                 // periodic Hann
-        float u = (float)(t - (M - 1)) / hw;                             // dynamic raised cosine, ir_build_tc.cu's
-        if (u > 1.f) u = 0.f;                                            // formula: cos(pi u) by exact period
-        const float r = fmaf(-2.0f, rintf(0.5f * u), u);                 // reduction (cosf's large-argument path
-        return v * ((1.f + __cosf(B2D_PI_F * r)) * 0.5f);                // would put a stack frame here)
-    };
-    for (int n = tid; n < kMaxTaps / 2; n += kThreads) {
-        float2 e = make_float2(0.f, 0.f);
-        if (n >= 1 && n < half) {
-            const float lo = dr(n), hi = dr(N - n);
-            e = make_float2(lo + hi, lo - hi);
-        }
-        s.eo[n] = e;
-    }
-    if (tid == 0) { s.d0 = dr(0); s.dN = dr(half); }
-    __syncthreads();
-
-    // ---- adjoint of irfft per bin, then the activation ----
-    const int nblk = (half + kSub - 1) / kSub;
-    for (int j = tid; j < M; j += kThreads) {
-        float dre, dim;
-        b2d_firadj::irfft_adjoint_bin(j, M, N, nblk, s.cosT, s.sinT, s.eo, s.d0, s.dN, dre, dim);
-        if (ap) {
-            float sn, cs;
-            sincosf((float)s.cum[j], &sn, &cs);
-            s.tmp[j] = dim * cs - dre * sn;                    // dphi_j = Im(dH conj(H))
-        } else if (harm) {
-            grow[p.Ma + j] = dre * expf(crow[j]);
-        } else {
-            grow[p.Ma + p.Mh + j] = (dre * 0.0078125f) * expf(crow[j]);
-        }
-    }
-    if (ap) {
-        __syncthreads();
-        b2d_firadj::block_scan<kThreads>(s.tmp, s.cum, M, true, s.part);    // reverse cumsum: sum_{i >= j} dphi_i
-        for (int j = tid; j < M; j += kThreads) {
-            const float th = tanhf(crow[j]);
-            grow[j] = ((float)s.cum[j] * B2D_PI_F) * (1.0f - th * th);
-        }
-    }
-    __syncthreads();   // the next filter restages every buffer
-}
+using CsSmem = b2d_firadj::FirSmem<kMaxTaps>;
 
 // stage 1: harmonic filter (dh_h, da) and noise filter; stage 2: all-pass filter on da
 template <int STAGE>
 __global__ void __launch_bounds__(kThreads) combsub_bwd_kernel(CsBwdParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     CsSmem& s = *reinterpret_cast<CsSmem*>(smem_raw);
+    const size_t frow = (size_t)blockIdx.y * p.nF + blockIdx.x;
+    float* grow = p.grad + frow * (size_t)(p.Ma + p.Mh + p.Mn);
+    b2d_firadj::FirArgs a{};
+    a.nF = p.nF; a.seed = p.seed; a.utt_off = p.utt_off; a.grad_row = grow;
     if (STAGE == 1) {
-        filter_bwd(p, s, kHarmonic);
-        filter_bwd(p, s, kNoise);
+        a.M = p.Mh; a.x = p.allpassed; a.g = p.g; a.g_add = p.g_harm; a.ir = p.ir_h; a.dx = p.da;
+        a.f0 = p.f0 + frow; a.hw_num = p.hw_num;
+        a.ctrl = p.c_hm + frow * (size_t)p.ctrl_stride; a.col = p.Ma;
+        b2d_firadj::fir_adjoint<b2d_firadj::kHarmonic>(s, a);
+
+        a.M = p.Mn; a.x = p.noise_in; a.g_add = p.g_noise; a.ir = nullptr; a.dx = nullptr;
+        a.ctrl = p.c_nm + frow * (size_t)p.ctrl_stride; a.col = p.Ma + p.Mh;
+        b2d_firadj::fir_adjoint<b2d_firadj::kNoise>(s, a);
     } else {
-        filter_bwd(p, s, kAllpass);
+        a.M = p.Ma; a.x = p.comb; a.g = p.da;
+        a.ctrl = p.c_gd + frow * (size_t)p.ctrl_stride; a.col = 0;
+        b2d_firadj::fir_adjoint<b2d_firadj::kAllpass>(s, a);
     }
 }
 

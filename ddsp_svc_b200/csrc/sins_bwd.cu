@@ -25,12 +25,10 @@
 
 namespace {
 
-constexpr int kP = 512;                      // block size the backward is built for
+using b2d_firadj::kP;                        // block size the backward is built for
+using b2d_firadj::kThreads;
 constexpr int kMaxTaps = 512;                // 2 (n_mag - 1), n_mag <= 257
 constexpr int kMaxBins = kMaxTaps / 2 + 1;
-constexpr int kThreads = 128;
-constexpr int kWin = 2 * kP + kMaxTaps + 4;  // cotangent window of one frame (+ the register window's overhang)
-constexpr int kSub = 16;                     // DFT adjoint: n = kSub a + r, exact table twiddles per (bin, r) and per a
 
 struct FirBwdParams {
     const float* sinus;       // [B, T] the forward's oscillator-bank output
@@ -50,198 +48,23 @@ struct FirBwdParams {
     float* grad;              // dense [B, nF, H + Ma + Mn]
 };
 
-struct FirSmem {
-    float gw[kWin];                    // cotangent window, origin at sample (f-1)P - L/2
-    float v[2 * kP];                   // weighted filter input of hops f-1, f
-    float hA[kMaxTaps], hB[kMaxTaps];  // h_f, h_{f+1}, zero-padded
-    float dh[kMaxTaps];
-    float cosT[kMaxTaps], sinT[kMaxTaps];   // cos / sin(2 pi t / N)
-    float2 eo[kMaxTaps / 2];           // (dr[n] + dr[N-n], dr[n] - dr[N-n]) for 1 <= n < N/2, zero elsewhere
-    float d0, dN;                      // dr[0], dr[N/2]
-    float tmp[kMaxBins + 3];
-    double cum[kMaxBins + 3];
-    double part[2 * kThreads];
-};
+using FirSmem = b2d_firadj::FirSmem<kMaxTaps>;
 
 __global__ void __launch_bounds__(kThreads) sins_fir_bwd_kernel(FirBwdParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     FirSmem& s = *reinterpret_cast<FirSmem*>(smem_raw);
-    const int f = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
-    const int nF = p.nF;
-    const long long T = (long long)nF * kP;
-    const size_t row = (size_t)b * (size_t)T;
-    const size_t frow = (size_t)b * nF + f;
+    const size_t frow = (size_t)blockIdx.y * p.nF + blockIdx.x;
     float* grow = p.grad + frow * (size_t)(p.H + p.Ma + p.Mn);
+    b2d_firadj::FirArgs a{};
+    a.nF = p.nF; a.seed = p.seed; a.utt_off = p.utt_off; a.grad_row = grow; a.g = p.g;
 
-    for (int branch = 0; branch < 2; ++branch) {
-        const bool harm = branch == 0;
-        const int M = harm ? p.Ma : p.Mn, L = 2 * (M - 1), N = L, half = L / 2;
-        const float* ir = (harm ? p.ir_ap : p.ir_n) + (size_t)b * nF * L;
-        const float* gadd = harm ? p.g_harm : p.g_noise;
-        const float* crow = (harm ? p.c_gd : p.c_nm) + frow * (size_t)p.ctrl_stride;
-        const long long n0 = (long long)(f - 1) * kP - half;
+    a.M = p.Ma; a.x = p.sinus; a.g_add = p.g_harm; a.ir = p.ir_ap; a.dx = p.dx;
+    a.ctrl = p.c_gd + frow * (size_t)p.ctrl_stride; a.col = p.H;
+    b2d_firadj::fir_adjoint<b2d_firadj::kAllpass>(s, a);
 
-        // ---- stage: cotangent window, weighted input, filter rows, DFT table, raw activations ----
-        for (int i = tid; i < kWin; i += kThreads) {
-            const long long n = n0 + i;
-            float v = 0.f;
-            if (i < 2 * kP + L - 1 && n >= 0 && n < T) {
-                if (p.g) v = p.g[row + n];
-                if (gadd) v += gadd[row + n];
-            }
-            s.gw[i] = v;
-        }
-        for (int q = tid; q < 2 * kP / 4; q += kThreads) {
-            const int i = 4 * q;
-            const long long m = (long long)(f - 1) * kP + i;
-            float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (m >= 0 && m < T) {          // whole quads: m and T are multiples of 4
-                if (harm) x = *reinterpret_cast<const float4*>(p.sinus + row + m);
-                else if (p.noise_in) x = *reinterpret_cast<const float4*>(p.noise_in + row + m);
-                else x = b2d::philox_uniform_pm1(p.seed, (unsigned long long)(p.utt_off + b), (uint32_t)(m >> 2));
-            }
-            const float xs[4] = {x.x, x.y, x.z, x.w};
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const int ii = i + k;
-                float w;
-                if (ii < kP) w = (float)ii * (1.0f / kP);                                  // hop f-1: phi
-                else w = (f == nF - 1) ? 1.0f : 1.0f - (float)(ii - kP) * (1.0f / kP);    // hop f: 1 - phi (+ held row)
-                s.v[ii] = w * xs[k];
-            }
-        }
-        if (harm) {
-            const int f1 = min(f + 1, nF - 1);
-            for (int t = tid; t < kMaxTaps; t += kThreads) {
-                s.hA[t] = t < L ? ir[(size_t)f * L + t] : 0.f;
-                s.hB[t] = t < L ? ir[(size_t)f1 * L + t] : 0.f;
-            }
-        }
-        for (int t = tid; t < N; t += kThreads) {
-            double sd, cd;
-            sincospi(2.0 * (double)t / (double)N, &sd, &cd);
-            s.cosT[t] = (float)cd;
-            s.sinT[t] = (float)sd;
-        }
-        for (int j = tid; j < M; j += kThreads)
-            s.tmp[j] = harm ? B2D_PI_F * tanhf(crow[j]) : 0.f;     // the forward's pi tanh(c), scanned below
-        __syncthreads();
-
-        // ---- dh: thread owns taps 4 tid .. 4 tid + 3; an 8-float register window slides along the cotangent ----
-        {
-            float acc[4] = {0.f, 0.f, 0.f, 0.f};
-            if (4 * tid < L) b2d_firadj::corr4(s.gw, s.v, tid, 2 * kP / 4, acc);
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-                if (4 * tid + k < L) s.dh[4 * tid + k] = acc[k];
-        }
-        // ---- dx of hop f (all-pass filter only): thread owns samples 4 tid .. 4 tid + 3 ----
-        if (harm) {
-            float a[4] = {0.f, 0.f, 0.f, 0.f}, c[4] = {0.f, 0.f, 0.f, 0.f};
-            const float4* g4 = reinterpret_cast<const float4*>(s.gw + kP);
-            const float4* hA4 = reinterpret_cast<const float4*>(s.hA);
-            const float4* hB4 = reinterpret_cast<const float4*>(s.hB);
-            const int L4 = (L + 3) / 4;
-            float4 cur = g4[tid];
-            for (int u = 0; u < L4; ++u) {
-                const float4 nx = g4[tid + u + 1];
-                const float4 ha = hA4[u], hb = hB4[u];
-                const float w[8] = {cur.x, cur.y, cur.z, cur.w, nx.x, nx.y, nx.z, nx.w};
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    a[k] = fmaf(ha.x, w[k], a[k]);
-                    a[k] = fmaf(ha.y, w[k + 1], a[k]);
-                    a[k] = fmaf(ha.z, w[k + 2], a[k]);
-                    a[k] = fmaf(ha.w, w[k + 3], a[k]);
-                    c[k] = fmaf(hb.x, w[k], c[k]);
-                    c[k] = fmaf(hb.y, w[k + 1], c[k]);
-                    c[k] = fmaf(hb.z, w[k + 2], c[k]);
-                    c[k] = fmaf(hb.w, w[k + 3], c[k]);
-                }
-                cur = nx;
-            }
-            float o[4];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const float ph = (float)(4 * tid + k) * (1.0f / kP);
-                o[k] = fmaf(1.0f - ph, a[k], ph * c[k]);
-            }
-            *reinterpret_cast<float4*>(p.dx + row + (size_t)f * kP + 4 * tid) = make_float4(o[0], o[1], o[2], o[3]);
-        }
-        if (harm) b2d_firadj::block_scan<kThreads>(s.tmp, s.cum, M, false, s.part);    // forward phase phi_j = cumsum(pi tanh c) (barrier)
-        else __syncthreads();
-
-        // ---- un-roll the causal form: dr[n] = dh[(n + L/2) mod L] (noise: times the Hann window of that tap) ----
-        auto dr = [&](int n) -> float {
-            int t = n + half;
-            if (t >= L) t -= L;
-            const float v = s.dh[t];
-            return harm ? v : v * (0.5f - 0.5f * s.cosT[t]);
-        };
-        for (int n = tid; n < kMaxTaps / 2; n += kThreads) {
-            float2 e = make_float2(0.f, 0.f);
-            if (n >= 1 && n < half) {
-                const float lo = dr(n), hi = dr(N - n);
-                e = make_float2(lo + hi, lo - hi);
-            }
-            s.eo[n] = e;
-        }
-        if (tid == 0) { s.d0 = dr(0); s.dN = dr(half); }
-        __syncthreads();
-
-        // ---- adjoint of irfft per bin j:  C_j = sum_n dr[n] cos(2 pi j n / N),  S_j = sum_n dr[n] sin(2 pi j n / N);
-        // n = kSub a + r: cos / sin of (alpha_a + beta_r) from the exact table entries of alpha_a and beta_r ----
-        const int nblk = (half + kSub - 1) / kSub;
-        for (int j = tid; j < M; j += kThreads) {
-            float cb[kSub], sb[kSub];
-#pragma unroll
-            for (int r = 0; r < kSub; ++r) {
-                const int idx = (j * r) % N;
-                cb[r] = s.cosT[idx];
-                sb[r] = s.sinT[idx];
-            }
-            float C = 0.f, S = 0.f;
-            int ia = 0;
-            const int step = (j * kSub) % N;
-            for (int a = 0; a < nblk; ++a) {
-                float U = 0.f, V = 0.f, U2 = 0.f, V2 = 0.f;
-#pragma unroll
-                for (int r = 0; r < kSub; ++r) {
-                    const float2 e = s.eo[a * kSub + r];
-                    U = fmaf(e.x, cb[r], U);
-                    V = fmaf(e.x, sb[r], V);
-                    U2 = fmaf(e.y, cb[r], U2);
-                    V2 = fmaf(e.y, sb[r], V2);
-                }
-                const float ca = s.cosT[ia], sa = s.sinT[ia];
-                C = fmaf(ca, U, fmaf(-sa, V, C));          // sum e cos(alpha + beta)
-                S = fmaf(sa, U2, fmaf(ca, V2, S));         // sum o sin(alpha + beta)
-                ia += step;
-                if (ia >= N) ia -= N;
-            }
-            C += s.d0 + ((j & 1) ? -s.dN : s.dN);
-            const bool edge = (j == 0 || j == M - 1);
-            const float wj = (edge ? 1.0f : 2.0f) / (float)N;
-            const float dre = wj * C, dim = edge ? 0.f : -wj * S;
-            if (harm) {
-                float sn, cs;
-                sincosf((float)s.cum[j], &sn, &cs);
-                s.tmp[j] = dim * cs - dre * sn;                // dphi_j = Im(dH conj(H))
-            } else {
-                const float c = crow[j];
-                grow[p.H + p.Ma + j] = (dre * 0.0078125f) * expf(c);
-            }
-        }
-        if (harm) {
-            __syncthreads();
-            b2d_firadj::block_scan<kThreads>(s.tmp, s.cum, M, true, s.part);          // reverse cumsum: d(pi tanh c)_j = sum_{i >= j} dphi_i
-            for (int j = tid; j < M; j += kThreads) {
-                const float th = tanhf(crow[j]);
-                grow[p.H + j] = ((float)s.cum[j] * B2D_PI_F) * (1.0f - th * th);
-            }
-        }
-        __syncthreads();   // the next branch restages every buffer
-    }
+    a.M = p.Mn; a.x = p.noise_in; a.g_add = p.g_noise; a.ir = nullptr; a.dx = nullptr;
+    a.ctrl = p.c_nm + frow * (size_t)p.ctrl_stride; a.col = p.H + p.Ma;
+    b2d_firadj::fir_adjoint<b2d_firadj::kNoise>(s, a);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

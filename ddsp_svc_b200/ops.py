@@ -98,6 +98,60 @@ def _ctrl_view(name, c, B, nF):
     return c, c.stride(1)
 
 
+def _same_stride(named, B, nF):
+    """Views of one dense control tensor share a frame stride; otherwise densify."""
+    views = [_ctrl_view(n, c, B, nF) for n, c in named]
+    if len({s for _, s in views}) == 1:
+        return [c for c, _ in views], views[0][1]
+    dense = torch.cat([c.contiguous() for c, _ in views], dim=-1)
+    parts = torch.split(dense, [c.shape[2] for c, _ in views], dim=-1)
+    return list(parts), dense.stride(1)
+
+
+def _signal_dest(signal_out, B, T, device):
+    """where a synthesizer writes its [B, T] mixed signal: a new tensor, or the caller's ``signal_out``"""
+    if signal_out is None:
+        return torch.empty(B, T, dtype=torch.float32, device=device)
+    _need_cuda_f32("signal_out", signal_out, local=False)        # may be peer-mapped memory of another GPU
+    if tuple(signal_out.shape) != (B, T) or not signal_out.is_contiguous():
+        raise ValueError("signal_out must be a contiguous [B, T] tensor")
+    return signal_out
+
+
+def _cotangent(name, g, B, T):
+    """a cotangent of a [B, T] output, checked -> contiguous"""
+    _need_cuda_f32(name, g)
+    if tuple(g.shape) != (B, T):
+        raise ValueError("%s must be [B, n_frames*block] = [%d, %d], got %s" % (name, B, T, tuple(g.shape)))
+    return g.contiguous()
+
+
+def _output_cotangents(grad_signal, grad_harmonic, grad_noise, B, T):
+    """checked cotangents of (signal, harmonic, noise), None = zero"""
+    named = (("grad_signal", grad_signal), ("grad_harmonic", grad_harmonic), ("grad_noise", grad_noise))
+    return [None if g is None else _cotangent(name, g, B, T) for name, g in named]
+
+
+def _grad_gate(synth, unsupported, f0_frames, ctrls, block, infer, signal_out):
+    """True when a synthesizer call must be differentiable (a control requires grad and grad mode is on); raises
+    when its backward does not cover the call.  ``unsupported``: the synthesizer's *_grad_unsupported, called with the
+    block size and the controls' widths."""
+    if not (torch.is_grad_enabled() and any(isinstance(c, torch.Tensor) and c.requires_grad for c in ctrls)):
+        return False
+    if infer:
+        raise NotImplementedError("the %s backward covers the training phase only: call with infer=False (what the "
+                                  "reference's solver.py does), or under torch.no_grad() for inference" % synth)
+    if signal_out is not None:
+        raise ValueError("signal_out cannot be used when the controls require grad (it may be peer-mapped memory "
+                         "that autograd does not own)")
+    if isinstance(f0_frames, torch.Tensor) and f0_frames.requires_grad:
+        raise NotImplementedError("%s has no gradient with respect to f0_frames; pass f0 as data" % synth)
+    why = unsupported(block, *(c.shape[-1] for c in ctrls))
+    if why is not None:
+        raise NotImplementedError("the %s backward does not cover %s" % (synth, why))
+    return True
+
+
 def dft_tables(n_mag, device):
     """Constant cos/sin matrices of the 2(n_mag-1)-point inverse real DFT, cached per device."""
     key = (int(n_mag), torch.device(device).index)
@@ -215,19 +269,7 @@ def sins_synth(f0_frames, frame_phase, c_amp, c_group_delay, c_noise, block, sam
     Differentiable with respect to the three controls when one of them requires grad (and grad mode is on), in the
     training phase (``infer=False``, frame_phase from phase_scan(..., infer=False)): the backward runs
     sins_synth_backward with the forward's workspace, noise and seed.  All three outputs are differentiable."""
-    ctrls = (c_amp, c_group_delay, c_noise)
-    if torch.is_grad_enabled() and any(isinstance(c, torch.Tensor) and c.requires_grad for c in ctrls):
-        if signal_out is not None:
-            raise ValueError("signal_out cannot be used when the controls require grad (it may be peer-mapped memory "
-                             "that autograd does not own)")
-        if infer:
-            raise NotImplementedError("the Sins backward covers the training phase only: call with infer=False (what "
-                                      "the reference's solver.py does), or under torch.no_grad() for inference")
-        if isinstance(f0_frames, torch.Tensor) and f0_frames.requires_grad:
-            raise NotImplementedError("Sins has no gradient with respect to f0_frames; pass f0 as data")
-        why = sins_grad_unsupported(block, c_amp.shape[-1], c_group_delay.shape[-1], c_noise.shape[-1])
-        if why is not None:
-            raise NotImplementedError("the Sins backward does not cover " + why)
+    if _grad_gate("Sins", sins_grad_unsupported, f0_frames, (c_amp, c_group_delay, c_noise), block, infer, signal_out):
         if noise_in is not None:
             noise_in = noise_in.detach()
         return _SinsSynth.apply(f0_frames.detach(), frame_phase, int(block), float(sampling_rate), noise_in, int(seed),
@@ -241,17 +283,11 @@ def _sins_args(f0_frames, frame_phase, c_amp, c_group_delay, c_noise, block, noi
     f0 = _frames_2d(f0_frames)
     B, nF = f0.shape
     _need_frame_phase(frame_phase, B, nF)
-    ca, s0 = _ctrl_view("amplitudes", c_amp, B, nF)
-    cg, s1 = _ctrl_view("group_delay", c_group_delay, B, nF)
-    cn, s2 = _ctrl_view("noise_magnitude", c_noise, B, nF)
-    if not (s0 == s1 == s2):  # views of different tensors: densify so one stride describes all
-        ca, cg, cn = ca.contiguous(), cg.contiguous(), cn.contiguous()
-        dense = torch.cat((ca, cg, cn), dim=-1)
-        ca, cg, cn = torch.split(dense, [ca.shape[2], cg.shape[2], cn.shape[2]], dim=-1)
-        s0 = dense.stride(1)
+    (ca, cg, cn), stride = _same_stride([("amplitudes", c_amp), ("group_delay", c_group_delay),
+                                         ("noise_magnitude", c_noise)], B, nF)
     if noise_in is not None:
         noise_in = _noise_rows(noise_in, B, nF * int(block))
-    return f0, ca, cg, cn, s0, noise_in
+    return f0, ca, cg, cn, stride, noise_in
 
 
 def sins_synth_backward(f0_frames, frame_phase, c_amp, c_group_delay, c_noise, ws, grad_signal, block, sampling_rate,
@@ -270,14 +306,7 @@ def sins_synth_backward(f0_frames, frame_phase, c_amp, c_group_delay, c_noise, w
     if not isinstance(ws, torch.Tensor) or not ws.is_cuda or ws.dtype != torch.uint8 or \
             ws.numel() < L.b2d_sins_workspace_bytes(B, nF, int(block), Ma, Mn):
         raise ValueError("ws must be the workspace sins_synth filled for the same shapes")
-    cots = []
-    for name, g in (("grad_signal", grad_signal), ("grad_harmonic", grad_harmonic), ("grad_noise", grad_noise)):
-        if g is not None:
-            _need_cuda_f32(name, g)
-            if tuple(g.shape) != (B, T):
-                raise ValueError("%s must be [B, n_frames*block] = [%d, %d], got %s" % (name, B, T, tuple(g.shape)))
-            g = g.contiguous()
-        cots.append(g)
+    cots = _output_cotangents(grad_signal, grad_harmonic, grad_noise, B, T)
     grad = torch.empty(B, nF, H + Ma + Mn, dtype=torch.float32, device=f0.device)
     bws_bytes = L.b2d_sins_synth_backward_workspace_bytes(B, nF, int(block))
     bws = torch.empty(bws_bytes, dtype=torch.uint8, device=f0.device)
@@ -320,32 +349,15 @@ class _SinsSynth(torch.autograd.Function):
 def _sins_synth(f0_frames, frame_phase, c_amp, c_group_delay, c_noise, block, sampling_rate, noise_in=None,
                 seed=0, utterance_offset=0, infer=True, want_parts=True, signal_out=None):
     """-> (signal, harmonic, noise, workspace)"""
-    f0 = _frames_2d(f0_frames)
+    f0, ca, cg, cn, s0, noise_in = _sins_args(f0_frames, frame_phase, c_amp, c_group_delay, c_noise, block, noise_in)
     B, nF = f0.shape
-    _need_frame_phase(frame_phase, B, nF)
-    ca, s0 = _ctrl_view("amplitudes", c_amp, B, nF)
-    cg, s1 = _ctrl_view("group_delay", c_group_delay, B, nF)
-    cn, s2 = _ctrl_view("noise_magnitude", c_noise, B, nF)
-    if not (s0 == s1 == s2):  # views of different tensors: densify so one stride describes all
-        ca, cg, cn = ca.contiguous(), cg.contiguous(), cn.contiguous()
-        dense = torch.cat((ca, cg, cn), dim=-1)
-        ca, cg, cn = torch.split(dense, [ca.shape[2], cg.shape[2], cn.shape[2]], dim=-1)
-        s0 = dense.stride(1)
     H, Ma, Mn = ca.shape[2], cg.shape[2], cn.shape[2]
     dev = f0.device
     T = nF * block
-    if noise_in is not None:
-        noise_in = _noise_rows(noise_in, B, T)
     L = _lib.lib()
     ws_bytes = L.b2d_sins_workspace_bytes(B, nF, int(block), Ma, Mn)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    if signal_out is not None:
-        _need_cuda_f32("signal_out", signal_out, local=False)        # may be peer-mapped memory of another GPU
-        if tuple(signal_out.shape) != (B, T) or not signal_out.is_contiguous():
-            raise ValueError("signal_out must be a contiguous [B, T] tensor")
-        signal = signal_out
-    else:
-        signal = torch.empty(B, T, dtype=torch.float32, device=dev)
+    signal = _signal_dest(signal_out, B, T, dev)
     harmonic = torch.empty(B, T, dtype=torch.float32, device=dev) if want_parts else None
     noise = torch.empty(B, T, dtype=torch.float32, device=dev) if (want_parts or Ma != Mn) else None
     ta, tn = dft_tables(Ma, dev), dft_tables(Mn, dev)
@@ -400,16 +412,6 @@ def comb_source(f0_frames, frame_phase, block, sampling_rate, infer=True):
     return out
 
 
-def _same_stride(named, B, nF):
-    """Views of one dense control tensor share a frame stride; otherwise densify."""
-    views = [_ctrl_view(n, c, B, nF) for n, c in named]
-    if len({s for _, s in views}) == 1:
-        return [c for c, _ in views], views[0][1]
-    dense = torch.cat([c.contiguous() for c, _ in views], dim=-1)
-    parts = torch.split(dense, [c.shape[2] for c, _ in views], dim=-1)
-    return list(parts), dense.stride(1)
-
-
 COMBSUB_GRAD_MAX_MAG = 513
 
 
@@ -430,19 +432,8 @@ def combsub_synth(f0_frames, frame_phase, c_group_delay, c_harmonic, c_noise, bl
     Differentiable with respect to the three controls when one of them requires grad (and grad mode is on), in the
     training phase (``infer=False``, frame_phase from phase_scan(..., infer=False)): the backward runs
     combsub_synth_backward with the forward's workspace, noise and seed.  All three outputs are differentiable."""
-    ctrls = (c_group_delay, c_harmonic, c_noise)
-    if torch.is_grad_enabled() and any(isinstance(c, torch.Tensor) and c.requires_grad for c in ctrls):
-        if signal_out is not None:
-            raise ValueError("signal_out cannot be used when the controls require grad (it may be peer-mapped memory "
-                             "that autograd does not own)")
-        if infer:
-            raise NotImplementedError("the CombSub backward covers the training phase only: call with infer=False "
-                                      "(what the reference's solver.py does), or under torch.no_grad() for inference")
-        if isinstance(f0_frames, torch.Tensor) and f0_frames.requires_grad:
-            raise NotImplementedError("CombSub has no gradient with respect to f0_frames; pass f0 as data")
-        why = combsub_grad_unsupported(block, c_group_delay.shape[-1], c_harmonic.shape[-1], c_noise.shape[-1])
-        if why is not None:
-            raise NotImplementedError("the CombSub backward does not cover " + why)
+    if _grad_gate("CombSub", combsub_grad_unsupported, f0_frames, (c_group_delay, c_harmonic, c_noise), block, infer,
+                  signal_out):
         if noise_in is not None:
             noise_in = noise_in.detach()
         return _CombSubSynth.apply(f0_frames.detach(), frame_phase, int(block), float(sampling_rate), noise_in,
@@ -466,12 +457,8 @@ def _combsub_synth(f0_frames, frame_phase, c_group_delay, c_harmonic, c_noise, b
     L = _lib.lib()
     ws_bytes = L.b2d_combsub_workspace_bytes(B, nF, int(block), Ma, Mh, Mn)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    signal, harmonic, noise = (torch.empty(B, T, dtype=torch.float32, device=dev) for _ in range(3))
-    if signal_out is not None:
-        _need_cuda_f32("signal_out", signal_out, local=False)        # may be peer-mapped memory of another GPU
-        if tuple(signal_out.shape) != (B, T) or not signal_out.is_contiguous():
-            raise ValueError("signal_out must be a contiguous [B, T] tensor")
-        signal = signal_out
+    signal = _signal_dest(signal_out, B, T, dev)
+    harmonic, noise = (torch.empty(B, T, dtype=torch.float32, device=dev) for _ in range(2))
     rc = L.b2d_combsub_synth(f0.data_ptr(), frame_phase.data_ptr(), cg.data_ptr(), ch.data_ptr(), cn.data_ptr(),
                              stride, _ptr(noise_in), int(seed), int(utterance_offset), dft_tables(Ma, dev).data_ptr(),
                              dft_tables(Mh, dev).data_ptr(), dft_tables(Mn, dev).data_ptr(), B, nF, int(block), Ma,
@@ -500,14 +487,7 @@ def combsub_synth_backward(f0_frames, c_group_delay, c_harmonic, c_noise, ws, gr
     if not isinstance(ws, torch.Tensor) or not ws.is_cuda or ws.dtype != torch.uint8 or \
             ws.numel() < L.b2d_combsub_workspace_bytes(B, nF, int(block), Ma, Mh, Mn):
         raise ValueError("ws must be the workspace combsub_synth filled for the same shapes")
-    cots = []
-    for name, g in (("grad_signal", grad_signal), ("grad_harmonic", grad_harmonic), ("grad_noise", grad_noise)):
-        if g is not None:
-            _need_cuda_f32(name, g)
-            if tuple(g.shape) != (B, T):
-                raise ValueError("%s must be [B, n_frames*block] = [%d, %d], got %s" % (name, B, T, tuple(g.shape)))
-            g = g.contiguous()
-        cots.append(g)
+    cots = _output_cotangents(grad_signal, grad_harmonic, grad_noise, B, T)
     grad = torch.empty(B, nF, Ma + Mh + Mn, dtype=torch.float32, device=f0.device)
     bws_bytes = L.b2d_combsub_synth_backward_workspace_bytes(B, nF, int(block))
     bws = torch.empty(bws_bytes, dtype=torch.uint8, device=f0.device)
@@ -601,11 +581,7 @@ def superfast_synth_backward(ws, c_hm, c_hp, c_nm, c_np, grad_signal, block, win
     source spectra and regenerates the in-kernel noise).  -> dense [B, nF, 4*(win_length/2+1)]: harmonic_magnitude |
     harmonic_phase | noise_magnitude | noise_phase along the last axis (the split_to_dict layout)."""
     (hm, hp, nm, npz), stride, noise_in, B, nF = _superfast_args(ws, c_hm, c_hp, c_nm, c_np, block, win_length, noise_in)
-    _need_cuda_f32("grad_signal", grad_signal)
-    if tuple(grad_signal.shape) != (B, nF * block):
-        raise ValueError("grad_signal must be [B, n_frames*block] = [%d, %d], got %s"
-                         % (B, nF * block, tuple(grad_signal.shape)))
-    grad_signal = grad_signal.contiguous()
+    grad_signal = _cotangent("grad_signal", grad_signal, B, nF * block)
     grad = torch.empty(B, nF, 4 * (win_length // 2 + 1), dtype=torch.float32, device=hm.device)
     rc = _lib.lib().b2d_superfast_synth_backward(ws.data_ptr(), hm.data_ptr(), hp.data_ptr(), nm.data_ptr(),
                                                  npz.data_ptr(), stride, _ptr(noise_in), int(seed), int(utterance_offset),
@@ -640,14 +616,7 @@ class _SuperFastSynth(torch.autograd.Function):
 def _superfast_synth(ws, c_hm, c_hp, c_nm, c_np, block, win_length, noise_in=None, seed=0, utterance_offset=0,
                      signal_out=None):
     (hm, hp, nm, npz), stride, noise_in, B, nF = _superfast_args(ws, c_hm, c_hp, c_nm, c_np, block, win_length, noise_in)
-    T = nF * block
-    if signal_out is not None:
-        _need_cuda_f32("signal_out", signal_out, local=False)        # may be peer-mapped memory of another GPU
-        if tuple(signal_out.shape) != (B, T) or not signal_out.is_contiguous():
-            raise ValueError("signal_out must be a contiguous [B, T] tensor")
-        signal = signal_out
-    else:
-        signal = torch.empty(B, T, dtype=torch.float32, device=hm.device)
+    signal = _signal_dest(signal_out, B, nF * block, hm.device)
     rc = _lib.lib().b2d_superfast_synth(ws.data_ptr(), hm.data_ptr(), hp.data_ptr(), nm.data_ptr(), npz.data_ptr(),
                                         stride, _ptr(noise_in), int(seed), int(utterance_offset), B, nF, int(block),
                                         int(win_length), signal.data_ptr(), _stream())
@@ -709,11 +678,7 @@ def combsubfast_filter_backward(comb, c_hm, c_hp, c_nm, grad_signal, block, nois
     source spectra and regenerates the in-kernel noise).  -> dense [B, nF, 3*(block+1)]: harmonic_magnitude |
     harmonic_phase | noise_magnitude along the last axis (the split_to_dict layout)."""
     comb, (hm, hp, nm), stride, noise_in, B, nF = _combsubfast_args(comb, c_hm, c_hp, c_nm, block, noise_in)
-    _need_cuda_f32("grad_signal", grad_signal)
-    if tuple(grad_signal.shape) != (B, nF * block):
-        raise ValueError("grad_signal must be [B, n_frames*block] = [%d, %d], got %s"
-                         % (B, nF * block, tuple(grad_signal.shape)))
-    grad_signal = grad_signal.contiguous()
+    grad_signal = _cotangent("grad_signal", grad_signal, B, nF * block)
     grad = torch.empty(B, nF, 3 * (block + 1), dtype=torch.float32, device=comb.device)
     rc = _lib.lib().b2d_combsubfast_filter_backward(comb.data_ptr(), hm.data_ptr(), hp.data_ptr(), nm.data_ptr(), stride,
                                                     _ptr(noise_in), int(seed), int(utterance_offset),

@@ -90,18 +90,6 @@ class Sins(_SynthBase):
         frame_phase, phase_frames = ops.phase_scan(f0_frames, block, sr, initial_phase, infer)
         ctrls, hidden = self.unit2ctrl(units_frames, f0_frames, phase_frames, volume_frames, spk_id=spk_id,
                                        spk_mix_dict=spk_mix_dict)
-        if torch.is_grad_enabled() and any(v.requires_grad for v in ctrls.values()):
-            if infer:
-                raise NotImplementedError(
-                    "Sins is differentiable in the training phase only: call it with infer=False (what the "
-                    "reference's solver.py does), or under torch.no_grad() for inference (main.py:250)")
-            if signal_out is not None:
-                raise ValueError("signal_out cannot be combined with controls that require grad; call under "
-                                 "torch.no_grad() or drop signal_out")
-            why = ops.sins_grad_unsupported(block, ctrls["amplitudes"].shape[-1], ctrls["group_delay"].shape[-1],
-                                            ctrls["noise_magnitude"].shape[-1])
-            if why is not None:
-                raise NotImplementedError("the Sins backward does not cover " + why)
         signal, harmonic, noise_out = ops.sins_synth(
             f0_frames, frame_phase, ctrls["amplitudes"], ctrls["group_delay"], ctrls["noise_magnitude"], block, sr,
             noise_in=noise, seed=0 if noise is not None else _host_seed(), utterance_offset=utterance_offset,
@@ -144,19 +132,6 @@ class CombSub(_SynthBase):
         frame_phase, phase_frames = ops.phase_scan(f0_frames, block, sr, initial_phase, infer)
         ctrls, hidden = self.unit2ctrl(units_frames, f0_frames, phase_frames, volume_frames, spk_id=spk_id,
                                        spk_mix_dict=spk_mix_dict)
-        if torch.is_grad_enabled() and any(v.requires_grad for v in ctrls.values()):
-            if infer:
-                raise NotImplementedError(
-                    "CombSub is differentiable in the training phase only: call it with infer=False (what the "
-                    "reference's solver.py does), or under torch.no_grad() for inference (main.py:250)")
-            if signal_out is not None:
-                raise ValueError("signal_out cannot be combined with controls that require grad; call under "
-                                 "torch.no_grad() or drop signal_out")
-            why = ops.combsub_grad_unsupported(block, ctrls["group_delay"].shape[-1],
-                                               ctrls["harmonic_magnitude"].shape[-1],
-                                               ctrls["noise_magnitude"].shape[-1])
-            if why is not None:
-                raise NotImplementedError("the CombSub backward does not cover " + why)
         signal, harmonic, noise_out = ops.combsub_synth(
             f0_frames, frame_phase, ctrls["group_delay"], ctrls["harmonic_magnitude"], ctrls["noise_magnitude"],
             block, sr, noise_in=noise, seed=0 if noise is not None else _host_seed(),
