@@ -30,6 +30,53 @@ inline int check_launch(const char* what) {
 extern std::atomic<int> g_fft_packed;   // debug A/B switch (b2d_set_fft_arith), read once per call
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
+inline size_t align256(size_t bytes) { return (bytes + 255) / 256 * 256; }
+inline float* ws_at(void* ws, size_t off) { return reinterpret_cast<float*>(static_cast<char*>(ws) + off); }
+inline const float* ws_at(const void* ws, size_t off) {
+    return reinterpret_cast<const float*>(static_cast<const char*>(ws) + off);
+}
+// appends a buffer of `floats` floats to a workspace of `bytes` bytes (each buffer 256-byte aligned) -> its offset
+inline size_t ws_append(size_t& bytes, size_t floats) {
+    const size_t off = bytes;
+    bytes += align256(floats * 4);
+    return off;
+}
+
+// Forward workspaces of b2d_sins_synth / b2d_combsub_synth.  The backwards read the forward's buffers back from them, so
+// the drivers, the workspace queries and the backwards all take their byte offsets from here.  bytes == 0: bad shape.
+size_t fir_spec_floats(int B, int nF);     // ltv_fir_fft.cu: one filter's packed spectra
+// sinusoids [B, T] | ir_allpass [B, nF, 2 (Ma - 1)] | ir_noise [B, nF, 2 (Mn - 1)]; with `spectrum` (b2d_set_sins_impl(3))
+// also spec_allpass | spec_noise
+struct SinsWorkspace { size_t sinus, ir_ap, ir_n, spec_ap, spec_n, bytes; };
+inline SinsWorkspace sins_workspace(int B, int nF, int block, int n_mag_allpass, int n_mag_noise, bool spectrum) {
+    SinsWorkspace w{};
+    if (B <= 0 || nF <= 0 || block <= 0 || n_mag_allpass < 2 || n_mag_noise < 2) return w;
+    const size_t T = (size_t)B * nF * block, F = (size_t)B * nF;
+    w.sinus = ws_append(w.bytes, T);
+    w.ir_ap = ws_append(w.bytes, F * 2 * (n_mag_allpass - 1));
+    w.ir_n = ws_append(w.bytes, F * 2 * (n_mag_noise - 1));
+    if (spectrum) {
+        w.spec_ap = ws_append(w.bytes, fir_spec_floats(B, nF));
+        w.spec_n = ws_append(w.bytes, fir_spec_floats(B, nF));
+    }
+    return w;
+}
+// comb [B, T] | allpassed [B, T] | noise [B, T] | ir_allpass | ir_harmonic | ir_noise [B, nF, 2 (M - 1)]
+struct CombSubWorkspace { size_t comb, allpassed, noise, ir_ap, ir_h, ir_n, bytes; };
+inline CombSubWorkspace combsub_workspace(int B, int nF, int block, int n_mag_allpass, int n_mag_harmonic,
+                                          int n_mag_noise) {
+    CombSubWorkspace w{};
+    if (B <= 0 || nF <= 0 || block <= 0 || n_mag_allpass < 2 || n_mag_harmonic < 2 || n_mag_noise < 2) return w;
+    const size_t T = (size_t)B * nF * block, F = (size_t)B * nF;
+    w.comb = ws_append(w.bytes, T);
+    w.allpassed = ws_append(w.bytes, T);
+    w.noise = ws_append(w.bytes, T);
+    w.ir_ap = ws_append(w.bytes, F * 2 * (n_mag_allpass - 1));
+    w.ir_h = ws_append(w.bytes, F * 2 * (n_mag_harmonic - 1));
+    w.ir_n = ws_append(w.bytes, F * 2 * (n_mag_noise - 1));
+    return w;
+}
+
 }  // namespace b2d
 
 // ---------------------------------------------------------------------------------------

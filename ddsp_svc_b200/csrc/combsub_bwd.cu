@@ -79,8 +79,6 @@ __global__ void __launch_bounds__(kThreads) combsub_bwd_kernel(CsBwdParams p) {
 
 #ifndef B2D_HOST_EMU
 namespace {
-inline size_t align256(size_t v) { return (v + 255) / 256 * 256; }
-
 template <int STAGE>
 int stage_launch(const CsBwdParams& p, int B, cudaStream_t st) {
     auto kern = combsub_bwd_kernel<STAGE>;
@@ -95,7 +93,7 @@ int stage_launch(const CsBwdParams& p, int B, cudaStream_t st) {
 
 extern "C" size_t b2d_combsub_synth_backward_workspace_bytes(int B, int n_frames, int block) {
     if (B <= 0 || n_frames <= 0 || block <= 0) return 0;
-    return align256((size_t)B * n_frames * block * 4);     // dL/dallpassed
+    return b2d::align256((size_t)B * n_frames * block * 4);     // dL/dallpassed
 }
 
 extern "C" int b2d_combsub_synth_backward(const float* f0_frames, const float* c_group_delay, const float* c_harmonic,
@@ -124,15 +122,11 @@ extern "C" int b2d_combsub_synth_backward(const float* f0_frames, const float* c
         return b2d::fail(B2D_ERR_ALIGN, "combsub_synth_backward: workspaces must be 256-byte aligned, noise_in 16-byte "
                          "aligned");
 
-    // forward workspace (api.cu b2d_combsub_synth): comb | allpassed | noise | ir_ap | ir_h | ir_n
-    const size_t BT = (size_t)B * n_frames * block, BF = (size_t)B * n_frames;
-    const size_t sBT = align256(BT * 4);
-    const int La = 2 * (n_mag_allpass - 1);
-    const char* fws = static_cast<const char*>(forward_workspace);
+    const b2d::CombSubWorkspace fw = b2d::combsub_workspace(B, n_frames, block, n_mag_allpass, n_mag_harmonic, n_mag_noise);
     CsBwdParams p;
-    p.comb = reinterpret_cast<const float*>(fws);
-    p.allpassed = reinterpret_cast<const float*>(fws + sBT);
-    p.ir_h = reinterpret_cast<const float*>(fws + 3 * sBT + align256(BF * La * 4));
+    p.comb = b2d::ws_at(forward_workspace, fw.comb);
+    p.allpassed = b2d::ws_at(forward_workspace, fw.allpassed);
+    p.ir_h = b2d::ws_at(forward_workspace, fw.ir_h);
     p.noise_in = noise_in; p.seed = seed; p.utt_off = utterance_offset;
     p.f0 = f0_frames; p.hw_num = 1.5f * (float)sampling_rate;
     p.c_gd = c_group_delay; p.c_hm = c_harmonic; p.c_nm = c_noise; p.ctrl_stride = ctrl_stride;

@@ -168,8 +168,6 @@ __global__ void __launch_bounds__(kThreads) sins_bank_bwd_kernel(BankBwdParams p
 
 #ifndef B2D_HOST_EMU
 namespace {
-inline size_t align256(size_t v) { return (v + 255) / 256 * 256; }
-
 template <int G>
 int bank_bwd_launch(const BankBwdParams& p, int B, cudaStream_t st) {
     sins_bank_bwd_kernel<G><<<dim3((unsigned)p.nF, (unsigned)B), kThreads, sizeof(BankSmem), st>>>(p);
@@ -179,7 +177,7 @@ int bank_bwd_launch(const BankBwdParams& p, int B, cudaStream_t st) {
 
 extern "C" size_t b2d_sins_synth_backward_workspace_bytes(int B, int n_frames, int block) {
     if (B <= 0 || n_frames <= 0 || block <= 0) return 0;
-    return 2 * align256((size_t)B * n_frames * block * 4);     // dL/dsinusoids | sinusoids rebuilt when not in the forward's
+    return 2 * b2d::align256((size_t)B * n_frames * block * 4);     // dL/dsinusoids | sinusoids rebuilt when not in the forward's
 }
 
 extern "C" int b2d_sins_synth_backward(const float* f0_frames, const double* frame_phase, const float* c_amp,
@@ -207,17 +205,13 @@ extern "C" int b2d_sins_synth_backward(const float* f0_frames, const double* fra
         (noise_in && !b2d::aligned16(noise_in)) || (reinterpret_cast<uintptr_t>(grad_ctrl) & 3u))
         return b2d::fail(B2D_ERR_ALIGN, "sins_synth_backward: workspaces must be 256-byte aligned, noise_in 16-byte aligned");
 
-    const size_t BT = (size_t)B * n_frames * block, BF = (size_t)B * n_frames;
-    const int La = 2 * (n_mag_allpass - 1);
-    const char* fws = static_cast<const char*>(forward_workspace);
-    const float* ir_ap = reinterpret_cast<const float*>(fws + align256(BT * 4));
-    const float* ir_n = reinterpret_cast<const float*>(fws + align256(BT * 4) + align256(BF * La * 4));
-    char* ws = static_cast<char*>(workspace);
-    float* dx = reinterpret_cast<float*>(ws);
-    const float* sinus = reinterpret_cast<const float*>(fws);
+    // the forward's buffers precede its spectrum buffers, so the spectrum flag does not move them
+    const b2d::SinsWorkspace fw = b2d::sins_workspace(B, n_frames, block, n_mag_allpass, n_mag_noise, false);
+    const float* sinus = b2d::ws_at(forward_workspace, fw.sinus);
+    float* dx = static_cast<float*>(workspace);
     cudaStream_t st = (cudaStream_t)stream;
     if (!forward_has_sinusoids) {     // the fused forward evaluates the bank inside its FIR kernel: rebuild the sinusoids
-        float* rebuilt = reinterpret_cast<float*>(ws + align256(BT * 4));
+        float* rebuilt = b2d::ws_at(workspace, b2d::align256((size_t)B * n_frames * block * 4));
         const int rc = b2d_sins_bank(f0_frames, frame_phase, c_amp, ctrl_stride, B, n_frames, block, n_harmonics,
                                      sampling_rate, 1, rebuilt, stream);
         if (rc) return rc;
@@ -226,7 +220,8 @@ extern "C" int b2d_sins_synth_backward(const float* f0_frames, const double* fra
 
     FirBwdParams fp;
     fp.sinus = sinus; fp.noise_in = noise_in; fp.seed = seed; fp.utt_off = utterance_offset;
-    fp.ir_ap = ir_ap; fp.ir_n = ir_n; fp.c_gd = c_group_delay; fp.c_nm = c_noise; fp.ctrl_stride = ctrl_stride;
+    fp.ir_ap = b2d::ws_at(forward_workspace, fw.ir_ap); fp.ir_n = b2d::ws_at(forward_workspace, fw.ir_n);
+    fp.c_gd = c_group_delay; fp.c_nm = c_noise; fp.ctrl_stride = ctrl_stride;
     fp.g = grad_signal; fp.g_harm = grad_harmonic; fp.g_noise = grad_noise;
     fp.nF = n_frames; fp.Ma = n_mag_allpass; fp.Mn = n_mag_noise; fp.H = n_harmonics;
     fp.dx = dx; fp.grad = grad_ctrl;

@@ -74,15 +74,16 @@ def _kernel_names(fn, *args, **kwargs):
 def profiled(fn, *args, **kwargs):
     """-> (fn(*args, **kwargs), demangled names of the CUDA kernels it launched), recorded by torch.profiler with CUDA
     activities only.  The first profiling session of a process starts CUPTI and comes back without kernel records, so
-    one session around a trivial kernel runs first.  A later session occasionally comes back empty as well; fn (a pure
-    call here) is then run again under a fresh session, up to PROFILE_ATTEMPTS times in all."""
+    one session around a trivial kernel runs first.  A later session occasionally comes back without kernel records as
+    well, either empty or holding only the copies fn made; fn (a pure call here) is then run again under a fresh session,
+    up to PROFILE_ATTEMPTS times in all."""
     global _profiler_started
     if not _profiler_started:
         _kernel_names(lambda: torch.ones(1, device=DEV).add_(1))
         _profiler_started = True
     for _ in range(PROFILE_ATTEMPTS):
         out, names = _kernel_names(fn, *args, **kwargs)
-        if names:
+        if any(not n.startswith(("Memcpy", "Memset")) for n in names):
             break
     return out, names
 
