@@ -76,6 +76,19 @@ SIGNATURES = {
                                                 ctypes.c_float, c_stream]),
     "b2d_u2c_linear_attention": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                                 ctypes.c_int, ctypes.c_int, ctypes.c_float, c_stream]),
+    "b2d_u2c_backward_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int] * 4),
+    "b2d_u2c_glu_dwconv_silu_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int,
+                                                        ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                                        ctypes.c_size_t, c_stream]),
+    "b2d_u2c_colsum": (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, c_f32p, ctypes.c_void_p, ctypes.c_size_t, c_stream]),
+    "b2d_u2c_layernorm_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_float, ctypes.c_int, ctypes.c_int, c_f32p,
+                                                  c_f32p, ctypes.c_void_p, ctypes.c_size_t, c_stream]),
+    "b2d_u2c_groupnorm_lrelu_backward": (ctypes.c_int, [c_f32p, c_f64p, c_f32p, c_f32p, ctypes.c_float, ctypes.c_float, c_f32p,
+                                                        ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p, c_f32p,
+                                                        ctypes.c_void_p, ctypes.c_size_t, c_stream]),
+    "b2d_u2c_embed_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, c_f32p,
+                                              c_f32p, ctypes.c_void_p, ctypes.c_size_t, c_stream]),
+    "b2d_u2c_conv3_fold": (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p, c_stream]),
     "b2d_mel_frames": (ctypes.c_int, [ctypes.c_int] * 4),
     "b2d_mel_spectrogram": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                            ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, c_f32p, c_stream]),

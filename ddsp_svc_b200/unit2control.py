@@ -10,14 +10,22 @@ controls are strided views of ONE dense [B, T, n_out] tensor, which is what the 
 Execution: activations stay token-major [B, T, C].  Plain GEMMs (the k = 3 convolutions as one product over the three
 shifted inputs, 1 x 1 convolutions, attention projections and contractions, dense_out) are library GEMMs (cuBLAS through
 torch.addmm / bmm, fp32); everything between them runs in the fused kernels of csrc/unit2control.cu (embedding sum,
-GroupNorm + LeakyReLU, LayerNorm, GLU + depthwise k = 31 convolution + SiLU, performer feature maps).  Inference only
-(the reference's train.py keeps using its own class); CPU tensors raise.
+GroupNorm + LeakyReLU, LayerNorm, GLU + depthwise k = 31 convolution + SiLU, performer feature maps).  CPU tensors raise.
+
+Training: with the convolution-only decoder (``use_naive_v2=True``: what CombSubSuperFast builds, so configs/combsub.yaml,
+reflow.yaml and diffusion-fast.yaml) the module is differentiable with respect to all of its parameters when grad mode is
+on and a parameter requires grad: ONE autograd Function (_NaiveFunction) around the whole network whose forward is the
+inference forward (same kernels, bit-identical outputs; that decoder has no dropout) plus the saved activations, and whose
+backward walks the layers in reverse on the kernels of csrc/unit2control_bwd.cu and library GEMMs.  The inputs are data:
+units, f0, phase, volume or aug_shift that require grad, and spk_mix_dict under grad, raise NotImplementedError.  The PCmer
+decoder stays inference only (outputs detached in every mode); train it with a differentiable ``unit2ctrl=``.
 """
 import math
 
 import numpy as np
 import torch
 import torch.nn as nn
+from torch.autograd.function import once_differentiable
 from torch.nn.utils import weight_norm
 
 from . import _lib
@@ -165,6 +173,25 @@ class _Gemm:
         out.addmm_(xh, wl.t())
         return out
 
+    def split(self, x2d):
+        """an activation prepared for the products below: (hi, lo) in 3xtf32 mode, itself otherwise"""
+        return _split(x2d) if self.mode == "3xtf32" else x2d.contiguous()
+
+    def grad_input(self, gy, w, out=None):
+        """(out +) gy [N, O] @ w [O, K]: the adjoint of ``linear`` towards its input; gy from ``split``, w packed"""
+        if self.mode != "3xtf32":
+            return torch.mm(gy, w) if out is None else out.addmm_(gy, w)
+        (gh, gl), (wh, wl) = gy, w
+        out = torch.mm(gh, wh) if out is None else out.addmm_(gh, wh)
+        return out.addmm_(gl, wh).addmm_(gh, wl)
+
+    def grad_weight(self, gy, x):
+        """gy^T [O, N] @ x [N, K]: the adjoint of ``linear`` towards its weight; both operands from ``split``"""
+        if self.mode != "3xtf32":
+            return torch.mm(gy.t(), x)
+        (gh, gl), (xh, xl) = gy, x
+        return torch.mm(gh.t(), xh).addmm_(gl.t(), xh).addmm_(gh.t(), xl)
+
     def matmul(self, a, b):
         """batched a @ b of two activations (the per-head contractions of the linear attention: 256 small problems).
         In 3xtf32 mode these stay fp32 SIMT: cuBLAS serves batched TF32 problems of this shape with sm_80 kernels that are
@@ -176,6 +203,112 @@ class _Gemm:
             return torch.matmul(a, b)
         finally:
             torch.backends.cuda.matmul.allow_tf32 = True
+
+
+class _NaiveFunction(torch.autograd.Function):
+    """The whole control network with the convolution-only decoder as ONE differentiable op:
+    (module, parameter names, inputs..., dense_out weight, *parameters) -> (dense [B, T, n_out], hidden [B, T, 256]).
+
+    forward is Unit2Control._forward as it stands (same kernels and launches, so bit-identical to the no_grad call) and
+    keeps: the first convolution's output before GroupNorm + the forward's fp64 statistics, the GroupNorm output, per
+    decoder layer its input [N, 256], the pw1 output [N, 1024] and the GLU-conv-SiLU output [N, 512], the final LayerNorm's
+    input and output (N = B T tokens; about 30 MB per layer at 24 x 172).  backward walks the layers in reverse: the
+    kernels of csrc/unit2control_bwd.cu (no atomics, fixed summation order: bit-identical from run to run) between library
+    GEMMs at the module's gemm_precision (dX = gY W on the packed weights, dW = gY^T X with both activations split in
+    3xtf32 mode).  Everything inside the GLU -> depthwise conv -> SiLU stage is recomputed from the saved pw1 output.
+    Either cotangent may be absent.  Not differentiable twice."""
+
+    @staticmethod
+    def forward(ctx, mod, names, units, f0, phase, volume, spk_id, aug_shift, do_w, *params):
+        save = {}
+        with _Gemm(mod.gemm_precision) as g:
+            e, hidden = mod._forward(g, units, f0, phase, volume, spk_id, None, aug_shift, save=save)
+        ctx.mod, ctx.names, ctx.saved, ctx.spk_id = mod, names, save, spk_id
+        ctx.save_for_backward(units, hidden)
+        ctx.set_materialize_grads(False)
+        return e, hidden
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, ge, gh):
+        mod, S = ctx.mod, ctx.saved
+        units, hidden = ctx.saved_tensors
+        P, (B, T, _) = S["P"], units.shape
+        N, n_out, inner, dev = B * T, mod.n_out, P["layers"][0]["dw_w"].shape[0], units.device
+        L = _lib.lib()
+        ws_bytes = L.b2d_u2c_backward_workspace_bytes(B, T, inner, max(n_out, 2 * inner))
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        new = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)
+        unk3 = lambda dw: dw.reshape(dw.shape[0], 3, -1).permute(0, 2, 1).contiguous()        # [O, 3 I] -> Conv1d's [O, I, 3]
+
+        def colsum(g2d):
+            out = new(g2d.shape[1])
+            _k(L.b2d_u2c_colsum(g2d.data_ptr(), N, g2d.shape[1], out.data_ptr(), ws.data_ptr(), ws_bytes, _stream()), "b2d_u2c_colsum")
+            return out
+
+        G, d_do_w = {}, None
+        with _Gemm(mod.gemm_precision) as g:
+            # dense_out, then the final LayerNorm (whose output is also `hidden`)
+            if ge is not None:
+                ge = ge.contiguous().reshape(N, n_out)
+                ges = g.split(ge)
+                d_do_w = g.grad_weight(ges, g.split(hidden.reshape(N, 256)))
+                G["dense_out.bias"] = colsum(ge)
+                gy = g.grad_input(ges, P["do_w"])
+                if gh is not None:
+                    gy += gh.reshape(N, 256)
+            else:
+                gy = gh.contiguous().reshape(N, 256)
+            gx, dgb = new(N, 256), new(2, 256)
+            _k(L.b2d_u2c_layernorm_backward(S["ln_in"].data_ptr(), gy.data_ptr(), P["n_w"].data_ptr(), 1e-5, N, 256, gx.data_ptr(),
+                                            dgb.data_ptr(), ws.data_ptr(), ws_bytes, _stream()), "b2d_u2c_layernorm_backward")
+            G["norm.weight"], G["norm.bias"] = dgb[0], dgb[1]
+            # decoder layers: x_out = x_in + pw2(glu_dwconv_silu(pw1(x_in)))
+            for i in reversed(range(len(P["layers"]))):
+                (x_in, h, s), Ly, pre = S["layers"][i], P["layers"][i], "decoder.encoder_layers.%d.conformer.net." % i
+                gxs = g.split(gx)
+                G[pre + "6.weight"] = g.grad_weight(gxs, g.split(s.reshape(N, inner))).unsqueeze(-1)
+                G[pre + "6.bias"] = colsum(gx)
+                gs = g.grad_input(gxs, Ly["pw2_w"])
+                ghh, dwb = new(N, 2 * inner), new(inner, 32)
+                _k(L.b2d_u2c_glu_dwconv_silu_backward(h.data_ptr(), Ly["dw_w"].data_ptr(), Ly["dw_b"].data_ptr(), gs.data_ptr(),
+                                                      ghh.data_ptr(), dwb.data_ptr(), B, T, inner, Ly["dw_w"].shape[1], ws.data_ptr(),
+                                                      ws_bytes, _stream()), "b2d_u2c_glu_dwconv_silu_backward")
+                G[pre + "4.weight"], G[pre + "4.bias"] = dwb[:, :31].unsqueeze(1).contiguous(), dwb[:, 31].contiguous()
+                ghs = g.split(ghh)
+                G[pre + "2.weight"] = g.grad_weight(ghs, g.split(x_in.reshape(N, 256))).unsqueeze(-1)
+                G[pre + "2.bias"] = colsum(ghh)
+                gx = g.grad_input(ghs, Ly["pw1_w"], out=gx)                     # + the residual branch
+            # embedding sum: gx passes through to the stack unchanged
+            dtable, rowsum, aug = new(7, 256), new(B, 256), S["aug"]
+            _k(L.b2d_u2c_embed_backward(gx.data_ptr(), S["f0"].data_ptr(), S["phase"].data_ptr(), S["volume"].data_ptr(),
+                                        0 if aug is None else aug.data_ptr(), B, T, dtable.data_ptr(), rowsum.data_ptr(),
+                                        ws.data_ptr(), ws_bytes, _stream()), "b2d_u2c_embed_backward")
+            for row, name in enumerate(("f0_embed", "phase_embed", "volume_embed")):
+                G[name + ".weight"], G[name + ".bias"] = dtable[2 * row].unsqueeze(1), dtable[2 * row + 1]
+            if aug is not None:
+                G["aug_shift_embed.weight"] = dtable[6].unsqueeze(1)
+            if mod.n_spk is not None and mod.n_spk > 1:
+                # utterance b adds its row sum into row spk_id[b] - 1: a one-hot product in fp64 (utterance order, no atomics)
+                ids = (ctx.spk_id.reshape(1, -1) - 1).expand(1, B)
+                onehot = torch.zeros(mod.n_spk, B, dtype=torch.float64, device=dev).scatter_(0, ids, 1.0)
+                G["spk_embed.weight"] = (onehot @ rowsum.double()).float()
+            # convolution stack: the first convolution's input is data (dW, db only)
+            first = "stack."
+            if mod.use_conv_stack:
+                first, gxs = "stack.0.", g.split(gx)
+                G["stack.3.weight"] = unk3(g.grad_weight(gxs, g.split(mod._gather3(S["y1"]).reshape(N, -1))))
+                G["stack.3.bias"] = colsum(gx)
+                gcat, gy1, gx, dgb = g.grad_input(gxs, P["c2_w"]), new(N, 256), new(N, 256), new(2, 256)
+                _k(L.b2d_u2c_conv3_fold(gcat.data_ptr(), B, T, 256, gy1.data_ptr(), _stream()), "b2d_u2c_conv3_fold")
+                _k(L.b2d_u2c_groupnorm_lrelu_backward(S["x1"].data_ptr(), S["stats"].data_ptr(), P["gn_w"].data_ptr(),
+                                                      P["gn_b"].data_ptr(), 1e-5, 0.01, gy1.data_ptr(), B, T, 256, 4, gx.data_ptr(),
+                                                      dgb.data_ptr(), ws.data_ptr(), ws_bytes, _stream()),
+                   "b2d_u2c_groupnorm_lrelu_backward")
+                G["stack.1.weight"], G["stack.1.bias"] = dgb[0], dgb[1]
+            G[first + "weight"] = unk3(g.grad_weight(g.split(gx), g.split(mod._gather3(units).reshape(N, -1))))
+            G[first + "bias"] = colsum(gx)
+        return (None,) * 8 + (d_do_w,) + tuple(G.get(n) for n in ctx.names)
 
 
 class Unit2Control(nn.Module):
@@ -266,10 +399,15 @@ class Unit2Control(nn.Module):
     @staticmethod
     def _conv3(g, x, w, b):
         """Conv1d(k = 3, padding 1) on token-major x [B, T, I] as ONE GEMM over the three shifted inputs."""
+        cat = Unit2Control._gather3(x)
+        return g.linear(cat.reshape(-1, cat.shape[-1]), w, b).reshape(x.shape[0], x.shape[1], -1)
+
+    @staticmethod
+    def _gather3(x):
+        """[B, T, I] -> [B, T, 3 I]: rows (x[t-1], x[t], x[t+1]) with zero padding"""
         xp = torch.nn.functional.pad(x, (0, 0, 1, 1))
         T = x.shape[1]
-        cat = torch.cat((xp[:, 0:T], xp[:, 1:T + 1], xp[:, 2:T + 2]), dim=-1)
-        return g.linear(cat.reshape(-1, cat.shape[-1]), w, b).reshape(x.shape[0], T, -1)
+        return torch.cat((xp[:, 0:T], xp[:, 1:T + 1], xp[:, 2:T + 2]), dim=-1)
 
     @staticmethod
     def _layernorm(x, w, b):
@@ -278,7 +416,7 @@ class Unit2Control(nn.Module):
                                         b.data_ptr(), 1e-5, _stream()), "b2d_u2c_layernorm")
         return y
 
-    def _conv_module(self, g_, x, L, pre_norm):
+    def _conv_module(self, g_, x, L, pre_norm, save=None):
         B, T, C = x.shape
         h = self._layernorm(x, L["cln_w"], L["cln_b"]) if pre_norm else x
         h = g_.linear(h.reshape(-1, C), L["pw1_w"], L["pw1_b"])                              # [B T, 4 C]: value | gate
@@ -286,6 +424,8 @@ class Unit2Control(nn.Module):
         g = torch.empty(B, T, inner, dtype=torch.float32, device=x.device)
         _k(_lib.lib().b2d_u2c_glu_dwconv_silu(h.data_ptr(), L["dw_w"].data_ptr(), L["dw_b"].data_ptr(), g.data_ptr(), B, T, inner,
                                               L["dw_w"].shape[1], _stream()), "b2d_u2c_glu_dwconv_silu")
+        if save is not None:
+            save["layers"].append((x, h, g))
         return g_.linear(g.reshape(-1, inner), L["pw2_w"], L["pw2_b"]).reshape(B, T, C)
 
     def _attention(self, g_, x, L):
@@ -320,13 +460,36 @@ class Unit2Control(nn.Module):
         out = out.permute(0, 2, 1, 3).reshape(B * T, H * d)
         return g_.linear(out, L["out_w"], L["out_b"]).reshape(B, T, C)
 
-    @torch.no_grad()
     def forward(self, units, f0, phase, volume, spk_id=None, spk_mix_dict=None, aug_shift=None):
-        """units B x n_frames x n_unit; f0, phase, volume B x n_frames x 1 -> (dict of B x n_frames x feat, hidden)"""
-        with _Gemm(self.gemm_precision) as g:
-            return self._forward(g, units, f0, phase, volume, spk_id, spk_mix_dict, aug_shift)
+        """units B x n_frames x n_unit; f0, phase, volume B x n_frames x 1 -> (dict of B x n_frames x feat, hidden).
+        Convolution-only decoder, grad mode on and a parameter that requires grad: both outputs carry the CUDA backward
+        towards every parameter (module docstring); otherwise the outputs are detached."""
+        if self.use_naive_v2 and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            for name, t in (("units", units), ("f0", f0), ("phase", phase), ("volume", volume), ("aug_shift", aug_shift)):
+                if torch.is_tensor(t) and t.requires_grad:
+                    raise NotImplementedError("Unit2Control: no gradient with respect to %s (the inputs are data)" % name)
+            if spk_mix_dict is not None:
+                raise NotImplementedError("Unit2Control: spk_mix_dict is an inference feature; train with spk_id")
+            names, params = self._grad_params()
+            # weight norm is parameter-side (once per step, not per token): autograd turns dW into d weight_g, d weight_v
+            do_w = torch._weight_norm(self.dense_out.weight_v, self.dense_out.weight_g, 0)
+            e, hidden = _NaiveFunction.apply(self, names, units, f0, phase, volume, spk_id, aug_shift, do_w, *params)
+            return split_to_dict(e, self.output_splits), hidden
+        with torch.no_grad(), _Gemm(self.gemm_precision) as g:
+            e, hidden = self._forward(g, units, f0, phase, volume, spk_id, spk_mix_dict, aug_shift)
+            return split_to_dict(e, self.output_splits), hidden
 
-    def _forward(self, g, units, f0, phase, volume, spk_id=None, spk_mix_dict=None, aug_shift=None):
+    def _grad_params(self):
+        """(names, tensors) of the parameters the backward of the convolution-only decoder produces gradients for, in the
+        order _NaiveFunction returns them: all but dense_out.weight_g / weight_v (reached through the weight-norm product)
+        and the decoder layers' LayerNorms (in the state dict, unused when conv_only)"""
+        skip = ("dense_out.weight_g", "dense_out.weight_v")
+        items = [(n, p) for n, p in self.named_parameters()
+                 if n not in skip and not (n.startswith("decoder.encoder_layers.") and ".norm." in n)]
+        return tuple(n for n, _ in items), tuple(p for _, p in items)
+
+    def _forward(self, g, units, f0, phase, volume, spk_id=None, spk_mix_dict=None, aug_shift=None, save=None):
+        """-> (dense [B, T, n_out], hidden [B, T, 256]); ``save``: a dict that receives what the backward needs"""
         _need_cuda_f32("units", units)
         B, T, _ = units.shape
         P = self._pack()
@@ -334,10 +497,16 @@ class Unit2Control(nn.Module):
         x = self._conv3(g, units, P["c1_w"], P["c1_b"])
         if self.use_conv_stack:
             stats = torch.empty(B * 4 * 2, dtype=torch.float64, device=x.device)
+            if save is not None:
+                save["x1"], save["stats"] = x.clone(), stats       # the GroupNorm kernel works in place
             _k(L.b2d_u2c_groupnorm_lrelu(x.data_ptr(), B, T, 256, 4, P["gn_w"].data_ptr(), P["gn_b"].data_ptr(), 1e-5, 0.01,
                                          stats.data_ptr(), _stream()), "b2d_u2c_groupnorm_lrelu")
+            if save is not None:
+                save["y1"] = x
             x = self._conv3(g, x, P["c2_w"], P["c2_b"])
         spk, spk_rows = None, 1
+        if save is not None:
+            save["layers"] = []
         if self.n_spk is not None and self.n_spk > 1:
             if spk_mix_dict is not None:
                 spk = sum(float(v) * self.spk_embed.weight[int(k) - 1] for k, v in spk_mix_dict.items()).reshape(1, 256).contiguous()
@@ -357,7 +526,9 @@ class Unit2Control(nn.Module):
         for Ly in P["layers"]:
             if not self.use_naive_v2:
                 x = x + self._attention(g, x, Ly)
-            x = x + self._conv_module(g, x, Ly, pre_norm=not self.use_naive_v2)
+            x = x + self._conv_module(g, x, Ly, pre_norm=not self.use_naive_v2, save=save)
+        if save is not None:
+            save.update(P=P, f0=f0c, phase=phc, volume=voc, aug=aug, ln_in=x)
         x = self._layernorm(x, P["n_w"], P["n_b"])
         e = g.linear(x.reshape(-1, 256), P["do_w"], P["do_b"]).reshape(B, T, self.n_out)
-        return split_to_dict(e, self.output_splits), x
+        return e, x

@@ -355,6 +355,37 @@ int b2d_u2c_softmax_features(float* projected, const float* data, int rows, int 
 int b2d_u2c_linear_attention(const float* q_features, const float* k_features, const float* v, float* out, int B, int H,
                              int T, int n_features, int dim_head, float eps, void* stream);
 
+/* ---- backward of the control network with the convolution-only decoder (unit2control_bwd.cu): the adjoints of the
+ * kernels above that the naive decoder runs; the GEMM adjoints are library GEMMs of the caller.  No atomics: sums over
+ * tokens are taken per fixed slab of tokens into the workspace, then added in slab order in fp64, so every result is
+ * bit-identical from run to run and independent of the device.  `ws` is scratch of at least
+ * b2d_u2c_backward_workspace_bytes(B, T, inner_channels, max_cols) bytes (enough for each call below with n_tokens = B T,
+ * that inner_channels, and n_cols <= max_cols; 0 = bad shape); too small a workspace returns B2D_ERR_WORKSPACE.
+ * u2c_glu_dwconv_silu_backward: h [B, T, 2 Ci] is the forward's INPUT (the stage is recomputed from it), gout [B, T, Ci]
+ *   the cotangent of its output -> gh [B, T, 2 Ci] and dwb [Ci, 32]: 31 tap gradients, then the bias gradient.
+ * u2c_colsum: out [n_cols] = column sums of g [n_tokens, n_cols] (the bias gradient of a GEMM).
+ * u2c_layernorm_backward (C = 256): x the forward's input, gy the cotangent of its output -> gx, and dgamma_dbeta [2, C].
+ * u2c_groupnorm_lrelu_backward (C = 256): x_pre [B, T, C] the activation BEFORE the in-place forward, stats the
+ *   B * groups * 2 doubles the forward left in stats_ws, gy the cotangent of the LeakyReLU output -> gx, dgamma_dbeta [2, C].
+ * u2c_embed_backward: gx [B*T, 256] the cotangent of u2c_embed's output (which is also the cotangent of its input x) ->
+ *   dtable [7, 256], the gradient of embed_table, and rowsum [B, 256] = per-utterance sums of gx (the gradient of each
+ *   utterance's speaker row); aug_shift [B] or NULL as in the forward.
+ * u2c_conv3_fold: adjoint of gathering (x[t-1], x[t], x[t+1]) (zero padded) into rows of 3 * channels:
+ *   gx[t] = gcat[t+1][0:I] + gcat[t][I:2I] + gcat[t-1][2I:3I]. */
+size_t b2d_u2c_backward_workspace_bytes(int B, int T, int inner_channels, int max_cols);
+int b2d_u2c_glu_dwconv_silu_backward(const float* h, const float* weight, const float* bias, const float* gout, float* gh,
+                                     float* dwb, int B, int T, int inner_channels, int kernel_size, void* ws, size_t ws_bytes,
+                                     void* stream);
+int b2d_u2c_colsum(const float* g, int n_tokens, int n_cols, float* out, void* ws, size_t ws_bytes, void* stream);
+int b2d_u2c_layernorm_backward(const float* x, const float* gy, const float* gamma, float eps, int n_tokens, int C, float* gx,
+                               float* dgamma_dbeta, void* ws, size_t ws_bytes, void* stream);
+int b2d_u2c_groupnorm_lrelu_backward(const float* x_pre, const double* stats, const float* gamma, const float* beta, float eps,
+                                     float slope, const float* gy, int B, int T, int C, int groups, float* gx,
+                                     float* dgamma_dbeta, void* ws, size_t ws_bytes, void* stream);
+int b2d_u2c_embed_backward(const float* gx, const float* f0, const float* phase, const float* volume, const float* aug_shift,
+                           int B, int T, float* dtable, float* rowsum, void* ws, size_t ws_bytes, void* stream);
+int b2d_u2c_conv3_fold(const float* gcat, int B, int T, int channels, float* gx, void* stream);
+
 /* ---- log-mel front end of the NSF-HiFiGAN vocoder: STFT.get_mel, nsf_hifigan/nvSTFT.py:73-117 (keyshift 0, speed 1) ----
  * audio [B, n_samples] -> mel [B, n_mels, n_frames], n_frames = b2d_mel_frames(...) (0 = signal too short):
  * reflect / constant padding by (win - hop)/2, frames of win_size = n_fft = 2048 at `hop`, periodic Hann `window` [2048],
