@@ -89,6 +89,13 @@ SIGNATURES = {
     "b2d_u2c_embed_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, c_f32p,
                                               c_f32p, ctypes.c_void_p, ctypes.c_size_t, c_stream]),
     "b2d_u2c_conv3_fold": (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p, c_stream]),
+    "b2d_u2c_attn_readout_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                                     ctypes.c_int, c_f32p, c_stream]),
+    "b2d_u2c_softmax_features_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int,
+                                                         ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, c_f32p,
+                                                         c_stream]),
+    "b2d_u2c_qkv_gather_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                                   ctypes.c_int, ctypes.c_int, c_f32p, c_stream]),
     "b2d_mel_frames": (ctypes.c_int, [ctypes.c_int] * 4),
     "b2d_mel_spectrogram": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                            ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, c_f32p, c_stream]),

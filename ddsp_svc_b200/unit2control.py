@@ -13,12 +13,14 @@ torch.addmm / bmm, fp32); everything between them runs in the fused kernels of c
 GroupNorm + LeakyReLU, LayerNorm, GLU + depthwise k = 31 convolution + SiLU, performer feature maps).  CPU tensors raise.
 
 Training: with the convolution-only decoder (``use_naive_v2=True``: what CombSubSuperFast builds, so configs/combsub.yaml,
-reflow.yaml and diffusion-fast.yaml) the module is differentiable with respect to all of its parameters when grad mode is
-on and a parameter requires grad: ONE autograd Function (_NaiveFunction) around the whole network whose forward is the
-inference forward (same kernels, bit-identical outputs; that decoder has no dropout) plus the saved activations, and whose
-backward walks the layers in reverse on the kernels of csrc/unit2control_bwd.cu and library GEMMs.  The inputs are data:
-units, f0, phase, volume or aug_shift that require grad, and spk_mix_dict under grad, raise NotImplementedError.  The PCmer
-decoder stays inference only (outputs detached in every mode); train it with a differentiable ``unit2ctrl=``.
+reflow.yaml and diffusion-fast.yaml), and with the PCmer decoder when ``pcmer_backward`` is set (what Sins, CombSub and
+CombSubFast build: configs/sins.yaml, combsub-old, diffusion-new.yaml), the module is differentiable with respect to all
+of its parameters when grad mode is on and a parameter requires grad: ONE autograd Function (_Unit2ControlFunction)
+around the whole network whose forward is the inference forward (same kernels, bit-identical outputs; neither decoder has
+an active dropout) plus the saved activations, and whose backward walks the layers in reverse on the kernels of
+csrc/unit2control_bwd.cu and csrc/pcmer_bwd.cu and library GEMMs.  The inputs are data: units, f0, phase, volume or
+aug_shift that require grad, and spk_mix_dict under grad, raise NotImplementedError.  With ``pcmer_backward`` off (the
+default) the PCmer decoder's outputs are detached in every mode.
 """
 import math
 
@@ -205,18 +207,23 @@ class _Gemm:
             torch.backends.cuda.matmul.allow_tf32 = True
 
 
-class _NaiveFunction(torch.autograd.Function):
-    """The whole control network with the convolution-only decoder as ONE differentiable op:
+class _Unit2ControlFunction(torch.autograd.Function):
+    """The whole control network (either decoder) as ONE differentiable op:
     (module, parameter names, inputs..., dense_out weight, *parameters) -> (dense [B, T, n_out], hidden [B, T, 256]).
 
     forward is Unit2Control._forward as it stands (same kernels and launches, so bit-identical to the no_grad call) and
     keeps: the first convolution's output before GroupNorm + the forward's fp64 statistics, the GroupNorm output, per
-    decoder layer its input [N, 256], the pw1 output [N, 1024] and the GLU-conv-SiLU output [N, 512], the final LayerNorm's
-    input and output (N = B T tokens; about 30 MB per layer at 24 x 172).  backward walks the layers in reverse: the
-    kernels of csrc/unit2control_bwd.cu (no atomics, fixed summation order: bit-identical from run to run) between library
-    GEMMs at the module's gemm_precision (dX = gY W on the packed weights, dW = gY^T X with both activations split in
-    3xtf32 mode).  Everything inside the GLU -> depthwise conv -> SiLU stage is recomputed from the saved pw1 output.
-    Either cotangent may be absent.  Not differentiable twice."""
+    decoder layer the convolution module's input and (PCmer) its LayerNorm output [N, 256], the pw1 output [N, 1024] and
+    the GLU-conv-SiLU output [N, 512], the final LayerNorm's input and output (N = B T tokens; about 30 MB per layer at
+    24 x 172).  A PCmer layer also keeps its attention's input and LayerNorm output, the qkv projection [N, 1536], the
+    feature maps' inputs q, k and v [B, H, T, 64], the features phi_q, phi_k [B, H, T, 266] and the read-out [N, 512]
+    (about 170 MB per layer at 24 x 172).  backward walks the layers in reverse: the kernels of csrc/unit2control_bwd.cu
+    and csrc/pcmer_bwd.cu (no atomics, fixed summation order: bit-identical from run to run) between library GEMMs at the
+    module's gemm_precision (dX = gY W on the packed weights, dW = gY^T X with both activations split in 3xtf32 mode; the
+    per-head products through _Gemm.matmul, as in the forward).  Everything inside the GLU -> depthwise conv -> SiLU
+    stage is recomputed from the saved pw1 output, and the attention's k-sum, context and normaliser from the saved
+    features and v, so one backward serves both fused_attention settings.  Either cotangent may be absent.  Not
+    differentiable twice."""
 
     @staticmethod
     def forward(ctx, mod, names, units, f0, phase, volume, spk_id, aug_shift, do_w, *params):
@@ -236,7 +243,8 @@ class _NaiveFunction(torch.autograd.Function):
         P, (B, T, _) = S["P"], units.shape
         N, n_out, inner, dev = B * T, mod.n_out, P["layers"][0]["dw_w"].shape[0], units.device
         L = _lib.lib()
-        ws_bytes = L.b2d_u2c_backward_workspace_bytes(B, T, inner, max(n_out, 2 * inner))
+        max_cols = max([n_out, 2 * inner] + [Ly["qkv_b"].shape[0] for Ly in P["layers"] if "qkv_b" in Ly])
+        ws_bytes = L.b2d_u2c_backward_workspace_bytes(B, T, inner, max_cols)
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
         new = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)
         unk3 = lambda dw: dw.reshape(dw.shape[0], 3, -1).permute(0, 2, 1).contiguous()        # [O, 3 I] -> Conv1d's [O, I, 3]
@@ -259,13 +267,61 @@ class _NaiveFunction(torch.autograd.Function):
                     gy += gh.reshape(N, 256)
             else:
                 gy = gh.contiguous().reshape(N, 256)
-            gx, dgb = new(N, 256), new(2, 256)
-            _k(L.b2d_u2c_layernorm_backward(S["ln_in"].data_ptr(), gy.data_ptr(), P["n_w"].data_ptr(), 1e-5, N, 256, gx.data_ptr(),
-                                            dgb.data_ptr(), ws.data_ptr(), ws_bytes, _stream()), "b2d_u2c_layernorm_backward")
-            G["norm.weight"], G["norm.bias"] = dgb[0], dgb[1]
-            # decoder layers: x_out = x_in + pw2(glu_dwconv_silu(pw1(x_in)))
+
+            def layernorm_backward(x, gy, w, name):
+                """-> the cotangent of x through LayerNorm(x); gamma / beta gradients into G[name + ".weight" / ".bias"]"""
+                gx, dgb = new(N, 256), new(2, 256)
+                _k(L.b2d_u2c_layernorm_backward(x.data_ptr(), gy.data_ptr(), w.data_ptr(), 1e-5, N, 256, gx.data_ptr(), dgb.data_ptr(),
+                                                ws.data_ptr(), ws_bytes, _stream()), "b2d_u2c_layernorm_backward")
+                G[name + ".weight"], G[name + ".bias"] = dgb[0], dgb[1]
+                return gx
+
+            def attention_backward(gy, Ly, A, name):
+                """performer self-attention y = to_out(read-out(phi_q, phi_k, v)) on a = LN_a(x) with q, k, v = qkv(a):
+                gy [N, 256] the cotangent of y -> that of a; parameter gradients into G[name + ...]"""
+                qf, kf, v = A["qf"], A["kf"], A["v"]                                          # [B, H, T, J], [B, H, T, 64]
+                H, J, d = qf.shape[1], qf.shape[3], v.shape[3]
+                R = B * H * T
+                gys = g.split(gy)
+                G[name + "to_out.weight"] = g.grad_weight(gys, g.split(A["out"].reshape(N, H * d)))
+                G[name + "to_out.bias"] = colsum(gy)
+                g_out = g.grad_input(gys, Ly["out_w"])                                        # [N, H d] token-major
+                # k-sum, normaliser and context recomputed with the forward's own expressions
+                k_sum = kf.sum(dim=-2)
+                d_inv = 1.0 / (torch.einsum("bhnj,bhj->bhn", qf, k_sum) + 1e-8)
+                context = g.matmul(kf.transpose(-1, -2), v)                                   # [B, H, J, d]
+                gn = new(B, H, T, d + 1)                                                      # [g_num | g_D]
+                _k(L.b2d_u2c_attn_readout_backward(g_out.data_ptr(), A["out"].data_ptr(), d_inv.data_ptr(), B, H, T, d, gn.data_ptr(),
+                                                   _stream()), "b2d_u2c_attn_readout_backward")
+                gc = g.matmul(qf.transpose(-1, -2), gn)                                       # [B, H, J, d + 1]: [g_ctx | g_ksum]
+                g_ctx = gc[..., :d]
+                g_qf = g.matmul(gn[..., :d], context.transpose(-1, -2))                       # [B, H, T, J]
+                g_kf = g.matmul(v, g_ctx.transpose(-1, -2))
+                g_v = g.matmul(kf, g_ctx)                                                     # [B, H, T, d]
+                proj = Ly["proj"] if g.mode == "3xtf32" else Ly["proj_t"].t()
+                g_data = []
+                for gf, feat, data, vec, scal, is_q in ((g_qf, qf, A["q"], k_sum, gn[..., d].contiguous(), 1),
+                                                        (g_kf, kf, A["k"], gc[..., d].contiguous(), None, 0)):
+                    gd = new(R, d)
+                    _k(L.b2d_u2c_softmax_features_backward(gf.data_ptr(), feat.data_ptr(), data.data_ptr(), vec.data_ptr(),
+                                                           0 if scal is None else scal.data_ptr(), R, T, J, d, is_q, 1e-4,
+                                                           gd.data_ptr(), _stream()), "b2d_u2c_softmax_features_backward")
+                    g_data.append(g.grad_input(g.split(gf.reshape(R, J)), proj, out=gd))
+                g_qkv = new(N, 3 * H * d)
+                _k(L.b2d_u2c_qkv_gather_backward(g_data[0].data_ptr(), g_data[1].data_ptr(), g_v.data_ptr(), A["qkv"].data_ptr(), B, H,
+                                                 T, d, int(mod.pcmer_norm), g_qkv.data_ptr(), _stream()), "b2d_u2c_qkv_gather_backward")
+                gqs = g.split(g_qkv)
+                dw, db = g.grad_weight(gqs, g.split(A["a"].reshape(N, 256))), colsum(g_qkv)
+                for j, part in enumerate(("to_q.", "to_k.", "to_v.")):
+                    G[name + part + "weight"], G[name + part + "bias"] = dw[j * H * d:(j + 1) * H * d], db[j * H * d:(j + 1) * H * d]
+                return g.grad_input(gqs, Ly["qkv_w"])
+
+            gx = layernorm_backward(S["ln_in"], gy, P["n_w"], "norm")
+            # decoder layers: x1 = x + attention(LN_a(x)) (PCmer only), x2 = x1 + pw2(glu_dwconv_silu(pw1(LN_c(x1))))
+            naive = mod.use_naive_v2
             for i in reversed(range(len(P["layers"]))):
-                (x_in, h, s), Ly, pre = S["layers"][i], P["layers"][i], "decoder.encoder_layers.%d.conformer.net." % i
+                lpre = ("decoder.encoder_layers.%d." if naive else "decoder._layers.%d.") % i
+                (x_in, hn, h, s), Ly, pre = S["layers"][i], P["layers"][i], lpre + "conformer.net."
                 gxs = g.split(gx)
                 G[pre + "6.weight"] = g.grad_weight(gxs, g.split(s.reshape(N, inner))).unsqueeze(-1)
                 G[pre + "6.bias"] = colsum(gx)
@@ -274,11 +330,17 @@ class _NaiveFunction(torch.autograd.Function):
                 _k(L.b2d_u2c_glu_dwconv_silu_backward(h.data_ptr(), Ly["dw_w"].data_ptr(), Ly["dw_b"].data_ptr(), gs.data_ptr(),
                                                       ghh.data_ptr(), dwb.data_ptr(), B, T, inner, Ly["dw_w"].shape[1], ws.data_ptr(),
                                                       ws_bytes, _stream()), "b2d_u2c_glu_dwconv_silu_backward")
-                G[pre + "4.weight"], G[pre + "4.bias"] = dwb[:, :31].unsqueeze(1).contiguous(), dwb[:, 31].contiguous()
+                dw = pre + ("4." if naive else "4.conv.")
+                G[dw + "weight"], G[dw + "bias"] = dwb[:, :31].unsqueeze(1).contiguous(), dwb[:, 31].contiguous()
                 ghs = g.split(ghh)
-                G[pre + "2.weight"] = g.grad_weight(ghs, g.split(x_in.reshape(N, 256))).unsqueeze(-1)
+                G[pre + "2.weight"] = g.grad_weight(ghs, g.split(hn.reshape(N, 256))).unsqueeze(-1)
                 G[pre + "2.bias"] = colsum(ghh)
-                gx = g.grad_input(ghs, Ly["pw1_w"], out=gx)                     # + the residual branch
+                if naive:
+                    gx = g.grad_input(ghs, Ly["pw1_w"], out=gx)                 # + the residual branch
+                    continue
+                gx = gx + layernorm_backward(x_in, g.grad_input(ghs, Ly["pw1_w"]), Ly["cln_w"], pre + "0")
+                A = S["attn"][i]
+                gx = gx + layernorm_backward(A["x"], attention_backward(gx, Ly, A, lpre + "attn."), Ly["ln_w"], lpre + "norm")
             # embedding sum: gx passes through to the stack unchanged
             dtable, rowsum, aug = new(7, 256), new(B, 256), S["aug"]
             _k(L.b2d_u2c_embed_backward(gx.data_ptr(), S["f0"].data_ptr(), S["phase"].data_ptr(), S["volume"].data_ptr(),
@@ -319,6 +381,11 @@ class Unit2Control(nn.Module):
     #: (same 1.4e-6 on the controls); 256 CTAs of 9 warps, two per SM, single-buffered tiles -- it needs a split over frames
     #: and double buffering to compete with the batched SIMT GEMMs.
     fused_attention = False
+    #: PCmer: with grad mode on and a parameter that requires grad, make both outputs differentiable with respect to every
+    #: parameter (the backward of _Unit2ControlFunction; the forward issues the same kernels with the same results).  Off by
+    #: default: the PCmer decoder's outputs have always been detached and a test pins that; turning the default on is a
+    #: separate decision.  Set it on the class (``Unit2Control.pcmer_backward = True``) or per instance.
+    pcmer_backward = False
 
     def __init__(self, input_channel, n_spk, output_splits, use_pitch_aug=False, pcmer_norm=False, use_naive_v2=False,
                  use_conv_stack=True):
@@ -418,18 +485,19 @@ class Unit2Control(nn.Module):
 
     def _conv_module(self, g_, x, L, pre_norm, save=None):
         B, T, C = x.shape
-        h = self._layernorm(x, L["cln_w"], L["cln_b"]) if pre_norm else x
-        h = g_.linear(h.reshape(-1, C), L["pw1_w"], L["pw1_b"])                              # [B T, 4 C]: value | gate
+        hn = self._layernorm(x, L["cln_w"], L["cln_b"]) if pre_norm else x
+        h = g_.linear(hn.reshape(-1, C), L["pw1_w"], L["pw1_b"])                             # [B T, 4 C]: value | gate
         inner = L["dw_w"].shape[0]
         g = torch.empty(B, T, inner, dtype=torch.float32, device=x.device)
         _k(_lib.lib().b2d_u2c_glu_dwconv_silu(h.data_ptr(), L["dw_w"].data_ptr(), L["dw_b"].data_ptr(), g.data_ptr(), B, T, inner,
                                               L["dw_w"].shape[1], _stream()), "b2d_u2c_glu_dwconv_silu")
         if save is not None:
-            save["layers"].append((x, h, g))
+            save["layers"].append((x, hn, h, g))
         return g_.linear(g.reshape(-1, inner), L["pw2_w"], L["pw2_b"]).reshape(B, T, C)
 
-    def _attention(self, g_, x, L):
-        """performer self-attention of one PCmer layer on LayerNorm(x) (pcmer.py:148, :220-229, :283-309, :343-381)"""
+    def _attention(self, g_, x, L, save=None):
+        """performer self-attention of one PCmer layer on LayerNorm(x) (pcmer.py:148, :220-229, :283-309, :343-381);
+        ``save``: a dict whose "attn" list receives what the backward needs"""
         B, T, C = x.shape
         a = self.decoder._layers[0].attn
         H, d = a.heads, a.dim_head
@@ -452,19 +520,23 @@ class Unit2Control(nn.Module):
             out = torch.empty(B, T, H, d, dtype=torch.float32, device=x.device)
             _k(_lib.lib().b2d_u2c_linear_attention(qf.data_ptr(), kf.data_ptr(), v.data_ptr(), out.data_ptr(), B, H, T, J, d, 1e-8,
                                                    _stream()), "b2d_u2c_linear_attention")
-            return g_.linear(out.reshape(B * T, H * d), L["out_w"], L["out_b"]).reshape(B, T, C)
-        k_sum = kf.sum(dim=-2)                                                               # [B, H, J]
-        d_inv = 1.0 / (torch.einsum("bhnj,bhj->bhn", qf, k_sum) + 1e-8)
-        context = g_.matmul(kf.transpose(-1, -2), v)                                         # [B, H, J, d]
-        out = g_.matmul(qf, context) * d_inv.unsqueeze(-1)                                   # [B, H, T, d]
-        out = out.permute(0, 2, 1, 3).reshape(B * T, H * d)
+        else:
+            k_sum = kf.sum(dim=-2)                                                           # [B, H, J]
+            d_inv = 1.0 / (torch.einsum("bhnj,bhj->bhn", qf, k_sum) + 1e-8)
+            context = g_.matmul(kf.transpose(-1, -2), v)                                     # [B, H, J, d]
+            out = g_.matmul(qf, context) * d_inv.unsqueeze(-1)                               # [B, H, T, d]
+            out = out.permute(0, 2, 1, 3)
+        out = out.reshape(B * T, H * d)
+        if save is not None:                 # the feature kernel worked in place: qf, kf are the features, q, k their inputs
+            save["attn"].append(dict(x=x, a=h, qkv=qkv, q=q, k=k, v=v, qf=qf, kf=kf, out=out))
         return g_.linear(out, L["out_w"], L["out_b"]).reshape(B, T, C)
 
     def forward(self, units, f0, phase, volume, spk_id=None, spk_mix_dict=None, aug_shift=None):
         """units B x n_frames x n_unit; f0, phase, volume B x n_frames x 1 -> (dict of B x n_frames x feat, hidden).
-        Convolution-only decoder, grad mode on and a parameter that requires grad: both outputs carry the CUDA backward
-        towards every parameter (module docstring); otherwise the outputs are detached."""
-        if self.use_naive_v2 and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+        Convolution-only decoder, or PCmer decoder with ``pcmer_backward``, grad mode on and a parameter that requires
+        grad: both outputs carry the CUDA backward towards every parameter (module docstring); otherwise the outputs are
+        detached."""
+        if (self.use_naive_v2 or self.pcmer_backward) and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             for name, t in (("units", units), ("f0", f0), ("phase", phase), ("volume", volume), ("aug_shift", aug_shift)):
                 if torch.is_tensor(t) and t.requires_grad:
                     raise NotImplementedError("Unit2Control: no gradient with respect to %s (the inputs are data)" % name)
@@ -473,16 +545,17 @@ class Unit2Control(nn.Module):
             names, params = self._grad_params()
             # weight norm is parameter-side (once per step, not per token): autograd turns dW into d weight_g, d weight_v
             do_w = torch._weight_norm(self.dense_out.weight_v, self.dense_out.weight_g, 0)
-            e, hidden = _NaiveFunction.apply(self, names, units, f0, phase, volume, spk_id, aug_shift, do_w, *params)
+            e, hidden = _Unit2ControlFunction.apply(self, names, units, f0, phase, volume, spk_id, aug_shift, do_w, *params)
             return split_to_dict(e, self.output_splits), hidden
         with torch.no_grad(), _Gemm(self.gemm_precision) as g:
             e, hidden = self._forward(g, units, f0, phase, volume, spk_id, spk_mix_dict, aug_shift)
             return split_to_dict(e, self.output_splits), hidden
 
     def _grad_params(self):
-        """(names, tensors) of the parameters the backward of the convolution-only decoder produces gradients for, in the
-        order _NaiveFunction returns them: all but dense_out.weight_g / weight_v (reached through the weight-norm product)
-        and the decoder layers' LayerNorms (in the state dict, unused when conv_only)"""
+        """(names, tensors) of the parameters the backward produces gradients for, in the order _Unit2ControlFunction
+        returns them: all but dense_out.weight_g / weight_v (reached through the weight-norm product) and the
+        convolution-only decoder's layer LayerNorms (in the state dict, unused when conv_only); the PCmer layers' norms are
+        used and included.  The performer's projection matrix is a buffer."""
         skip = ("dense_out.weight_g", "dense_out.weight_v")
         items = [(n, p) for n, p in self.named_parameters()
                  if n not in skip and not (n.startswith("decoder.encoder_layers.") and ".norm." in n)]
@@ -506,7 +579,7 @@ class Unit2Control(nn.Module):
             x = self._conv3(g, x, P["c2_w"], P["c2_b"])
         spk, spk_rows = None, 1
         if save is not None:
-            save["layers"] = []
+            save["layers"], save["attn"] = [], []
         if self.n_spk is not None and self.n_spk > 1:
             if spk_mix_dict is not None:
                 spk = sum(float(v) * self.spk_embed.weight[int(k) - 1] for k, v in spk_mix_dict.items()).reshape(1, 256).contiguous()
@@ -525,7 +598,7 @@ class Unit2Control(nn.Module):
            "b2d_u2c_embed")
         for Ly in P["layers"]:
             if not self.use_naive_v2:
-                x = x + self._attention(g, x, Ly)
+                x = x + self._attention(g, x, Ly, save=save)
             x = x + self._conv_module(g, x, Ly, pre_norm=not self.use_naive_v2, save=save)
         if save is not None:
             save.update(P=P, f0=f0c, phase=phc, volume=voc, aug=aug, ln_in=x)

@@ -23,7 +23,8 @@ from . import ops
 def _reference_unit2ctrl(n_unit, n_spk, split_map, **kw):
     """The control network: this package's own Unit2Control (same parameter tree as the reference's
     ddsp/unit2control.py, so its checkpoints load strictly; fused kernels + library GEMMs; trainable with the convolution-only decoder that
-    CombSubSuperFast selects, inference only with the PCmer decoder)."""
+    CombSubSuperFast selects, and with the PCmer decoder of Sins, CombSub and CombSubFast when
+    ``Unit2Control.pcmer_backward`` is set -- off by default, outputs detached)."""
     from .unit2control import Unit2Control
     return Unit2Control(n_unit, n_spk, split_map, **kw)
 

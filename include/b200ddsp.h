@@ -386,6 +386,26 @@ int b2d_u2c_embed_backward(const float* gx, const float* f0, const float* phase,
                            int B, int T, float* dtable, float* rowsum, void* ws, size_t ws_bytes, void* stream);
 int b2d_u2c_conv3_fold(const float* gcat, int B, int T, int channels, float* gx, void* stream);
 
+/* ---- backward of the PCmer decoder's performer attention (pcmer_bwd.cu): the stages between the caller's library GEMMs.
+ * Rows are (b, h, t) of B * H * T; dim_head must be 64.  No atomics and no workspace: one warp per row, so every result is
+ * bit-identical from run to run.
+ * u2c_attn_readout_backward: out = (phi_q ctx) d_inv with d_inv [B, H, T] = 1 / (phi_q . ksum + 1e-8); g_out and out
+ *   [B, T, H, 64] token-major -> gn [B, H, T, 65]: g_out d_inv, then g_D = -(g_out . out) d_inv.
+ * u2c_softmax_features_backward: adjoint of u2c_softmax_features.  g [rows, n_features] (n_features <= 288) holds the
+ *   cotangent of the features on entry and that of `projected` on return; features the forward's output, data its input
+ *   [rows, 64]; the full cotangent is g + scal[row] vec[row / T] (queries: scal = g_D, vec = ksum [rows / T, n_features])
+ *   or g + vec[row / T] (keys: vec = g_ksum, scal ignored).  The query's maximum takes its term at the first maximum of
+ *   the features row.  gx [rows, 64] receives the diag term of the cotangent of data (the caller adds g proj).
+ * u2c_qkv_gather_backward: g_q, g_k, g_v [B, H, T, 64] -> g_qkv [B, T, 3, H, 64]; normalized = 1 (pcmer_norm): g_q, g_k
+ *   are cotangents of x / (|x| + 1e-8) with x read from qkv [B, T, 3, H, 64] (the forward's projection). */
+int b2d_u2c_attn_readout_backward(const float* g_out, const float* out, const float* d_inv, int B, int H, int T, int dim_head,
+                                  float* gn, void* stream);
+int b2d_u2c_softmax_features_backward(float* g, const float* features, const float* data, const float* vec, const float* scal,
+                                      int rows, int T, int n_features, int dim_head, int is_query, float eps, float* gx,
+                                      void* stream);
+int b2d_u2c_qkv_gather_backward(const float* g_q, const float* g_k, const float* g_v, const float* qkv, int B, int H, int T,
+                                int dim_head, int normalized, float* g_qkv, void* stream);
+
 /* ---- log-mel front end of the NSF-HiFiGAN vocoder: STFT.get_mel, nsf_hifigan/nvSTFT.py:73-117 (keyshift 0, speed 1) ----
  * audio [B, n_samples] -> mel [B, n_mels, n_frames], n_frames = b2d_mel_frames(...) (0 = signal too short):
  * reflect / constant padding by (win - hop)/2, frames of win_size = n_fft = 2048 at `hop`, periodic Hann `window` [2048],
