@@ -17,6 +17,7 @@ from ddsp_svc_b200 import synthetic as syn
 from oracle import closed_form as cf
 from tests import util
 from tests.golden import cases as G
+from tests import regimes as R
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SR, P = G.SR, G.P
@@ -110,3 +111,21 @@ def test_output_is_bit_identical_for_any_chunking(emu):
     odd = emu(comb[:, :23 * P], dense[:, :23], noise[:, :23 * P], G_hops=32)       # odd frame count
     for hops in (2, 8):
         assert np.array_equal(emu(comb[:, :23 * P], dense[:, :23], noise[:, :23 * P], G_hops=hops), odd), hops
+
+
+@pytest.mark.parametrize("case", R.TABLE, ids=R.CASE_IDS)
+def test_kernel_source_at_input_regimes(emu, case):
+    """The filter kernel source at the pitch and control regimes of tests/regimes.py (fed the reference's fp32 comb),
+    to the criterion of tests/test_gpu_regimes_forward.py: within max(floor, 2 x the fp32 reference's own error) of
+    float64, per row.
+    The emulator evaluates __sinf, __sincosf, __expf and __fdividef with exact libm calls (tests/emu/host_emu.h), so
+    this checks indexing, chunking and the host-visible arithmetic at these inputs; it says nothing about the SFU
+    intrinsics' range reduction or large-argument error, which only tests/test_gpu_regimes_*.py see."""
+    inp = R.build("combsubfast", *case)
+    truth = R.truth_forward(inp)["signal"]
+    with torch.no_grad():
+        ref = R.port_forward(inp)["signal"].numpy()
+    got = emu(_comb_fp32({"f0": inp["f0"]}), inp["dense"].numpy(), inp["noise"].numpy())
+    assert np.isfinite(got).all()
+    bad = R.within_budget(R.forward_errors(got, ref, truth), 2.0, 3.0)
+    assert not bad, (case, bad)

@@ -12,6 +12,7 @@ import torch
 
 from oracle import closed_form as cf
 from tests import util
+from tests import regimes as R
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 P = 512
@@ -249,3 +250,28 @@ def test_spectrum_path_is_bit_identical_for_any_chunking_and_shard(emu_spec):
         assert np.array_equal(a[k], b[k]), k
     part = emu_spec(x1[1:], ir1[1:], None, ir2[1:], hops=4, seed=5, utt_off=1)
     assert np.array_equal(a["y2"][1:], part["y2"]) and np.array_equal(a["mix"][1:], part["mix"])
+
+
+@pytest.mark.parametrize("synth,case", [("sins", ("octave_jumps", "saturated_gd")), ("sins", ("high", "phase_turns")),
+                                        ("sins", ("onsets", "mixed_rows")), ("combsub", ("low", "trained")),
+                                        ("combsub", ("glide", "hot")), ("combsub", ("near_zero", "cold"))],
+                         ids=lambda v: v if isinstance(v, str) else "-".join(v))
+def test_kernel_source_at_input_regimes(emu, synth, case):
+    """The FFT-domain FIR kernel source on the filters of tests/regimes.py: Sins' saturated all-pass (510 taps) with the
+    noise filter as second job, CombSub's dynamic-window harmonic filter (1022 taps), each fed the float64 stage before
+    it rounded to fp32.  Within max(floor, 2 x the fp32 reference FIR's own error) of the float64 FIR, per row.
+    The emulator evaluates __sinf, __sincosf, __expf and __fdividef with exact libm calls (tests/emu/host_emu.h), so
+    this checks indexing, chunking and the host-visible arithmetic at these inputs; it says nothing about the SFU
+    intrinsics' range reduction or large-argument error, which only tests/test_gpu_regimes_*.py see."""
+    from oracle import torch_port as tp
+    inp = R.build(synth, *case)
+    t = R.truth_forward(inp)
+    x1, ir1 = (t["sinusoids"], t["ir_allpass"]) if synth == "sins" else (t["allpassed"], t["ir_harmonic"])
+    jobs = [(x1.astype(np.float32), ir1.astype(np.float32)), (inp["noise"].numpy(), t["ir_noise"].astype(np.float32))]
+    out = emu(jobs[0][0], jobs[0][1], jobs[1][0], jobs[1][1], want=("y1", "y2"))
+    for (x, ir), key in zip(jobs, ("y1", "y2")):
+        truth = cf.ltv_fir(x, ir, P)
+        ref = tp.ltv_fir(torch.from_numpy(x), torch.from_numpy(ir)).numpy()
+        assert np.isfinite(out[key]).all()
+        bad = R.within_budget(R.forward_errors(out[key], ref, truth), 2.0, 3.0)
+        assert not bad, (synth, case, key, bad)

@@ -12,6 +12,8 @@ import pytest
 
 from tests import util
 from tests.golden import cases as G
+import torch
+from tests import regimes as R
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SR, P, WIN = G.SR, G.P, 2048
@@ -82,3 +84,20 @@ def test_in_kernel_noise_is_shard_invariant(emu):
     full = emu(f0, dense, None, seed=3)
     part = emu(f0[1:], dense[1:], None, seed=3, utt_off=1)
     assert np.array_equal(full[1:], part) and np.isfinite(full).all()
+
+
+@pytest.mark.parametrize("case", R.TABLE, ids=R.CASE_IDS)
+def test_kernel_source_at_input_regimes(emu, case):
+    """The forward kernel source at the pitch and control regimes of tests/regimes.py, to the criterion of
+    tests/test_gpu_regimes_forward.py: within max(floor, 2 x the fp32 reference's own error) of float64, per row.
+    The emulator evaluates __sinf, __sincosf, __expf and __fdividef with exact libm calls (tests/emu/host_emu.h), so
+    this checks indexing, chunking and the host-visible arithmetic at these inputs; it says nothing about the SFU
+    intrinsics' range reduction or large-argument error, which only tests/test_gpu_regimes_*.py see."""
+    inp = R.build("superfast", *case)
+    truth = R.truth_forward(inp)["signal"]
+    with torch.no_grad():
+        ref = R.port_forward(inp)["signal"].numpy()
+    got = emu(inp["f0"].numpy(), inp["dense"].numpy(), inp["noise"].numpy())
+    assert np.isfinite(got).all()
+    bad = R.within_budget(R.forward_errors(got, ref, truth), 2.0, 3.0)
+    assert not bad, (case, bad)

@@ -13,6 +13,7 @@ from ddsp_svc_b200 import _lib
 from tests import util
 from tests.golden import make_golden_superfast_grad as GG
 from tests.test_emu_superfast import frame_par
+from tests import regimes as R
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 P, NB = GG.P, GG.WIN // 2 + 1
@@ -109,3 +110,22 @@ def test_backward_abi_argument_errors_do_not_touch_the_device():
     assert call(win=1024, stride=513) == -4 and call(block=256) == -4 and call(B=70000) == -4  # B2D_ERR_UNSUPPORTED
     assert call(g=20) == -3 and call(out=20) == -3 and call(noise=20) == -3 and call(ws=8) == -3   # B2D_ERR_ALIGN
     assert b"superfast_synth_backward" in L.b2d_last_error()
+
+
+@pytest.mark.parametrize("case", [("low", "saturated_gd"), ("high", "phase_turns"), ("onsets", "mixed_rows"),
+                                  ("near_zero", "cold"), ("glide", "hot"), ("octave_jumps", "saturated_gd")],
+                         ids=lambda c: "-".join(c))
+def test_backward_kernel_source_at_input_regimes(emu, case):
+    """The backward kernel source at the pitch and control regimes of tests/regimes.py, to the criterion of
+    tests/test_gpu_regimes_backward.py: per control group and per row, relative L2 error against the float64 closed
+    form within max(1e-5, 2 x the error of torch autograd through the fp32 port).
+    The emulator evaluates __sinf, __sincosf, __expf and __fdividef with exact libm calls (tests/emu/host_emu.h), so
+    this checks indexing, chunking and the host-visible arithmetic at these inputs; it says nothing about the SFU
+    intrinsics' range reduction or large-argument error, which only tests/test_gpu_regimes_*.py see."""
+    inp = R.build("superfast", *case, with_cotangents=True)
+    got = emu(inp["f0"].numpy(), inp["dense"].numpy(), inp["noise"].numpy(), inp["cot"].numpy())
+    assert np.isfinite(got).all()
+    got = dict(zip(R.SPLITS["superfast"], np.split(got, 4, axis=-1)))
+    for k, e in R.grad_errors(got, R.port_grad(inp), R.truth_grad(inp)).items():
+        bound = R.grad_bound(e, 2.0)
+        assert (e["got"] <= bound).all(), (case, k, e["got"], bound)
