@@ -96,6 +96,13 @@ SIGNATURES = {
                                                          c_stream]),
     "b2d_u2c_qkv_gather_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                                    ctypes.c_int, ctypes.c_int, c_f32p, c_stream]),
+    "b2d_rf_start": (ctypes.c_int, [c_f32p, c_f32p, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float,
+                                    ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p, c_f32p, c_f32p, c_stream]),
+    "b2d_rf_layer_input": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_int, c_f32p, ctypes.c_int, c_f32p, ctypes.c_int,
+                                          ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p, c_f32p, c_stream]),
+    "b2d_rf_ode_update": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_float, ctypes.c_int,
+                                         ctypes.c_int, c_f32p, c_f32p, c_stream]),
+    "b2d_rf_finish": (ctypes.c_int, [c_f32p, ctypes.c_float, ctypes.c_float, ctypes.c_int, c_f32p, c_stream]),
     "b2d_mel_frames": (ctypes.c_int, [ctypes.c_int] * 4),
     "b2d_mel_spectrogram": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                            ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, c_f32p, c_stream]),

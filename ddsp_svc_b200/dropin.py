@@ -12,6 +12,7 @@ kernels:
 checkpoint -> class dispatch -> strict load_state_dict) for use without patching.
 """
 import os
+import sys
 
 import torch
 import yaml
@@ -70,11 +71,35 @@ def load_model(model_path, device="cuda"):
     return model, args
 
 
-def patch_reference():
+_REFLOW_MODULES = ("reflow.vocoder", "reflow.naive_v2_diff", "reflow.reflow")
+
+
+def _patch_reflow(saved):
+    """rebind NaiveV2Diff / RectifiedFlow in the reference's reflow modules (those that import); originals into saved"""
+    import importlib
+    from . import reflow as own
+    for modname in _REFLOW_MODULES:
+        try:
+            mod = importlib.import_module(modname)
+        except ImportError as e:
+            saved.setdefault("_not_patched", {})[modname] = "%s: %s" % (type(e).__name__, e)
+            continue
+        for name in ("NaiveV2Diff", "RectifiedFlow"):
+            if hasattr(mod, name):
+                saved.setdefault(name, getattr(mod, name))
+                setattr(mod, name, getattr(own, name))
+
+
+def patch_reference(reflow=False):
     """Swap the synthesizer classes inside the (importable) reference package.  Returns the dict
     of original classes so a caller can restore them; its keys say what was patched.  If the enhancer stack
     (nsf_hifigan.models) cannot be imported, only the synthesizers are patched and the reason is returned under
-    ``"_not_patched"`` -- any other failure propagates."""
+    ``"_not_patched"`` -- any other failure propagates.
+
+    ``reflow=True`` also rebinds the reflow model's velocity network and sampler (``NaiveV2Diff``, ``RectifiedFlow``)
+    in reflow.vocoder, reflow.naive_v2_diff and reflow.reflow, so Unit2Wav samples on the kernels; a module that does not
+    import is reported under ``"_not_patched"``.  Off by default: the package's sampler is inference only, and
+    train_reflow.py needs the reflow loss's backward."""
     import ddsp.vocoder as ref_vocoder          # the reference checkout must be on sys.path
     names = ("Sins", "CombSub", "CombSubSuperFast", "CombSubFast")
     saved = {name: getattr(ref_vocoder, name) for name in names}
@@ -94,11 +119,14 @@ def patch_reference():
         import nsf_hifigan.models as ref_nsf
     except ImportError as e:                    # enhancer stack not importable: synthesizers only (reported below)
         saved.setdefault("_not_patched", {})["nsf_hifigan.models"] = "%s: %s" % (type(e).__name__, e)
-        return saved
-    saved["SineGen"] = ref_nsf.SineGen
-    saved["SourceModuleHnNSF"] = ref_nsf.SourceModuleHnNSF
-    ref_nsf.SineGen = sinegen.SineGen
-    ref_nsf.SourceModuleHnNSF = sinegen.SourceModuleHnNSF
+        ref_nsf = None
+    if ref_nsf is not None:
+        saved["SineGen"] = ref_nsf.SineGen
+        saved["SourceModuleHnNSF"] = ref_nsf.SourceModuleHnNSF
+        ref_nsf.SineGen = sinegen.SineGen
+        ref_nsf.SourceModuleHnNSF = sinegen.SourceModuleHnNSF
+    if reflow:
+        _patch_reflow(saved)
     return saved
 
 
@@ -115,3 +143,9 @@ def unpatch_reference(saved):
         ref_nsf.SineGen = saved["SineGen"]
         if "SourceModuleHnNSF" in saved:
             ref_nsf.SourceModuleHnNSF = saved["SourceModuleHnNSF"]
+    if "NaiveV2Diff" in saved or "RectifiedFlow" in saved:
+        for modname in _REFLOW_MODULES:
+            mod = sys.modules.get(modname)
+            for name in ("NaiveV2Diff", "RectifiedFlow"):
+                if mod is not None and name in saved and hasattr(mod, name):
+                    setattr(mod, name, saved[name])

@@ -175,6 +175,15 @@ class _Gemm:
         out.addmm_(xh, wl.t())
         return out
 
+    def mm(self, xs, w, bias=None):
+        """xs [N, K] @ w^T (+ bias) with xs already in operand form (from ``split``, or from a kernel that writes the
+        TF32 halves itself); w packed"""
+        if self.mode != "3xtf32":
+            return torch.mm(xs, w.t()) if bias is None else torch.addmm(bias, xs, w.t())
+        (xh, xl), (wh, wl) = xs, w
+        out = torch.mm(xh, wh.t()) if bias is None else torch.addmm(bias, xh, wh.t())
+        return out.addmm_(xl, wh.t()).addmm_(xh, wl.t())
+
     def split(self, x2d):
         """an activation prepared for the products below: (hi, lo) in 3xtf32 mode, itself otherwise"""
         return _split(x2d) if self.mode == "3xtf32" else x2d.contiguous()

@@ -406,6 +406,30 @@ int b2d_u2c_softmax_features_backward(float* g, const float* features, const flo
 int b2d_u2c_qkv_gather_backward(const float* g_q, const float* g_k, const float* g_v, const float* qkv, int B, int H, int T,
                                 int dim_head, int normalized, float* g_qkv, void* stream);
 
+/* ---- rectified-flow sampler of the reflow model (reflow.cu; reflow/reflow.py:51-111 around the velocity network
+ * reflow/naive_v2_diff.py with conv_only and use_mlp=False): the stages between the caller's library GEMMs.  Activations
+ * are token-major [B, T, C] fp32, G is a GEMM's output WITHOUT its bias.  Every output that feeds a GEMM is written as the
+ * GEMM's operand: fp32 into `hi` when `lo` is NULL, else the TF32-exact halves (hi, lo) of b2d_split_tf32.  Elementwise,
+ * no atomics: bit-identical from run to run.
+ * rf_start: x0 [B, T, M] = t_start norm(gt) + one_minus_t_start noise with norm(v) = ((v - spec_min) / spec_range) 2 - 1,
+ *   noise [B, 1, M, T] channel-major, gt [B, T, M] or NULL (then x0 = noise: also the transposing entry of a standalone
+ *   velocity evaluation); x [B, T, M] receives x0 (or NULL), hi / lo its operand.
+ * rf_layer_input: h [B, T, D] = GELU(G + bias) (exact erf; residual = 0) or (G + bias) + h (residual = 1), in place; then
+ *   u = (h + step[b]) + cond[b, t] into hi / lo, with step row b at step + b step_stride (0: one row for every
+ *   utterance) and cond row b T + t at cond + (b T + t) cond_stride; step = cond = NULL: u = h.  D, strides multiples of
+ *   4, buffers 16-byte aligned.
+ * rf_ode_update: v = G + bias over x [n_tokens, M].  stage -1: Euler x += v dt, emits x.  RK4 stages 0..3 with acc
+ *   [n_tokens, M]: 0: acc = v, emits x + (0.5 v) dt; 1: acc += 2 v, emits x + (0.5 v) dt; 2: acc += 2 v, emits x + v dt;
+ *   3: x += ((acc + v) dt) / 6, emits x.
+ * rf_finish: out [n] = ((x + 1) / 2) spec_range + spec_min. */
+int b2d_rf_start(const float* noise, const float* gt, float t_start, float one_minus_t_start, float spec_min,
+                 float spec_range, int B, int T, int M, float* x, float* hi, float* lo, void* stream);
+int b2d_rf_layer_input(const float* g, const float* bias, float* h, int residual, const float* step, int step_stride,
+                       const float* cond, int cond_stride, int B, int T, int D, float* hi, float* lo, void* stream);
+int b2d_rf_ode_update(const float* g, const float* bias, float* x, float* acc, int stage, float dt, int n_tokens, int M,
+                      float* hi, float* lo, void* stream);
+int b2d_rf_finish(const float* x, float spec_min, float spec_range, int n, float* out, void* stream);
+
 /* ---- log-mel front end of the NSF-HiFiGAN vocoder: STFT.get_mel, nsf_hifigan/nvSTFT.py:73-117 (keyshift 0, speed 1) ----
  * audio [B, n_samples] -> mel [B, n_mels, n_frames], n_frames = b2d_mel_frames(...) (0 = signal too short):
  * reflect / constant padding by (win - hop)/2, frames of win_size = n_fft = 2048 at `hop`, periodic Hann `window` [2048],
