@@ -103,6 +103,20 @@ SIGNATURES = {
     "b2d_rf_ode_update": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_float, ctypes.c_int,
                                          ctypes.c_int, c_f32p, c_f32p, c_stream]),
     "b2d_rf_finish": (ctypes.c_int, [c_f32p, ctypes.c_float, ctypes.c_float, ctypes.c_int, c_f32p, c_stream]),
+    "b2d_rf_backward_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int] * 3),
+    "b2d_rf_loss_input": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_float, ctypes.c_float, ctypes.c_int, ctypes.c_int,
+                                         ctypes.c_int, c_f32p, c_f32p, c_f32p, c_stream]),
+    "b2d_rf_loss": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                   ctypes.c_size_t, c_f32p, c_stream]),
+    "b2d_rf_loss_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                            c_f32p, c_f32p, c_f32p, c_stream]),
+    "b2d_rf_gelu_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, c_f32p, c_f32p, c_f32p,
+                                            c_stream]),
+    "b2d_rf_layer_backward": (ctypes.c_int, [c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                             ctypes.c_int, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_void_p,
+                                             ctypes.c_size_t, c_stream]),
+    "b2d_rf_step_sums": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p,
+                                        c_stream]),
     "b2d_mel_frames": (ctypes.c_int, [ctypes.c_int] * 4),
     "b2d_mel_spectrogram": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                            ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, c_f32p, c_stream]),

@@ -98,8 +98,10 @@ def patch_reference(reflow=False):
 
     ``reflow=True`` also rebinds the reflow model's velocity network and sampler (``NaiveV2Diff``, ``RectifiedFlow``)
     in reflow.vocoder, reflow.naive_v2_diff and reflow.reflow, so Unit2Wav samples on the kernels; a module that does not
-    import is reported under ``"_not_patched"``.  Off by default: the package's sampler is inference only, and
-    train_reflow.py needs the reflow loss's backward."""
+    import is reported under ``"_not_patched"``.  Off by default.  To run train_reflow.py on the kernels, also set
+    ``ddsp_svc_b200.NaiveV2Diff.reflow_backward = True``: then ``RectifiedFlow(infer=False)`` returns the reflow loss
+    with its backward, and Unit2Wav's training step trains every parameter (INTEGRATION.md section 3b); without it
+    infer=False and the sampler under grad raise NotImplementedError."""
     import ddsp.vocoder as ref_vocoder          # the reference checkout must be on sys.path
     names = ("Sins", "CombSub", "CombSubSuperFast", "CombSubFast")
     saved = {name: getattr(ref_vocoder, name) for name in names}

@@ -430,6 +430,34 @@ int b2d_rf_ode_update(const float* g, const float* bias, float* x, float* acc, i
                       float* hi, float* lo, void* stream);
 int b2d_rf_finish(const float* x, float spec_min, float spec_range, int n, float* out, void* stream);
 
+/* ---- reflow training loss (reflow/reflow.py:20-35, :63-68, loss_type 'l2_lognorm') and the velocity network's backward
+ * (reflow_bwd.cu): the stages between the caller's library GEMMs and their adjoints.  Token-major [B, T, C] fp32; G is a
+ * GEMM output WITHOUT its bias.  Operand outputs (hi, lo) as above, and optional where a fp32 output is also written
+ * (hi = lo = NULL: none; lo NULL: fp32 copy into hi).  No atomics: sums over tokens run per fixed slab of 32 frames of
+ * one utterance into `ws` (fp64), then slab by slab in order, so results are bit-identical from run to run and do not
+ * depend on the device.  `ws` is scratch of at least b2d_rf_backward_workspace_bytes(B, T, cols) bytes with cols = M
+ * (rf_loss) or D n_layers (rf_layer_backward / rf_step_sums); 0 = bad shape.
+ * rf_loss_input: gt [B, T, M], x0 [B, T, M] token-major, t [B] -> target = x1 - x0 with x1 = norm(gt) (as rf_start), and the
+ *   operand of x_t = x0 + t_b target (fp32 products and sums in that order, no contraction) into hi / lo (hi required).
+ * rf_loss: loss [1] (device) = mean over [B, T, M] of w_b (target - (G + bias[m]))^2, w [B] the per-utterance weights.
+ * rf_loss_backward: gv [B, T, M] = (g_loss[0] 2 w_b / (B T M)) ((G + bias) - target), g_loss a device scalar.
+ * rf_gelu_backward: gx [n_rows, C] = gy (Phi(x) + x phi(x)) with x = pre + bias[c] (bias NULL: x = pre).
+ * rf_layer_backward: for layer `layer` of n_layers: gh [B T, D] += gz in place (operand into gh_hi / gh_lo); gz into
+ *   columns [layer D, (layer + 1) D) of z [B T, D n_layers] (operand into z_hi / z_lo); gz's per-slab sums into ws.
+ * rf_step_sums: out [B, cols] = per-utterance token sums of every column rf_layer_backward wrote into ws. */
+size_t b2d_rf_backward_workspace_bytes(int B, int T, int cols);
+int b2d_rf_loss_input(const float* gt, const float* x0, const float* t, float spec_min, float spec_range, int B, int T, int M,
+                      float* target, float* hi, float* lo, void* stream);
+int b2d_rf_loss(const float* g, const float* bias, const float* target, const float* w, int B, int T, int M, void* ws,
+                size_t ws_bytes, float* loss, void* stream);
+int b2d_rf_loss_backward(const float* g, const float* bias, const float* target, const float* w, const float* g_loss, int B,
+                         int T, int M, float* gv, float* hi, float* lo, void* stream);
+int b2d_rf_gelu_backward(const float* gy, const float* pre, const float* bias, int n_rows, int C, float* gx, float* hi,
+                         float* lo, void* stream);
+int b2d_rf_layer_backward(const float* gz, float* gh, int B, int T, int D, int layer, int n_layers, float* gh_hi, float* gh_lo,
+                          float* z, float* z_hi, float* z_lo, void* ws, size_t ws_bytes, void* stream);
+int b2d_rf_step_sums(const void* ws, size_t ws_bytes, int B, int T, int cols, float* out, void* stream);
+
 /* ---- log-mel front end of the NSF-HiFiGAN vocoder: STFT.get_mel, nsf_hifigan/nvSTFT.py:73-117 (keyshift 0, speed 1) ----
  * audio [B, n_samples] -> mel [B, n_mels, n_frames], n_frames = b2d_mel_frames(...) (0 = signal too short):
  * reflect / constant padding by (win - hop)/2, frames of win_size = n_fft = 2048 at `hop`, periodic Hann `window` [2048],
