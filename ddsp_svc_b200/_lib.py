@@ -6,6 +6,7 @@ raises -- the product path never degrades to PyTorch or to the oracle.
 """
 import ctypes
 import os
+import re
 import subprocess
 import threading
 
@@ -19,155 +20,49 @@ HEADER = os.path.join(ROOT, "include", "b200ddsp.h")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
-c_f32p = ctypes.c_void_p   # device pointers travel as integers
-c_f64p = ctypes.c_void_p
-c_stream = ctypes.c_void_p
+# C type -> ctypes type of the scalars in include/b200ddsp.h and tests/emu/*.cpp.  Pointers are c_void_p (device
+# pointers travel as integers), except a returned `const char*`.  Anything else is an error: a new type is mapped here
+# on purpose, never guessed.
+_CTYPES = {"int": ctypes.c_int, "unsigned": ctypes.c_uint, "int64_t": ctypes.c_int64, "long long": ctypes.c_int64,
+          "uint64_t": ctypes.c_uint64, "unsigned long long": ctypes.c_uint64, "size_t": ctypes.c_size_t,
+          "float": ctypes.c_float, "double": ctypes.c_double}
+_TYPE_WORDS = {"const", "void", "bool", "char", "short", "int", "long", "signed", "unsigned", "float", "double"}
 
-# name -> (restype, argtypes); must list every symbol include/b200ddsp.h declares
-SIGNATURES = {
-    "b2d_version": (ctypes.c_int, []),
-    "b2d_last_error": (ctypes.c_char_p, []),
-    "b2d_phase_scan": (ctypes.c_int, [c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double,
-                                      ctypes.c_int, c_f64p, c_f32p, c_stream]),
-    "b2d_sins_bank": (ctypes.c_int, [c_f32p, c_f64p, c_f32p, ctypes.c_int64, ctypes.c_int, ctypes.c_int,
-                                     ctypes.c_int, ctypes.c_int, ctypes.c_double, ctypes.c_int, c_f32p, c_stream]),
-    "b2d_set_ir_impl": (ctypes.c_int, [ctypes.c_int]),
-    "b2d_dft_tables_bytes": (ctypes.c_size_t, [ctypes.c_int]),
-    "b2d_dft_tables": (ctypes.c_int, [ctypes.c_int, c_f32p, c_stream]),
-    "b2d_ir_build": (ctypes.c_int, [c_f32p, ctypes.c_int64, ctypes.c_int, c_f32p, c_f32p, ctypes.c_int,
-                                    ctypes.c_int, ctypes.c_int, ctypes.c_double, c_f32p, c_stream]),
-    "b2d_ltv_fir": (ctypes.c_int, [c_f32p, c_f32p, ctypes.c_int, c_f32p, c_f32p, c_f32p, ctypes.c_int, c_f32p,
-                                   c_f32p, ctypes.c_uint64, ctypes.c_int64, ctypes.c_int, ctypes.c_int,
-                                   ctypes.c_int, c_stream]),
-    "b2d_set_fir_impl": (ctypes.c_int, [ctypes.c_int]),
-    "b2d_ltv_fir_generic": (ctypes.c_int, [c_f32p, c_f32p, ctypes.c_int, c_f32p, ctypes.c_int, ctypes.c_int,
-                                           ctypes.c_int, c_stream]),
-    "b2d_sins_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int] * 5),
-    "b2d_sins_synth": (ctypes.c_int, [c_f32p, c_f64p, c_f32p, c_f32p, c_f32p, ctypes.c_int64, c_f32p,
-                                      ctypes.c_uint64, ctypes.c_int64, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int,
-                                      ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double,
-                                      ctypes.c_int, c_f32p, c_f32p, c_f32p, ctypes.c_void_p, ctypes.c_size_t,
-                                      c_stream]),
-    "b2d_sins_synth_backward_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int] * 3),
-    "b2d_sins_synth_backward": (ctypes.c_int, [c_f32p, c_f64p, c_f32p, c_f32p, c_f32p, ctypes.c_int64, c_f32p,
-                                               ctypes.c_uint64, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int, c_f32p,
-                                               c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                               ctypes.c_int, ctypes.c_int, ctypes.c_double, c_f32p, ctypes.c_void_p,
-                                               ctypes.c_size_t, c_stream]),
-    "b2d_sinegen": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_uint64, ctypes.c_int64, ctypes.c_int,
-                                   ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double, ctypes.c_float,
-                                   ctypes.c_float, ctypes.c_float, c_f32p, c_f32p, c_stream]),
-    "b2d_source_module": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_uint64, ctypes.c_int64, ctypes.c_int,
-                                         ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double, ctypes.c_float,
-                                         ctypes.c_float, ctypes.c_float, c_f32p, ctypes.c_float, c_f32p, c_f32p,
-                                         c_stream]),
-    "b2d_set_sinegen_impl": (ctypes.c_int, [ctypes.c_int]),
-    "b2d_set_fft_arith": (ctypes.c_int, [ctypes.c_int]),
-    "b2d_set_overlap": (ctypes.c_int, [ctypes.c_int]),
-    "b2d_split_tf32": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_size_t, c_stream]),
-    "b2d_u2c_embed": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int, c_f32p, ctypes.c_int,
-                                     ctypes.c_int, c_stream]),
-    "b2d_u2c_groupnorm_lrelu": (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p, c_f32p,
-                                               ctypes.c_float, ctypes.c_float, c_f64p, c_stream]),
-    "b2d_u2c_layernorm": (ctypes.c_int, [c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, c_f32p, c_f32p, ctypes.c_float, c_stream]),
-    "b2d_u2c_glu_dwconv_silu": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                               ctypes.c_int, c_stream]),
-    "b2d_u2c_softmax_features": (ctypes.c_int, [c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                                ctypes.c_float, c_stream]),
-    "b2d_u2c_linear_attention": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                                ctypes.c_int, ctypes.c_int, ctypes.c_float, c_stream]),
-    "b2d_u2c_backward_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int] * 4),
-    "b2d_u2c_glu_dwconv_silu_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int,
-                                                        ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
-                                                        ctypes.c_size_t, c_stream]),
-    "b2d_u2c_colsum": (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, c_f32p, ctypes.c_void_p, ctypes.c_size_t, c_stream]),
-    "b2d_u2c_layernorm_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_float, ctypes.c_int, ctypes.c_int, c_f32p,
-                                                  c_f32p, ctypes.c_void_p, ctypes.c_size_t, c_stream]),
-    "b2d_u2c_groupnorm_lrelu_backward": (ctypes.c_int, [c_f32p, c_f64p, c_f32p, c_f32p, ctypes.c_float, ctypes.c_float, c_f32p,
-                                                        ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p, c_f32p,
-                                                        ctypes.c_void_p, ctypes.c_size_t, c_stream]),
-    "b2d_u2c_embed_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, c_f32p,
-                                              c_f32p, ctypes.c_void_p, ctypes.c_size_t, c_stream]),
-    "b2d_u2c_conv3_fold": (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p, c_stream]),
-    "b2d_u2c_attn_readout_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                                     ctypes.c_int, c_f32p, c_stream]),
-    "b2d_u2c_softmax_features_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int,
-                                                         ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, c_f32p,
-                                                         c_stream]),
-    "b2d_u2c_qkv_gather_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                                   ctypes.c_int, ctypes.c_int, c_f32p, c_stream]),
-    "b2d_rf_start": (ctypes.c_int, [c_f32p, c_f32p, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float,
-                                    ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p, c_f32p, c_f32p, c_stream]),
-    "b2d_rf_layer_input": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_int, c_f32p, ctypes.c_int, c_f32p, ctypes.c_int,
-                                          ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p, c_f32p, c_stream]),
-    "b2d_rf_ode_update": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_float, ctypes.c_int,
-                                         ctypes.c_int, c_f32p, c_f32p, c_stream]),
-    "b2d_rf_finish": (ctypes.c_int, [c_f32p, ctypes.c_float, ctypes.c_float, ctypes.c_int, c_f32p, c_stream]),
-    "b2d_rf_backward_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int] * 3),
-    "b2d_rf_loss_input": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_float, ctypes.c_float, ctypes.c_int, ctypes.c_int,
-                                         ctypes.c_int, c_f32p, c_f32p, c_f32p, c_stream]),
-    "b2d_rf_loss": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
-                                   ctypes.c_size_t, c_f32p, c_stream]),
-    "b2d_rf_loss_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                            c_f32p, c_f32p, c_f32p, c_stream]),
-    "b2d_rf_gelu_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, c_f32p, c_f32p, c_f32p,
-                                            c_stream]),
-    "b2d_rf_layer_backward": (ctypes.c_int, [c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                             ctypes.c_int, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_void_p,
-                                             ctypes.c_size_t, c_stream]),
-    "b2d_rf_step_sums": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p,
-                                        c_stream]),
-    "b2d_mel_frames": (ctypes.c_int, [ctypes.c_int] * 4),
-    "b2d_mel_spectrogram": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                           ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, c_f32p, c_stream]),
-    "b2d_mel_spectrogram_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
-                                                    ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                                    ctypes.c_float, c_f32p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64,
-                                                    c_f32p, c_stream]),
-    "b2d_volume_extract": (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p, c_stream]),
-    "b2d_volume_mask": (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_float, c_f32p, c_stream]),
-    "b2d_mask_apply": (ctypes.c_int, [c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                      c_stream]),
-    "b2d_cross_fade": (ctypes.c_int, [c_f32p, ctypes.c_int64, c_f32p, ctypes.c_int64, ctypes.c_int64, c_f32p, c_stream]),
-    "b2d_set_sins_impl": (ctypes.c_int, [ctypes.c_int]),
-    "b2d_combsubfast_filter": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int64, c_f32p, ctypes.c_uint64,
-                                              ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p, c_stream]),
-    "b2d_combsubfast_filter_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int64, c_f32p,
-                                                       ctypes.c_uint64, ctypes.c_int64, c_f32p, ctypes.c_int,
-                                                       ctypes.c_int, ctypes.c_int, c_f32p, c_stream]),
-    "b2d_comb_source": (ctypes.c_int, [c_f32p, c_f64p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double,
-                                       ctypes.c_int, c_f32p, c_stream]),
-    "b2d_combsub_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int] * 6),
-    "b2d_combsub_synth": (ctypes.c_int, [c_f32p, c_f64p, c_f32p, c_f32p, c_f32p, ctypes.c_int64, c_f32p,
-                                         ctypes.c_uint64, ctypes.c_int64, c_f32p, c_f32p, c_f32p, ctypes.c_int,
-                                         ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                         ctypes.c_double, ctypes.c_int, c_f32p, c_f32p, c_f32p, ctypes.c_void_p,
-                                         ctypes.c_size_t, c_stream]),
-    "b2d_combsub_synth_backward_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int] * 3),
-    "b2d_combsub_synth_backward": (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int64, c_f32p,
-                                                  ctypes.c_uint64, ctypes.c_int64, ctypes.c_void_p, c_f32p, c_f32p,
-                                                  c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                                  ctypes.c_int, ctypes.c_int, ctypes.c_double, c_f32p,
-                                                  ctypes.c_void_p, ctypes.c_size_t, c_stream]),
-    "b2d_superfast_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int, ctypes.c_int]),
-    "b2d_superfast_scan": (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double,
-                                          ctypes.c_void_p, c_f32p, c_stream]),
-    "b2d_superfast_synth": (ctypes.c_int, [ctypes.c_void_p, c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int64, c_f32p,
-                                           ctypes.c_uint64, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                           ctypes.c_int, c_f32p, c_stream]),
-    "b2d_superfast_synth_backward": (ctypes.c_int, [ctypes.c_void_p, c_f32p, c_f32p, c_f32p, c_f32p, ctypes.c_int64,
-                                                    c_f32p, ctypes.c_uint64, ctypes.c_int64, c_f32p, ctypes.c_int,
-                                                    ctypes.c_int, ctypes.c_int, ctypes.c_int, c_f32p, c_stream]),
-    "b2d_rss_table_floats": (ctypes.c_int, [ctypes.c_int]),
-    "b2d_rss_frames": (ctypes.c_int, [ctypes.c_int, ctypes.c_int]),
-    "b2d_rss_loss_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
-    "b2d_rss_loss_forward": (ctypes.c_int, [c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
-                                            ctypes.c_void_p, ctypes.c_float, ctypes.c_float, ctypes.c_void_p,
-                                            ctypes.c_size_t, c_f64p, c_f32p, c_stream]),
-    "b2d_rss_loss_backward": (ctypes.c_int, [c_f32p, c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
-                                             ctypes.c_void_p, ctypes.c_float, ctypes.c_float, c_f64p, c_f32p, c_f32p,
-                                             c_stream]),
-}
+
+def _ctype(c_type, decl, result=False):
+    if "*" in c_type:
+        return ctypes.c_char_p if result and c_type == "const char*" else ctypes.c_void_p
+    if result and c_type == "void":
+        return None
+    if c_type not in _CTYPES:
+        raise ValueError("no ctypes mapping for %r in: %s" % (c_type, decl))
+    return _CTYPES[c_type]
+
+
+def prototypes(text, prefix):
+    """{name: (restype, [(ctype, param_name), ...])} of every function whose name starts with `prefix` that the C/C++
+    source `text` declares or defines (`<return type> <name>(<params>)` followed by `;` or `{`)."""
+    text = re.sub(r"/\*.*?\*/|//[^\n]*", " ", text, flags=re.S)
+    text = re.sub(r"^[ \t]*#[^\n]*", "", text, flags=re.M)
+    norm = lambda s: re.sub(r"\s*\*\s*", "* ", " ".join(s.split())).strip()
+    found = {}
+    for m in re.finditer(r"([A-Za-z_][\w\s*]*?)\s*\b(%s\w*)\s*\(([^()]*)\)\s*[;{]" % re.escape(prefix), text):
+        decl = " ".join(m.group(0).split())
+        params = []
+        if norm(m.group(3)) not in ("", "void"):
+            for p in m.group(3).split(","):
+                pm = re.fullmatch(r"(.*[\s*])(\w+)", norm(p))
+                if not pm or pm.group(2) in _TYPE_WORDS:
+                    raise ValueError("parameter without a name (%r) in: %s" % (norm(p), decl))
+                params.append((_ctype(pm.group(1).strip(), decl), pm.group(2)))
+        found[m.group(2)] = (_ctype(norm(m.group(1)), decl, result=True), params)
+    return found
+
+
+with open(HEADER) as _f:
+    PROTOTYPES = prototypes(_f.read(), "b2d_")
+# name -> (restype, argtypes) of every entry point include/b200ddsp.h declares
+SIGNATURES = dict((name, (res, [t for t, _ in params])) for name, (res, params) in PROTOTYPES.items())
 
 _lock = threading.Lock()
 _lib = None

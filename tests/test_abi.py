@@ -23,6 +23,24 @@ def test_header_and_binding_agree(lib):
         assert hasattr(lib, name), name
 
 
+def test_binding_is_parsed_from_the_header():
+    with open(_lib.HEADER) as f:
+        hdr = re.sub(r"/\*.*?\*/|//[^\n]*", " ", f.read(), flags=re.S)
+    parsed = _lib.prototypes(hdr, "b2d_")
+    # every declaration is read: one the parser could not read would otherwise drop out of the binding silently
+    assert len(parsed) == len(re.findall(r"\bb2d_\w+\s*\(", hdr)) == len(_lib.SIGNATURES)
+    assert parsed["b2d_last_error"][0] is ctypes.c_char_p
+    assert all(res is ctypes.c_size_t for name, (res, _) in parsed.items() if name.endswith("_workspace_bytes"))
+    assert parsed["b2d_rss_loss_forward"][1][6] == (ctypes.c_void_p, "tables")          # const float* const*
+    want = {"seed": ctypes.c_uint64, "ctrl_stride": ctypes.c_int64, "utterance_offset": ctypes.c_int64,
+            "sampling_rate": ctypes.c_double, "alpha": ctypes.c_float}
+    seen = {(p, t) for _, params in parsed.values() for t, p in params if p in want}
+    assert seen == set(want.items())
+    for decl in ("int b2d_x(bool flag);", "long double b2d_x(int n);", "int b2d_x(int);", "int b2d_x(const float*, int n);"):
+        with pytest.raises(ValueError, match=re.escape(decl)):
+            _lib.prototypes(decl, "b2d_")
+
+
 def test_version_and_error_string(lib):
     assert lib.b2d_version() == 100
     rc = lib.b2d_phase_scan(0, 0, 1, 1, 512, 44100.0, 0, 0, 0, 0)

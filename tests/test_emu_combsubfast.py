@@ -5,9 +5,6 @@ This is what stands in for the GPU parity run of this kernel until it has execut
 index arithmetic, barrier placement, in-place pairing and overlap-add of the .cu file (fp32, like the device), for
 full, ragged and single-frame chunks.  It cannot see PTX-level or performance problems."""
 import ctypes
-import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -18,25 +15,15 @@ from oracle import closed_form as cf
 from tests import util
 from tests.golden import cases as G
 from tests import regimes as R
+from tests.emu_harness import shared
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 SR, P = G.SR, G.P
-
-pytestmark = pytest.mark.skipif(shutil.which("g++") is None, reason="g++ not available")
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("emu") / "libemu_csfast.so")
-    cmd = ["g++", "-std=c++20", "-O2", "-shared", "-fPIC", "-pthread", "-Wno-unknown-pragmas", "-o", so,
-           os.path.join(HERE, "emu", "emu_combsubfast.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    assert proc.returncode == 0, proc.stderr
-    lib = ctypes.CDLL(so)
+    lib = shared("emu_combsubfast.cpp", tmp_path_factory)
     fp = ctypes.POINTER(ctypes.c_float)
-    lib.emu_combsubfast.argtypes = [fp, fp, fp, fp, ctypes.c_longlong, fp, ctypes.c_ulonglong, ctypes.c_longlong,
-                                    ctypes.c_int, ctypes.c_int, ctypes.c_int, fp]
-    lib.emu_combsubfast.restype = ctypes.c_int
 
     def run(comb, dense, noise, G_hops=32, seed=0, utt_off=0):
         """comb [B,T] f32, dense controls [B,nF,3*(P+1)] f32 (views share the frame stride), noise [B,T] or None"""

@@ -2,9 +2,6 @@
 autograd gradients (tests/golden/csfast_grad_*.npz), race-checked under ThreadSanitizer, plus the argument checks of
 its C ABI entry (no device touched).  The kernel itself runs on hardware in tests/test_gpu_combsubfast_backward.py."""
 import ctypes
-import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -15,30 +12,19 @@ from oracle import torch_port as tp
 from tests import util
 from tests.golden import make_golden_combsubfast_grad as GG
 from tests import regimes as R
+from tests.emu_harness import abi_call, assert_race_free, shared, tsan
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 P, NB = GG.P, GG.NB
 f32 = np.float32
 # per-control relative RMS bounds.  The emulation is fed the comb the reference filtered (the oracle port's, bit-identical),
 # so both sides sit at the fp32 floor of 1.5 single-precision 1024-point transforms per frame
 BOUND = {"harmonic_magnitude": 1e-5, "harmonic_phase": 1e-5, "noise_magnitude": 1e-5}
 
-needs_gxx = pytest.mark.skipif(shutil.which("g++") is None, reason="g++ not available")
-
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = str(tmp_path_factory.mktemp("emu") / "libemu_csfast_bwd.so")
-    cmd = ["g++", "-std=c++20", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-pthread", "-Wno-unknown-pragmas",
-           "-o", so, os.path.join(HERE, "emu", "emu_combsubfast_bwd.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    assert proc.returncode == 0, proc.stderr
-    lib = ctypes.CDLL(so)
+    lib = shared("emu_combsubfast_bwd.cpp", tmp_path_factory)
     fp = ctypes.POINTER(ctypes.c_float)
-    lib.emu_combsubfast_bwd.argtypes = [fp, fp, fp, fp, ctypes.c_longlong, fp, ctypes.c_ulonglong, ctypes.c_longlong,
-                                        fp, ctypes.c_int, ctypes.c_int, ctypes.c_int, fp]
 
     def run(comb, dense, noise, g, hops=32, seed=0, utt_off=0):
         B, T = comb.shape
@@ -102,38 +88,23 @@ def test_in_kernel_noise_rows_are_shard_invariant(emu):
     assert util.rms(full[noise] - other[noise]) >= 0.5 * util.rms(full[noise])
 
 
-@needs_gxx
 def test_backward_kernel_source_has_no_shared_memory_race(tmp_path):
-    exe = str(tmp_path / "tsan_combsubfast_bwd")
-    cmd = ["g++", "-std=c++20", "-O1", "-g", "-fsanitize=thread", "-pthread", "-Wno-unknown-pragmas", "-o", exe,
-           os.path.join(HERE, "emu", "tsan_combsubfast_bwd.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    if proc.returncode != 0 and "tsan" in proc.stderr.lower():
-        pytest.skip("ThreadSanitizer runtime not available: " + proc.stderr.strip().splitlines()[-1])
-    assert proc.returncode == 0, proc.stderr
-    res = subprocess.run([exe], capture_output=True, text=True, timeout=600,
-                         env=dict(os.environ, TSAN_OPTIONS="halt_on_error=0 exitcode=66"))
-    assert "ThreadSanitizer" not in res.stderr, res.stderr[-4000:]
-    assert res.returncode == 0 and "done" in res.stdout
+    assert_race_free(tsan("tsan_combsubfast_bwd.cpp", tmp_path))
 
 
 def test_backward_abi_argument_errors_do_not_touch_the_device():
     _lib.build()
     L = _lib.lib()
-    f = L.b2d_combsubfast_filter_backward
-    ok = dict(comb=16, hm=16, hp=16, nm=16, stride=3 * NB, noise=0, seed=0, off=0, g=16, B=1, nF=4, block=512, out=16,
-              stream=0)
-
-    def call(**kw):
-        a = dict(ok, **kw)
-        return f(a["comb"], a["hm"], a["hp"], a["nm"], a["stride"], a["noise"], a["seed"], a["off"], a["g"], a["B"],
-                 a["nF"], a["block"], a["out"], a["stream"])
-
-    assert call(comb=0) == -1 and call(hm=0) == -1 and call(hp=0) == -1 and call(nm=0) == -1     # B2D_ERR_NULL
-    assert call(g=0) == -1 and call(out=0) == -1
-    assert call(B=0) == -2 and call(nF=0) == -2 and call(nF=-3) == -2 and call(stride=512) == -2  # B2D_ERR_SHAPE
-    assert call(block=256) == -4 and call(block=1024) == -4 and call(B=70000) == -4            # B2D_ERR_UNSUPPORTED
-    assert call(comb=20) == -3 and call(g=20) == -3 and call(out=20) == -3 and call(noise=20) == -3   # B2D_ERR_ALIGN
+    ok = dict(comb=16, c_hm=16, c_hp=16, c_nm=16, ctrl_stride=3 * NB, noise_in=0, seed=0, utterance_offset=0,
+              grad_signal=16, B=1, n_frames=4, block=512, grad_ctrl=16, stream=0)
+    call = lambda **kw: abi_call("b2d_combsubfast_filter_backward", dict(ok, **kw))
+    assert call(comb=0) == -1 and call(c_hm=0) == -1 and call(c_hp=0) == -1 and call(c_nm=0) == -1   # B2D_ERR_NULL
+    assert call(grad_signal=0) == -1 and call(grad_ctrl=0) == -1
+    assert call(B=0) == -2 and call(n_frames=0) == -2 and call(n_frames=-3) == -2                      # B2D_ERR_SHAPE
+    assert call(ctrl_stride=512) == -2
+    assert call(block=256) == -4 and call(block=1024) == -4 and call(B=70000) == -4                    # B2D_ERR_UNSUPPORTED
+    assert call(comb=20) == -3 and call(grad_signal=20) == -3 and call(grad_ctrl=20) == -3             # B2D_ERR_ALIGN
+    assert call(noise_in=20) == -3
     assert b"combsubfast_backward" in L.b2d_last_error()
 
 

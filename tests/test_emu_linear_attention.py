@@ -2,28 +2,18 @@
 performer's non-causal linear attention (reference ddsp/pcmer.py:220-229) and against the reference function itself."""
 import ctypes
 import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-pytestmark = pytest.mark.skipif(shutil.which("g++") is None, reason="g++ not available")
+from tests.emu_harness import shared
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("emu") / "libemu_linattn.so")
-    cmd = ["g++", "-std=c++20", "-O2", "-shared", "-fPIC", "-pthread", "-Wno-unknown-pragmas", "-o", so,
-           os.path.join(HERE, "emu", "emu_linear_attention.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    assert proc.returncode == 0, proc.stderr
-    lib = ctypes.CDLL(so)
+    lib = shared("emu_linear_attention.cpp", tmp_path_factory)
     fp = ctypes.POINTER(ctypes.c_float)
-    lib.emu_linear_attention.argtypes = [fp, fp, fp, fp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float]
-    lib.emu_linear_attention.restype = ctypes.c_int
 
     def run(qf, kf, v, eps=1e-8):
         B, H, T, J = qf.shape

@@ -2,9 +2,6 @@
 FIR (fp64 closed form of ddsp/core.py:120-182 and the bit-identical torch port), for one and two jobs, equal and
 different tap counts, chunked / ragged hop ranges, the addend path and in-kernel noise."""
 import ctypes
-import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -13,25 +10,15 @@ import torch
 from oracle import closed_form as cf
 from tests import util
 from tests import regimes as R
+from tests.emu_harness import shared
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 P = 512
-
-pytestmark = pytest.mark.skipif(shutil.which("g++") is None, reason="g++ not available")
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("emu") / "libemu_firfft.so")
-    cmd = ["g++", "-std=c++20", "-O2", "-shared", "-fPIC", "-pthread", "-Wno-unknown-pragmas", "-o", so,
-           os.path.join(HERE, "emu", "emu_ltv_fir_fft.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    assert proc.returncode == 0, proc.stderr
-    lib = ctypes.CDLL(so)
+    lib = shared("emu_ltv_fir_fft.cpp", tmp_path_factory)
     fp = ctypes.POINTER(ctypes.c_float)
-    lib.emu_ltv_fir_fft.argtypes = [fp, fp, ctypes.c_int, fp, fp, fp, ctypes.c_int, fp, fp, fp, ctypes.c_ulonglong,
-                                    ctypes.c_longlong, ctypes.c_int, ctypes.c_int, ctypes.c_int]
-    lib.emu_ltv_fir_fft.restype = ctypes.c_int
 
     def run(x1, ir1, x2=None, ir2=None, addend=None, hops=32, seed=0, utt_off=0, want=("y1", "y2", "mix")):
         B, nF, L1 = ir1.shape
@@ -186,16 +173,8 @@ def test_random_shapes_fuzz(emu):
 # ---- spectrum path: ir_spectrum_kernel + the SPEC variant of the FIR kernel (impulse-response spectra read from memory) ----
 @pytest.fixture(scope="module")
 def emu_spec(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("emu") / "libemu_firfft_spec.so")
-    cmd = ["g++", "-std=c++20", "-O2", "-shared", "-fPIC", "-pthread", "-Wno-unknown-pragmas", "-o", so,
-           os.path.join(HERE, "emu", "emu_ltv_fir_fft.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    assert proc.returncode == 0, proc.stderr
-    lib = ctypes.CDLL(so)
+    lib = shared("emu_ltv_fir_fft.cpp", tmp_path_factory)
     fp = ctypes.POINTER(ctypes.c_float)
-    lib.emu_ltv_fir_fft_spec.argtypes = [fp, fp, ctypes.c_int, fp, fp, fp, ctypes.c_int, fp, fp, ctypes.c_ulonglong,
-                                         ctypes.c_longlong, ctypes.c_int, ctypes.c_int, ctypes.c_int, fp, fp]
-    lib.emu_ltv_fir_fft_spec.restype = ctypes.c_int
 
     def run(x1, ir1, x2, ir2, hops=32, seed=0, utt_off=0):
         B, nF, L1 = ir1.shape

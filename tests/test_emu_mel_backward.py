@@ -3,9 +3,6 @@ gradients (tests/golden/mel_grad_*.npz) and the float64 restatement, race-checke
 argument checks of its C ABI entry (no device touched).  The kernel itself runs on hardware in
 tests/test_gpu_mel_backward.py."""
 import ctypes
-import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -15,34 +12,22 @@ from ddsp_svc_b200 import _lib
 from ddsp_svc_b200 import mel as pm
 from tests import mel_grad_closed_form as CF
 from tests import util
+from tests.emu_harness import abi_call, assert_race_free, shared, tsan
 from tests.golden import make_golden_mel_grad as GG
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 f32 = np.float32
 # error model (see tests/test_gpu_mel_backward.py): the kernel's relative RMS error against float64 is at most RATIO
 # times the fp32 reference's own error on the same case (emulated: 1.0 .. 1.6x)
 RATIO = 3.0
 
-needs_gxx = pytest.mark.skipif(shutil.which("g++") is None, reason="g++ not available")
-
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = str(tmp_path_factory.mktemp("emu") / "libemu_mel_bwd.so")
-    cmd = ["g++", "-std=c++20", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-pthread", "-Wno-unknown-pragmas",
-           "-o", so, os.path.join(HERE, "emu", "emu_mel_bwd.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    assert proc.returncode == 0, proc.stderr
-    lib = ctypes.CDLL(so)
-    vp = ctypes.c_void_p
-    lib.emu_mel_bwd.argtypes = [vp] * 6 + [ctypes.c_longlong] * 3 + [ctypes.c_int] * 4 + [ctypes.c_float, ctypes.c_int, vp]
-    lib.emu_mel_fwd.argtypes = [vp] * 4 + [ctypes.c_int] * 4 + [ctypes.c_float, vp]
+    lib = shared("emu_mel_bwd.cpp", tmp_path_factory)
     basis = pm.mel_filterbank(44100, 2048, 128, 40, 16000)
     tabs = dict(basis=basis, lohi=pm._support(basis), bins=pm._bin_filters(basis),
                 window=torch.hann_window(2048).numpy())
-    ptr = lambda a: a.ctypes.data_as(vp)
+    ptr = lambda a: a.ctypes.data_as(ctypes.c_void_p)
 
     class Emu:
         def backward(self, y, hop, g, chunk):
@@ -96,19 +81,8 @@ def test_forward_kernel_source_matches_reference_mel(emu):
     assert np.abs(got.astype(np.float64) - z["mel"]).max() < 2e-3
 
 
-@needs_gxx
 def test_backward_kernel_source_has_no_shared_memory_race(tmp_path):
-    exe = str(tmp_path / "tsan_mel_bwd")
-    cmd = ["g++", "-std=c++20", "-O1", "-g", "-fsanitize=thread", "-pthread", "-Wno-unknown-pragmas", "-o", exe,
-           os.path.join(HERE, "emu", "tsan_mel_bwd.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    if proc.returncode != 0 and "tsan" in proc.stderr.lower():
-        pytest.skip("ThreadSanitizer runtime not available: " + proc.stderr.strip().splitlines()[-1])
-    assert proc.returncode == 0, proc.stderr
-    res = subprocess.run([exe], capture_output=True, text=True, timeout=600,
-                         env=dict(os.environ, TSAN_OPTIONS="halt_on_error=0 exitcode=66"))
-    assert "ThreadSanitizer" not in res.stderr, res.stderr[-4000:]
-    assert res.returncode == 0 and "done" in res.stdout
+    assert_race_free(tsan("tsan_mel_bwd.cpp", tmp_path))
 
 
 def test_bin_filter_ranges_cover_every_weight():
@@ -125,17 +99,13 @@ def test_bin_filter_ranges_cover_every_weight():
 def test_backward_abi_argument_errors_do_not_touch_the_device():
     _lib.build()
     L = _lib.lib()
-    f = L.b2d_mel_spectrogram_backward
-    ok = dict(y=16, w=16, basis=16, lohi=16, bins=16, B=1, T=8192, n_fft=2048, win=2048, hop=512, n_mels=128, clip=1e-5,
-              g=16, sb=0, sm=16, sf=1, out=16, stream=0)
-
-    def call(**kw):
-        a = dict(ok, **kw)
-        return f(a["y"], a["w"], a["basis"], a["lohi"], a["bins"], a["B"], a["T"], a["n_fft"], a["win"], a["hop"],
-                 a["n_mels"], a["clip"], a["g"], a["sb"], a["sm"], a["sf"], a["out"], a["stream"])
-
-    assert call(y=0) == -1 and call(bins=0) == -1 and call(g=0) == -1 and call(out=0) == -1     # B2D_ERR_NULL
-    assert call(B=0) == -2 and call(B=70000) == -2 and call(T=0) == -2 and call(hop=4096) == -2     # B2D_ERR_SHAPE
-    assert call(n_mels=129) == -2 and call(sf=-1) == -2 and call(sm=-128) == -2
-    assert call(n_fft=1024, win=1024) == -4                    # B2D_ERR_UNSUPPORTED: keyshift != 0
+    ok = dict(audio=16, window=16, mel_basis=16, filter_lohi=16, bin_filter_range=16, B=1, n_samples=8192, n_fft=2048,
+              win_size=2048, hop=512, n_mels=128, clip_val=1e-5, grad_mel=16, grad_stride_b=0, grad_stride_mel=16,
+              grad_stride_frame=1, grad_audio=16, stream=0)
+    call = lambda **kw: abi_call("b2d_mel_spectrogram_backward", dict(ok, **kw))
+    assert call(audio=0) == -1 and call(bin_filter_range=0) == -1 and call(grad_mel=0) == -1             # B2D_ERR_NULL
+    assert call(grad_audio=0) == -1
+    assert call(B=0) == -2 and call(B=70000) == -2 and call(n_samples=0) == -2 and call(hop=4096) == -2    # B2D_ERR_SHAPE
+    assert call(n_mels=129) == -2 and call(grad_stride_frame=-1) == -2 and call(grad_stride_mel=-128) == -2
+    assert call(n_fft=1024, win_size=1024) == -4               # B2D_ERR_UNSUPPORTED: keyshift != 0
     assert b"mel_spectrogram_backward" in L.b2d_last_error()

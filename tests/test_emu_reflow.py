@@ -1,37 +1,17 @@
 """csrc/reflow.cu's kernel source (start, layer epilogue, ODE update, finish of the rectified-flow sampler) executed on
 the CPU (tests/emu/host_emu.h) against float64 restatements, race-checked under ThreadSanitizer, plus the argument
 checks of the new C ABI entries (no device touched).  The kernels run on hardware in tests/test_gpu_reflow.py."""
-import ctypes
-import os
-import shutil
-import subprocess
-
 import numpy as np
 import pytest
 import torch
 
 from ddsp_svc_b200 import _lib
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-needs_gxx = pytest.mark.skipif(shutil.which("g++") is None, reason="g++ not available")
+from tests.emu_harness import abi_call, assert_race_free, shared, tsan
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = str(tmp_path_factory.mktemp("emu") / "libemu_reflow.so")
-    cmd = ["g++", "-std=c++20", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-pthread", "-Wno-unknown-pragmas",
-           "-o", so, os.path.join(HERE, "emu", "emu_reflow.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    assert proc.returncode == 0, proc.stderr
-    lib = ctypes.CDLL(so)
-    p, i, f = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
-    lib.emu_rf_start.argtypes = [p, p, f, f, f, f, i, i, i, p, p, p]
-    lib.emu_rf_layer_input.argtypes = [p, p, p, i, p, i, p, i, i, i, i, p, p]
-    lib.emu_rf_ode.argtypes = [p, p, p, p, i, f, i, i, p, p]
-    lib.emu_rf_finish.argtypes = [p, f, f, i, p]
-    return lib
+    return shared("emu_reflow.cpp", tmp_path_factory)
 
 
 def f32(a):
@@ -138,19 +118,8 @@ def test_finish_kernel(emu):
     assert np.abs(out - want).max() <= 1e-6 * np.abs(want).max()
 
 
-@needs_gxx
 def test_reflow_kernel_source_has_no_race(tmp_path):
-    exe = str(tmp_path / "tsan_reflow")
-    cmd = ["g++", "-std=c++20", "-O1", "-g", "-fsanitize=thread", "-pthread", "-Wno-unknown-pragmas", "-o", exe,
-           os.path.join(HERE, "emu", "tsan_reflow.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    if proc.returncode != 0 and "tsan" in proc.stderr.lower():
-        pytest.skip("ThreadSanitizer runtime not available: " + proc.stderr.strip().splitlines()[-1])
-    assert proc.returncode == 0, proc.stderr
-    res = subprocess.run([exe], capture_output=True, text=True, timeout=600,
-                         env=dict(os.environ, TSAN_OPTIONS="halt_on_error=0 exitcode=66"))
-    assert "ThreadSanitizer" not in res.stderr, res.stderr[-4000:]
-    assert res.returncode == 0 and "done" in res.stdout
+    assert_race_free(tsan("tsan_reflow.cpp", tmp_path))
 
 
 def test_reflow_abi_argument_errors_do_not_touch_the_device():
@@ -160,14 +129,15 @@ def test_reflow_abi_argument_errors_do_not_touch_the_device():
     assert L.b2d_rf_start(0, 0, 0.0, 1.0, -12.0, 14.0, 1, 8, 128, 0, p, 0, 0) == -1
     assert L.b2d_rf_start(p, 0, 0.0, 1.0, -12.0, 14.0, 1, 8, 128, 0, 0, 0, 0) == -1
     assert L.b2d_rf_start(p, 0, 0.0, 1.0, -12.0, 14.0, 1, 0, 128, 0, p, 0, 0) == -2
-    li = lambda **kw: L.b2d_rf_layer_input(*[{**dict(g=p, b=p, h=p, r=0, s=p, ss=0, c=p, cs=1536, B=1, T=8, D=512, hi=p, lo=0,
-                                                     st=0), **kw}[k]
-                                             for k in ("g", "b", "h", "r", "s", "ss", "c", "cs", "B", "T", "D", "hi", "lo", "st")])
-    assert li(g=0) == -1 and li(hi=0) == -1 and li(c=0) == -1 and li(s=0) == -1       # step and cond come together
-    assert li(B=0) == -2 and li(ss=100) == -2 and li(cs=256) == -2
-    assert li(D=510, cs=1530) == -3 and li(g=p + 4) == -3 and li(s=p + 4) == -3 and li(cs=1538) == -3
+    ok_li = dict(g=p, bias=p, h=p, residual=0, step=p, step_stride=0, cond=p, cond_stride=1536, B=1, T=8, D=512, hi=p,
+                 lo=0, stream=0)
+    li = lambda **kw: abi_call("b2d_rf_layer_input", dict(ok_li, **kw))
+    assert li(g=0) == -1 and li(hi=0) == -1 and li(cond=0) == -1 and li(step=0) == -1   # step and cond come together
+    assert li(B=0) == -2 and li(step_stride=100) == -2 and li(cond_stride=256) == -2
+    assert li(D=510, cond_stride=1530) == -3 and li(g=p + 4) == -3 and li(step=p + 4) == -3
+    assert li(cond_stride=1538) == -3
     assert b"rf_layer_input" in L.b2d_last_error()
-    ode = lambda **kw: L.b2d_rf_ode_update(*[{**dict(g=p, b=p, x=p, a=p, s=0, dt=0.1, n=8, M=128, hi=p, lo=0, st=0), **kw}[k]
-                                             for k in ("g", "b", "x", "a", "s", "dt", "n", "M", "hi", "lo", "st")])
-    assert ode(a=0) == -1 and ode(x=0) == -1 and ode(n=0) == -2 and ode(s=4) == -4 and ode(s=-2) == -4
+    ok_ode = dict(g=p, bias=p, x=p, acc=p, stage=0, dt=0.1, n_tokens=8, M=128, hi=p, lo=0, stream=0)
+    ode = lambda **kw: abi_call("b2d_rf_ode_update", dict(ok_ode, **kw))
+    assert ode(acc=0) == -1 and ode(x=0) == -1 and ode(n_tokens=0) == -2 and ode(stage=4) == -4 and ode(stage=-2) == -4
     assert L.b2d_rf_finish(0, -12.0, 14.0, 8, p, 0) == -1 and L.b2d_rf_finish(p, -12.0, 14.0, 0, p, 0) == -2

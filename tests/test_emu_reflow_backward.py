@@ -3,39 +3,19 @@ on the CPU (tests/emu/host_emu.h) against float64 restatements, on several grids
 the argument checks of the new C ABI entries (no device touched).  The kernels run on hardware in
 tests/test_gpu_reflow_backward.py.  They use no shared memory and no barrier, so no ThreadSanitizer driver is needed:
 every output element has one owner thread, which the grid-independence checks exercise."""
-import ctypes
-import os
-import shutil
-import subprocess
-
 import numpy as np
 import pytest
 import torch
 
 from ddsp_svc_b200 import _lib
+from tests.emu_harness import abi_call, shared
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 GRIDS = [(1, 32), (3, 32), (7, 64)]                # (CTAs, threads per CTA)
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = str(tmp_path_factory.mktemp("emu") / "libemu_reflow_bwd.so")
-    cmd = ["g++", "-std=c++20", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-pthread", "-Wno-unknown-pragmas",
-           "-o", so, os.path.join(HERE, "emu", "emu_reflow_bwd.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    assert proc.returncode == 0, proc.stderr
-    lib = ctypes.CDLL(so)
-    p, i, f, u = ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_uint
-    lib.emu_rf_loss_input.argtypes = [u, u, p, p, p, f, f, i, i, i, p, p, p]
-    lib.emu_rf_loss.argtypes = [u, u, p, p, p, p, i, i, i, p, p, p]
-    lib.emu_rf_loss_backward.argtypes = [u, u, p, p, p, p, p, i, i, i, p, p, p]
-    lib.emu_rf_gelu_backward.argtypes = [u, u, p, p, p, i, i, p, p, p]
-    lib.emu_rf_layer_backward.argtypes = [u, u, p, p, i, i, i, i, i, p, p, p, p, p, p]
-    lib.emu_rf_step_sums.argtypes = [u, u, p, i, i, i, p]
-    return lib
+    return shared("emu_reflow_bwd.cpp", tmp_path_factory)
 
 
 def f32(a):
@@ -215,29 +195,27 @@ def test_reflow_backward_abi_argument_errors_do_not_touch_the_device():
     assert L.b2d_rf_backward_workspace_bytes(0, 8, 128) == 0 and L.b2d_rf_backward_workspace_bytes(2, 8, 0) == 0
     ws_n = L.b2d_rf_backward_workspace_bytes(2, 40, 128)
     assert ws_n >= 2 * 2 * 128 * 8 + 128 * 8
-    li = lambda **kw: L.b2d_rf_loss_input(*[{**dict(gt=p, x0=p, t=p, smin=-12.0, rng=14.0, B=2, T=40, M=128, tg=p, hi=p, lo=0,
-                                                    st=0), **kw}[k]
-                                            for k in ("gt", "x0", "t", "smin", "rng", "B", "T", "M", "tg", "hi", "lo", "st")])
-    assert li(gt=0) == -1 and li(t=0) == -1 and li(hi=0) == -1 and li(tg=0) == -1 and li(B=0) == -2 and li(M=-1) == -2
-    lo = lambda **kw: L.b2d_rf_loss(*[{**dict(g=p, b=p, tg=p, w=p, B=2, T=40, M=128, ws=p, n=ws_n, out=p, st=0), **kw}[k]
-                                      for k in ("g", "b", "tg", "w", "B", "T", "M", "ws", "n", "out", "st")])
-    assert lo(w=0) == -1 and lo(ws=0) == -1 and lo(out=0) == -1 and lo(T=0) == -2 and lo(n=ws_n - 8) == -5 and lo(T=80) == -5
-    lb = lambda **kw: L.b2d_rf_loss_backward(*[{**dict(g=p, b=p, tg=p, w=p, gl=p, B=2, T=40, M=128, gv=p, hi=0, lo=0, st=0),
-                                                **kw}[k]
-                                               for k in ("g", "b", "tg", "w", "gl", "B", "T", "M", "gv", "hi", "lo", "st")])
-    assert lb(gl=0) == -1 and lb(gv=0) == -1 and lb(lo=p) == -1 and lb(B=0) == -2
-    gb = lambda **kw: L.b2d_rf_gelu_backward(*[{**dict(gy=p, pre=p, b=0, n=8, C=512, gx=p, hi=0, lo=0, st=0), **kw}[k]
-                                               for k in ("gy", "pre", "b", "n", "C", "gx", "hi", "lo", "st")])
-    assert gb(gy=0) == -1 and gb(gx=0) == -1 and gb(lo=p) == -1 and gb(n=0) == -2 and gb(C=0) == -2
+    ok_li = dict(gt=p, x0=p, t=p, spec_min=-12.0, spec_range=14.0, B=2, T=40, M=128, target=p, hi=p, lo=0, stream=0)
+    li = lambda **kw: abi_call("b2d_rf_loss_input", dict(ok_li, **kw))
+    assert li(gt=0) == -1 and li(t=0) == -1 and li(hi=0) == -1 and li(target=0) == -1 and li(B=0) == -2 and li(M=-1) == -2
+    ok_loss = dict(g=p, bias=p, target=p, w=p, B=2, T=40, M=128, ws=p, ws_bytes=ws_n, loss=p, stream=0)
+    loss = lambda **kw: abi_call("b2d_rf_loss", dict(ok_loss, **kw))
+    assert loss(w=0) == -1 and loss(ws=0) == -1 and loss(loss=0) == -1 and loss(T=0) == -2
+    assert loss(ws_bytes=ws_n - 8) == -5 and loss(T=80) == -5
+    ok_lb = dict(g=p, bias=p, target=p, w=p, g_loss=p, B=2, T=40, M=128, gv=p, hi=0, lo=0, stream=0)
+    lb = lambda **kw: abi_call("b2d_rf_loss_backward", dict(ok_lb, **kw))
+    assert lb(g_loss=0) == -1 and lb(gv=0) == -1 and lb(lo=p) == -1 and lb(B=0) == -2
+    ok_gb = dict(gy=p, pre=p, bias=0, n_rows=8, C=512, gx=p, hi=0, lo=0, stream=0)
+    gb = lambda **kw: abi_call("b2d_rf_gelu_backward", dict(ok_gb, **kw))
+    assert gb(gy=0) == -1 and gb(gx=0) == -1 and gb(lo=p) == -1 and gb(n_rows=0) == -2 and gb(C=0) == -2
     lay_n = L.b2d_rf_backward_workspace_bytes(2, 40, 3 * 128)
-    ly = lambda **kw: L.b2d_rf_layer_backward(*[{**dict(gz=p, gh=p, B=2, T=40, D=128, i=0, nL=3, hh=0, hl=0, z=p, zh=0, zl=0,
-                                                         ws=p, n=lay_n, st=0), **kw}[k]
-                                                for k in ("gz", "gh", "B", "T", "D", "i", "nL", "hh", "hl", "z", "zh", "zl", "ws",
-                                                          "n", "st")])
-    assert ly(gz=0) == -1 and ly(z=0) == -1 and ly(ws=0) == -1 and ly(hl=p) == -1 and ly(zl=p) == -1
-    assert ly(i=3) == -2 and ly(i=-1) == -2 and ly(nL=0) == -2 and ly(D=0) == -2
-    assert ly(n=lay_n // 2) == -5 and ly(T=200) == -5
-    ss = lambda **kw: L.b2d_rf_step_sums(*[{**dict(ws=p, n=lay_n, B=2, T=40, c=384, out=p, st=0), **kw}[k]
-                                           for k in ("ws", "n", "B", "T", "c", "out", "st")])
-    assert ss(ws=0) == -1 and ss(out=0) == -1 and ss(c=0) == -2 and ss(c=768) == -5
+    ok_ly = dict(gz=p, gh=p, B=2, T=40, D=128, layer=0, n_layers=3, gh_hi=0, gh_lo=0, z=p, z_hi=0, z_lo=0, ws=p,
+                 ws_bytes=lay_n, stream=0)
+    ly = lambda **kw: abi_call("b2d_rf_layer_backward", dict(ok_ly, **kw))
+    assert ly(gz=0) == -1 and ly(z=0) == -1 and ly(ws=0) == -1 and ly(gh_lo=p) == -1 and ly(z_lo=p) == -1
+    assert ly(layer=3) == -2 and ly(layer=-1) == -2 and ly(n_layers=0) == -2 and ly(D=0) == -2
+    assert ly(ws_bytes=lay_n // 2) == -5 and ly(T=200) == -5
+    ok_ss = dict(ws=p, ws_bytes=lay_n, B=2, T=40, cols=384, out=p, stream=0)
+    ss = lambda **kw: abi_call("b2d_rf_step_sums", dict(ok_ss, **kw))
+    assert ss(ws=0) == -1 and ss(out=0) == -1 and ss(cols=0) == -2 and ss(cols=768) == -5
     assert b"rf_step_sums" in L.b2d_last_error()

@@ -2,9 +2,6 @@
 (tests/golden/rss_*.npz) and the float64 restatement, race-checked under ThreadSanitizer, plus the argument checks of
 the C ABI entries (no device touched).  The kernels themselves run on hardware in tests/test_gpu_rss_loss.py."""
 import ctypes
-import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -13,34 +10,20 @@ from ddsp_svc_b200 import _lib
 from ddsp_svc_b200 import loss as pl
 from tests import rss_loss_closed_form as CF
 from tests import report, util
+from tests.emu_harness import abi_call, assert_race_free, shared, tsan
 from tests.golden import make_golden_rss_loss as GR
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 f32 = np.float32
 # error model (see tests/test_gpu_rss_loss.py): against float64 the loss (relative) and the gradient (relative RMS) stay
 # within RATIO times the fp32 reference's own error on the same case (the loss floor: at least one fp32 ulp)
 RATIO = 3.0
 
-needs_gxx = pytest.mark.skipif(shutil.which("g++") is None, reason="g++ not available")
-
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
+    lib = shared("emu_rss_loss.cpp", tmp_path_factory)
     _lib.build()
-    so = str(tmp_path_factory.mktemp("emu") / "libemu_rss_loss.so")
-    cmd = ["g++", "-std=c++20", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-pthread", "-Wno-unknown-pragmas",
-           "-o", so, os.path.join(HERE, "emu", "emu_rss_loss.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    assert proc.returncode == 0, proc.stderr
-    lib = ctypes.CDLL(so)
-    vp, ci, cf = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
-    lib.emu_rss_workspace_doubles.restype = ctypes.c_longlong
-    lib.emu_rss_workspace_doubles.argtypes = [ci, ci, ci, vp]
-    lib.emu_rss_forward.argtypes = [vp, vp, ci, ci, ci, vp, vp, cf, cf, vp, vp, vp]
-    lib.emu_rss_backward.argtypes = [vp, vp, ci, ci, ci, vp, vp, cf, cf, vp, vp, vp]
-    lib.emu_rss_spectra.argtypes = [vp, vp, ci, ci, ci, vp, cf, vp, vp]
+    vp, ci = ctypes.c_void_p, ctypes.c_int
     ptr = lambda a: a.ctypes.data_as(vp)
 
     class Emu:
@@ -155,19 +138,8 @@ def test_scale_order_changes_only_the_summation(emu):
     assert util.rms(g1 - g2) <= 1e-6 * util.rms(g1)
 
 
-@needs_gxx
 def test_kernel_source_has_no_shared_memory_race(tmp_path):
-    exe = str(tmp_path / "tsan_rss_loss")
-    cmd = ["g++", "-std=c++20", "-O1", "-g", "-fsanitize=thread", "-pthread", "-Wno-unknown-pragmas", "-o", exe,
-           os.path.join(HERE, "emu", "tsan_rss_loss.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    if proc.returncode != 0 and "tsan" in proc.stderr.lower():
-        pytest.skip("ThreadSanitizer runtime not available: " + proc.stderr.strip().splitlines()[-1])
-    assert proc.returncode == 0, proc.stderr
-    res = subprocess.run([exe], capture_output=True, text=True, timeout=900,
-                         env=dict(os.environ, TSAN_OPTIONS="halt_on_error=0 exitcode=66"))
-    assert "ThreadSanitizer" not in res.stderr, res.stderr[-4000:]
-    assert res.returncode == 0 and "done" in res.stdout
+    assert_race_free(tsan("tsan_rss_loss.cpp", tmp_path))
 
 
 def test_table_layout_and_bluestein_sizes():
@@ -192,24 +164,18 @@ def test_abi_argument_errors_do_not_touch_the_device():
     ns = (ctypes.c_int * 2)(512, 1031)
     tabs = (ctypes.c_void_p * 2)(256, 512)
     bad_n = (ctypes.c_int * 1)(2048)
-    ok = dict(xp=16, xt=16, B=2, T=8192, ns_count=2, ns=ns, tabs=tabs, ws=16, wsb=1 << 20, norms=16, loss=16)
-
-    def fwd(**kw):
-        a = dict(ok, **kw)
-        return L.b2d_rss_loss_forward(a["xp"], a["xt"], a["B"], a["T"], a["ns_count"], a["ns"], a["tabs"], 1.0, 1e-7,
-                                      a["ws"], a["wsb"], a["norms"], a["loss"], 0)
-
-    def bwd(**kw):
-        a = dict(ok, **kw)
-        return L.b2d_rss_loss_backward(a["xp"], a["xt"], a["B"], a["T"], a["ns_count"], a["ns"], a["tabs"], 1.0, 1e-7,
-                                       a["norms"], a["loss"], a["ws"], 0)
-
-    for f in (fwd, bwd):
-        assert f(xp=0) == -1 and f(xt=0) == -1 and f(norms=0) == -1 and f(loss=0) == -1      # B2D_ERR_NULL
-        assert f(tabs=(ctypes.c_void_p * 2)(256, 0)) == -1
-        assert f(xp=18) == -3 and f(norms=20) == -3 and f(tabs=(ctypes.c_void_p * 2)(256, 260)) == -3   # B2D_ERR_ALIGN
-        assert f(B=0) == -2 and f(B=70000) == -2 and f(T=1000) == -2 and f(ns_count=65) == -2  # B2D_ERR_SHAPE
-        assert f(ns=bad_n, ns_count=1) == -4 and f(ns=(ctypes.c_int * 1)(255), ns_count=1) == -4  # B2D_ERR_UNSUPPORTED
-    assert fwd(wsb=8) == -5                                                                    # B2D_ERR_WORKSPACE
+    common = dict(x_pred=16, x_true=16, B=2, n_samples=8192, n_scale=2, n_ffts=ns, tables=tabs, alpha=1.0, eps=1e-7,
+                  norms=16, stream=0)
+    ok_fwd = dict(common, workspace=16, workspace_bytes=1 << 20, loss=16)
+    ok_bwd = dict(common, grad_loss=16, grad_pred=16)
+    fwd = lambda **kw: abi_call("b2d_rss_loss_forward", dict(ok_fwd, **kw))
+    bwd = lambda **kw: abi_call("b2d_rss_loss_backward", dict(ok_bwd, **kw))
+    for f, scalar in ((fwd, "loss"), (bwd, "grad_loss")):       # the loss, or the cotangent of the loss
+        assert f(x_pred=0) == -1 and f(x_true=0) == -1 and f(norms=0) == -1 and f(**{scalar: 0}) == -1   # B2D_ERR_NULL
+        assert f(tables=(ctypes.c_void_p * 2)(256, 0)) == -1
+        assert f(x_pred=18) == -3 and f(norms=20) == -3 and f(tables=(ctypes.c_void_p * 2)(256, 260)) == -3   # ALIGN
+        assert f(B=0) == -2 and f(B=70000) == -2 and f(n_samples=1000) == -2 and f(n_scale=65) == -2   # B2D_ERR_SHAPE
+        assert f(n_ffts=bad_n, n_scale=1) == -4 and f(n_ffts=(ctypes.c_int * 1)(255), n_scale=1) == -4  # UNSUPPORTED
+    assert fwd(workspace_bytes=8) == -5                                                        # B2D_ERR_WORKSPACE
     assert b"rss_loss" in L.b2d_last_error()
     assert L.b2d_rss_loss_workspace_bytes(2, 8192, 2, ns) == 8 * 3 * 2 * (16 + 7)

@@ -5,9 +5,6 @@ its C ABI entry (no device touched).  The kernels run on hardware in tests/test_
 The emulated kernels are fed the port's fp32 forward quantities (sinusoids, impulse responses: the reference's own
 values) and the phase scan's float64 frame phase."""
 import ctypes
-import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -16,14 +13,12 @@ from ddsp_svc_b200 import _lib
 from oracle import torch_port as tp
 from tests import sins_grad_closed_form as cfg
 from tests import util
+from tests.emu_harness import abi_call, assert_race_free, shared, tsan
 from tests.golden import make_golden_sins_grad as GG
 from tests.test_oracle_sins_grad import KEYS, error_model, split_grad
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 P, SR = GG.P, GG.SR
 f32 = np.float32
-
-needs_gxx = pytest.mark.skipif(shutil.which("g++") is None, reason="g++ not available")
 
 
 def frame_phase(f0):
@@ -36,17 +31,8 @@ def frame_phase(f0):
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = str(tmp_path_factory.mktemp("emu") / "libemu_sins_bwd.so")
-    cmd = ["g++", "-std=c++20", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-pthread", "-Wno-unknown-pragmas",
-           "-o", so, os.path.join(HERE, "emu", "emu_sins_bwd.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    assert proc.returncode == 0, proc.stderr
-    lib = ctypes.CDLL(so)
+    lib = shared("emu_sins_bwd.cpp", tmp_path_factory)
     fp, dp = ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_double)
-    lib.emu_sins_bwd.argtypes = [fp, dp, fp, fp, fp, ctypes.c_longlong, fp, fp, fp, fp, ctypes.c_ulonglong,
-                                 ctypes.c_longlong, fp, fp, fp] + [ctypes.c_int] * 5 + [ctypes.c_double, fp, fp]
 
     def run(name, inp, noise="explicit", seed=0, utt_off=0, rows=None):
         c = GG.CASES[name]
@@ -107,39 +93,26 @@ def test_in_kernel_noise_rows_are_shard_invariant(emu):
     assert not np.array_equal(full, emu(name, inp, noise="kernel", seed=4))
 
 
-@needs_gxx
 def test_backward_kernel_source_has_no_shared_memory_race(tmp_path):
-    exe = str(tmp_path / "tsan_sins_bwd")
-    cmd = ["g++", "-std=c++20", "-O1", "-g", "-fsanitize=thread", "-pthread", "-Wno-unknown-pragmas", "-o", exe,
-           os.path.join(HERE, "emu", "tsan_sins_bwd.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    if proc.returncode != 0 and "tsan" in proc.stderr.lower():
-        pytest.skip("ThreadSanitizer runtime not available: " + proc.stderr.strip().splitlines()[-1])
-    assert proc.returncode == 0, proc.stderr
-    res = subprocess.run([exe], capture_output=True, text=True, timeout=900,
-                         env=dict(os.environ, TSAN_OPTIONS="halt_on_error=0 exitcode=66"))
-    assert "ThreadSanitizer" not in res.stderr, res.stderr[-4000:]
-    assert res.returncode == 0 and "done" in res.stdout
+    assert_race_free(tsan("tsan_sins_bwd.cpp", tmp_path))
 
 
 def test_backward_abi_argument_errors_do_not_touch_the_device():
     _lib.build()
     L = _lib.lib()
-    f = L.b2d_sins_synth_backward
     ws_need = L.b2d_sins_synth_backward_workspace_bytes(1, 4, 512)
     assert ws_need == 2 * 4 * 512 * 4 and L.b2d_sins_synth_backward_workspace_bytes(0, 4, 512) == 0
-    ok = dict(f0=256, fph=256, ca=256, cg=256, cn=256, stride=640, noise=0, seed=0, off=0, fws=256, has=1, g=256, gh=0,
-              gn=0, B=1, nF=4, block=512, H=128, Ma=256, Mn=256, sr=44100.0, out=256, ws=256, wsb=ws_need, stream=0)
-
-    def call(**kw):
-        a = dict(ok, **kw)
-        return f(a["f0"], a["fph"], a["ca"], a["cg"], a["cn"], a["stride"], a["noise"], a["seed"], a["off"], a["fws"],
-                 a["has"], a["g"], a["gh"], a["gn"], a["B"], a["nF"], a["block"], a["H"], a["Ma"], a["Mn"], a["sr"],
-                 a["out"], a["ws"], a["wsb"], a["stream"])
-
-    assert call(fws=0) == -1 and call(out=0) == -1 and call(ws=0) == -1 and call(cg=0) == -1      # B2D_ERR_NULL
-    assert call(B=0) == -2 and call(nF=0) == -2 and call(stride=200) == -2 and call(Ma=1) == -2    # B2D_ERR_SHAPE
-    assert call(block=1024) == -4 and call(Ma=258, stride=700) == -4 and call(H=513, stride=1100) == -4   # UNSUPPORTED
-    assert call(wsb=ws_need - 1) == -5                                                             # B2D_ERR_WORKSPACE
-    assert call(ws=272) == -3 and call(fws=272) == -3 and call(noise=260) == -3                     # B2D_ERR_ALIGN
+    ok = dict(f0_frames=256, frame_phase=256, c_amp=256, c_group_delay=256, c_noise=256, ctrl_stride=640, noise_in=0,
+              seed=0, utterance_offset=0, forward_workspace=256, forward_has_sinusoids=1, grad_signal=256,
+              grad_harmonic=0, grad_noise=0, B=1, n_frames=4, block=512, n_harmonics=128, n_mag_allpass=256,
+              n_mag_noise=256, sampling_rate=44100.0, grad_ctrl=256, workspace=256, workspace_bytes=ws_need, stream=0)
+    call = lambda **kw: abi_call("b2d_sins_synth_backward", dict(ok, **kw))
+    assert call(forward_workspace=0) == -1 and call(grad_ctrl=0) == -1 and call(workspace=0) == -1     # B2D_ERR_NULL
+    assert call(c_group_delay=0) == -1
+    assert call(B=0) == -2 and call(n_frames=0) == -2 and call(ctrl_stride=200) == -2                  # B2D_ERR_SHAPE
+    assert call(n_mag_allpass=1) == -2
+    assert call(block=1024) == -4 and call(n_mag_allpass=258, ctrl_stride=700) == -4                   # UNSUPPORTED
+    assert call(n_harmonics=513, ctrl_stride=1100) == -4
+    assert call(workspace_bytes=ws_need - 1) == -5                                                     # B2D_ERR_WORKSPACE
+    assert call(workspace=272) == -3 and call(forward_workspace=272) == -3 and call(noise_in=260) == -3  # B2D_ERR_ALIGN
     assert b"sins_synth_backward" in L.b2d_last_error()

@@ -3,9 +3,6 @@ goldens.  The kernel is validated on hardware (tests/test_gpu_superfast.py); the
 the shared FFT code can be checked -- and race-checked under ThreadSanitizer -- without a GPU.  The frame scan (warp
 shuffles) is restated here in numpy with the kernel's fp32 operation order."""
 import ctypes
-import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -14,12 +11,10 @@ from tests import util
 from tests.golden import cases as G
 import torch
 from tests import regimes as R
+from tests.emu_harness import shared
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 SR, P, WIN = G.SR, G.P, 2048
 f32 = np.float32
-
-pytestmark = pytest.mark.skipif(shutil.which("g++") is None, reason="g++ not available")
 
 
 def frame_par(f0):
@@ -41,15 +36,8 @@ def frame_par(f0):
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("emu") / "libemu_sf.so")
-    cmd = ["g++", "-std=c++20", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-pthread", "-Wno-unknown-pragmas",
-           "-o", so, os.path.join(HERE, "emu", "emu_superfast.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    assert proc.returncode == 0, proc.stderr
-    lib = ctypes.CDLL(so)
+    lib = shared("emu_superfast.cpp", tmp_path_factory)
     fp = ctypes.POINTER(ctypes.c_float)
-    lib.emu_superfast.argtypes = [fp, fp, fp, fp, fp, ctypes.c_longlong, fp, ctypes.c_ulonglong, ctypes.c_longlong,
-                                  ctypes.c_int, ctypes.c_int, ctypes.c_int, fp]
 
     def run(f0, dense, noise, hops=29, seed=0, utt_off=0):
         B, nF = f0.shape[0], f0.shape[1]

@@ -2,42 +2,28 @@
 autograd gradients (tests/golden/superfast_grad_*.npz), race-checked under ThreadSanitizer, plus the argument checks
 of its C ABI entry (no device touched).  The kernel itself runs on hardware in tests/test_gpu_superfast_backward.py."""
 import ctypes
-import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
 from ddsp_svc_b200 import _lib
 from tests import util
+from tests.emu_harness import abi_call, assert_race_free, shared, tsan
 from tests.golden import make_golden_superfast_grad as GG
 from tests.test_emu_superfast import frame_par
 from tests import regimes as R
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 P, NB = GG.P, GG.WIN // 2 + 1
 f32 = np.float32
 # per-control relative RMS bounds: the emulated comb source limits the harmonic side (the forward's emulation gate,
 # 2e-7 abs at a signal RMS of ~0.009, is ~2e-5 relative); the noise side involves no comb
 BOUND = {"harmonic_magnitude": 3e-5, "harmonic_phase": 3e-5, "noise_magnitude": 1e-5, "noise_phase": 1e-5}
 
-needs_gxx = pytest.mark.skipif(shutil.which("g++") is None, reason="g++ not available")
-
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = str(tmp_path_factory.mktemp("emu") / "libemu_sf_bwd.so")
-    cmd = ["g++", "-std=c++20", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-pthread", "-Wno-unknown-pragmas",
-           "-o", so, os.path.join(HERE, "emu", "emu_superfast_bwd.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    assert proc.returncode == 0, proc.stderr
-    lib = ctypes.CDLL(so)
+    lib = shared("emu_superfast_bwd.cpp", tmp_path_factory)
     fp = ctypes.POINTER(ctypes.c_float)
-    lib.emu_superfast_bwd.argtypes = [fp, fp, fp, fp, fp, ctypes.c_longlong, fp, ctypes.c_ulonglong, ctypes.c_longlong,
-                                      fp, ctypes.c_int, ctypes.c_int, ctypes.c_int, fp]
 
     def run(f0, dense, noise, g, hops=29, seed=0, utt_off=0):
         B, nF = f0.shape[0], f0.shape[1]
@@ -78,37 +64,23 @@ def test_in_kernel_noise_rows_are_shard_invariant(emu):
     assert not np.array_equal(full, emu(f0, dense, None, g, seed=4))
 
 
-@needs_gxx
 def test_backward_kernel_source_has_no_shared_memory_race(tmp_path):
-    exe = str(tmp_path / "tsan_superfast_bwd")
-    cmd = ["g++", "-std=c++20", "-O1", "-g", "-fsanitize=thread", "-pthread", "-Wno-unknown-pragmas", "-o", exe,
-           os.path.join(HERE, "emu", "tsan_superfast_bwd.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    if proc.returncode != 0 and "tsan" in proc.stderr.lower():
-        pytest.skip("ThreadSanitizer runtime not available: " + proc.stderr.strip().splitlines()[-1])
-    assert proc.returncode == 0, proc.stderr
-    res = subprocess.run([exe], capture_output=True, text=True, timeout=600,
-                         env=dict(os.environ, TSAN_OPTIONS="halt_on_error=0 exitcode=66"))
-    assert "ThreadSanitizer" not in res.stderr, res.stderr[-4000:]
-    assert res.returncode == 0 and "done" in res.stdout
+    assert_race_free(tsan("tsan_superfast_bwd.cpp", tmp_path))
 
 
 def test_backward_abi_argument_errors_do_not_touch_the_device():
     _lib.build()
     L = _lib.lib()
-    f = L.b2d_superfast_synth_backward
-    ok = dict(ws=16, hm=16, hp=16, nm=16, np_=16, stride=4100, noise=0, seed=0, off=0, g=16, B=1, nF=4, block=512,
-              win=2048, out=16, stream=0)
-
-    def call(**kw):
-        a = dict(ok, **kw)
-        return f(a["ws"], a["hm"], a["hp"], a["nm"], a["np_"], a["stride"], a["noise"], a["seed"], a["off"], a["g"],
-                 a["B"], a["nF"], a["block"], a["win"], a["out"], a["stream"])
-
-    assert call(ws=0) == -1 and call(g=0) == -1 and call(out=0) == -1 and call(np_=0) == -1     # B2D_ERR_NULL
-    assert call(B=0) == -2 and call(nF=0) == -2 and call(stride=1024) == -2                    # B2D_ERR_SHAPE
-    assert call(win=1024, stride=513) == -4 and call(block=256) == -4 and call(B=70000) == -4  # B2D_ERR_UNSUPPORTED
-    assert call(g=20) == -3 and call(out=20) == -3 and call(noise=20) == -3 and call(ws=8) == -3   # B2D_ERR_ALIGN
+    ok = dict(workspace=16, c_hm=16, c_hp=16, c_nm=16, c_np=16, ctrl_stride=4100, noise_in=0, seed=0, utterance_offset=0,
+              grad_signal=16, B=1, n_frames=4, block=512, win_length=2048, grad_ctrl=16, stream=0)
+    call = lambda **kw: abi_call("b2d_superfast_synth_backward", dict(ok, **kw))
+    assert call(workspace=0) == -1 and call(grad_signal=0) == -1 and call(grad_ctrl=0) == -1            # B2D_ERR_NULL
+    assert call(c_np=0) == -1
+    assert call(B=0) == -2 and call(n_frames=0) == -2 and call(ctrl_stride=1024) == -2                 # B2D_ERR_SHAPE
+    assert call(win_length=1024, ctrl_stride=513) == -4 and call(block=256) == -4                      # UNSUPPORTED
+    assert call(B=70000) == -4
+    assert call(grad_signal=20) == -3 and call(grad_ctrl=20) == -3 and call(noise_in=20) == -3         # B2D_ERR_ALIGN
+    assert call(workspace=8) == -3
     assert b"superfast_synth_backward" in L.b2d_last_error()
 
 

@@ -2,45 +2,17 @@
 (tests/emu/host_emu.h, one std::thread per CUDA thread, __syncthreads = std::barrier) under ThreadSanitizer.  A missing
 or misplaced __syncthreads around shared memory is a data race between those threads and gets reported; the `racy`
 control kernel proves the detector sees through the emulated barrier in both directions."""
-import os
-import shutil
-import subprocess
-
 import pytest
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-pytestmark = pytest.mark.skipif(shutil.which("g++") is None, reason="g++ not available")
-
-
-def _build(tmp, name, define):
-    exe = str(tmp / name)
-    cmd = ["g++", "-std=c++20", "-O1", "-g", "-fsanitize=thread", "-pthread", "-Wno-unknown-pragmas"]
-    if define:
-        cmd.append("-D" + define)
-    cmd += ["-o", exe, os.path.join(HERE, "emu", "tsan_main.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    if proc.returncode != 0 and "tsan" in proc.stderr.lower():
-        pytest.skip("ThreadSanitizer runtime not available: " + proc.stderr.strip().splitlines()[-1])
-    assert proc.returncode == 0, proc.stderr
-    return exe
-
-
-def _run(exe, *args):
-    env = dict(os.environ, TSAN_OPTIONS="halt_on_error=0 exitcode=66")
-    return subprocess.run([exe, *args], capture_output=True, text=True, timeout=600, env=env)
+from tests.emu_harness import assert_race_free, tsan
 
 
 def test_detector_sees_a_missing_barrier_and_accepts_a_correct_one(tmp_path):
-    exe = _build(tmp_path, "racy", None)
-    bad = _run(exe, "racy")
+    bad = tsan("tsan_main.cpp", tmp_path, None, "racy")
     assert "ThreadSanitizer: data race" in bad.stderr and bad.returncode == 66
-    good = _run(exe, "ok")
-    assert "ThreadSanitizer" not in good.stderr and good.returncode == 0, good.stderr[-2000:]
+    assert_race_free(tsan("tsan_main.cpp", tmp_path, None, "ok"))
 
 
 @pytest.mark.parametrize("define", ["TSAN_FIRFFT", "TSAN_CSFAST", "TSAN_SUPERFAST", "TSAN_LINATTN"])
 def test_kernel_source_has_no_shared_memory_race(tmp_path, define):
-    exe = _build(tmp_path, define.lower(), define)
-    res = _run(exe)
-    assert "ThreadSanitizer" not in res.stderr, res.stderr[-4000:]
-    assert res.returncode == 0 and "done" in res.stdout
+    assert_race_free(tsan("tsan_main.cpp", tmp_path, define))

@@ -3,9 +3,6 @@
 checks of the new C ABI entries (no device touched).  The kernels run on hardware in
 tests/test_gpu_unit2control_backward.py."""
 import ctypes
-import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -14,9 +11,7 @@ import torch.nn.functional as F
 
 from ddsp_svc_b200 import _lib
 from tests import util
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-needs_gxx = pytest.mark.skipif(shutil.which("g++") is None, reason="g++ not available")
+from tests.emu_harness import abi_call, assert_race_free, shared, tsan
 
 
 def glu_dwconv_silu_reference(h, w, bias, gout):
@@ -32,16 +27,8 @@ def glu_dwconv_silu_reference(h, w, bias, gout):
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = str(tmp_path_factory.mktemp("emu") / "libemu_u2c_glu_bwd.so")
-    cmd = ["g++", "-std=c++20", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-pthread", "-Wno-unknown-pragmas",
-           "-o", so, os.path.join(HERE, "emu", "emu_u2c_glu_bwd.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    assert proc.returncode == 0, proc.stderr
-    lib = ctypes.CDLL(so)
+    lib = shared("emu_u2c_glu_bwd.cpp", tmp_path_factory)
     fp = ctypes.POINTER(ctypes.c_float)
-    lib.emu_u2c_glu_bwd.argtypes = [fp] * 6 + [ctypes.c_int] * 3
 
     def run(h, w, bias, gout):
         B, T, Ci = gout.shape
@@ -68,19 +55,8 @@ def test_glu_backward_kernel_source_matches_float64_autograd(emu, B, T, Ci):
     assert (gh - want_gh).abs().max() <= 2e-5 * want_gh.abs().max()
 
 
-@needs_gxx
 def test_glu_backward_kernel_source_has_no_shared_memory_race(tmp_path):
-    exe = str(tmp_path / "tsan_u2c_glu_bwd")
-    cmd = ["g++", "-std=c++20", "-O1", "-g", "-fsanitize=thread", "-pthread", "-Wno-unknown-pragmas", "-o", exe,
-           os.path.join(HERE, "emu", "tsan_u2c_glu_bwd.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    if proc.returncode != 0 and "tsan" in proc.stderr.lower():
-        pytest.skip("ThreadSanitizer runtime not available: " + proc.stderr.strip().splitlines()[-1])
-    assert proc.returncode == 0, proc.stderr
-    res = subprocess.run([exe], capture_output=True, text=True, timeout=600,
-                         env=dict(os.environ, TSAN_OPTIONS="halt_on_error=0 exitcode=66"))
-    assert "ThreadSanitizer" not in res.stderr, res.stderr[-4000:]
-    assert res.returncode == 0 and "done" in res.stdout
+    assert_race_free(tsan("tsan_u2c_glu_bwd.cpp", tmp_path))
 
 
 def test_backward_abi_argument_errors_do_not_touch_the_device():
@@ -90,20 +66,22 @@ def test_backward_abi_argument_errors_do_not_touch_the_device():
     assert L.b2d_u2c_backward_workspace_bytes(0, 8, 512, 4100) == 0 and L.b2d_u2c_backward_workspace_bytes(2, 8, 512, 0) == 0
     # 24 x 172: the depthwise partials (24 utterances x 3 tiles x 512 channels x 32) outweigh the column-sum slabs
     assert L.b2d_u2c_backward_workspace_bytes(24, 172, 512, 4100) == max(24 * 3 * 512 * 32 * 4, 33 * 4100 * 4)
-    glu = lambda **kw: L.b2d_u2c_glu_dwconv_silu_backward(*[{**dict(h=p, w=p, b=p, g=p, gh=p, dwb=p, B=1, T=8, Ci=256, K=31,
-                                                                  ws=p, n=big, s=0), **kw}[k]
-                                                            for k in ("h", "w", "b", "g", "gh", "dwb", "B", "T", "Ci", "K", "ws", "n", "s")])
+    ok_glu = dict(h=p, weight=p, bias=p, gout=p, gh=p, dwb=p, B=1, T=8, inner_channels=256, kernel_size=31, ws=p,
+                  ws_bytes=big, stream=0)
+    glu = lambda **kw: abi_call("b2d_u2c_glu_dwconv_silu_backward", dict(ok_glu, **kw))
     assert glu(h=0) == -1 and glu(dwb=0) == -1 and glu(ws=0) == -1
-    assert glu(K=29) == -2 and glu(Ci=100) == -2 and glu(B=65536) == -2 and glu(T=0) == -2
-    assert glu(n=1 * 256 * 32 * 4 - 1) == -5
+    assert glu(kernel_size=29) == -2 and glu(inner_channels=100) == -2 and glu(B=65536) == -2 and glu(T=0) == -2
+    assert glu(ws_bytes=1 * 256 * 32 * 4 - 1) == -5
     assert b"u2c_glu_dwconv_silu_backward" in L.b2d_last_error()
     assert L.b2d_u2c_colsum(0, 4, 4, p, p, big, 0) == -1 and L.b2d_u2c_colsum(p, 0, 4, p, p, big, 0) == -2
     assert L.b2d_u2c_colsum(p, 129, 4, p, p, 2 * 4 * 4 - 1, 0) == -5                         # two slabs of 128 tokens
     assert L.b2d_u2c_layernorm_backward(p, p, p, 1e-5, 4, 128, p, p, p, big, 0) == -2        # C != 256
     assert L.b2d_u2c_layernorm_backward(p, p, 0, 1e-5, 4, 256, p, p, p, big, 0) == -1
     assert L.b2d_u2c_layernorm_backward(p, p, p, 1e-5, 4, 256, p, p, p, 2 * 256 * 4 - 1, 0) == -5
-    gn = lambda C=256, G=4, st=p, n=big: L.b2d_u2c_groupnorm_lrelu_backward(p, st, p, p, 1e-5, 0.01, p, 1, 8, C, G, p, p, p, n, 0)
-    assert gn(C=128) == -2 and gn(G=3) == -2 and gn(st=0) == -1 and gn(n=100) == -5
+    ok_gn = dict(x_pre=p, stats=p, gamma=p, beta=p, eps=1e-5, slope=0.01, gy=p, B=1, T=8, C=256, groups=4, gx=p,
+                 dgamma_dbeta=p, ws=p, ws_bytes=big, stream=0)
+    gn = lambda **kw: abi_call("b2d_u2c_groupnorm_lrelu_backward", dict(ok_gn, **kw))
+    assert gn(C=128) == -2 and gn(groups=3) == -2 and gn(stats=0) == -1 and gn(ws_bytes=100) == -5
     assert L.b2d_u2c_embed_backward(p, p, p, p, 0, 0, 8, p, p, p, big, 0) == -2              # B = 0 (aug_shift may be null)
     assert L.b2d_u2c_embed_backward(p, p, p, p, 0, 1, 8, 0, p, p, big, 0) == -1
     assert L.b2d_u2c_embed_backward(p, p, p, p, 0, 1, 8, p, p, p, 4 * 256 * 4 - 1, 0) == -5

@@ -3,9 +3,6 @@ driver's warp-shuffle shim) against float64 autograd of the same ops, plus the a
 device touched).  The kernels use neither shared memory nor barriers, so they have no ThreadSanitizer driver.  They run
 on hardware in tests/test_gpu_u2c_pcmer_backward.py."""
 import ctypes
-import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -13,8 +10,8 @@ import torch
 
 from ddsp_svc_b200 import _lib
 from tests import util
+from tests.emu_harness import abi_call, shared
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 EPS = 1e-4
 
 
@@ -56,19 +53,7 @@ def qkv_gather_reference(gq, gk, gv, qkv, normalized):
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = str(tmp_path_factory.mktemp("emu") / "libemu_u2c_pcmer_bwd.so")
-    cmd = ["g++", "-std=c++20", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-pthread", "-Wno-unknown-pragmas",
-           "-o", so, os.path.join(HERE, "emu", "emu_u2c_pcmer_bwd.cpp")]
-    proc = subprocess.run(cmd, capture_output=True, text=True)
-    assert proc.returncode == 0, proc.stderr
-    lib = ctypes.CDLL(so)
-    fp, i = ctypes.POINTER(ctypes.c_float), ctypes.c_int
-    lib.emu_attn_readout_bwd.argtypes = [fp] * 3 + [i] * 3 + [fp]
-    lib.emu_feat_bwd.argtypes = [fp] * 5 + [i] * 4 + [ctypes.c_float, fp]
-    lib.emu_qkv_gather_bwd.argtypes = [fp] * 4 + [i] * 4 + [fp]
-    return lib
+    return shared("emu_u2c_pcmer_bwd.cpp", tmp_path_factory)
 
 
 def _p(a):
@@ -159,19 +144,19 @@ def test_pcmer_backward_abi_argument_errors_do_not_touch_the_device():
     _lib.build()
     L = _lib.lib()
     p = 16                                                     # a non-null address
-    ro = lambda **kw: L.b2d_u2c_attn_readout_backward(*[{**dict(g=p, o=p, d=p, B=1, H=8, T=4, dh=64, gn=p, s=0), **kw}[k]
-                                                         for k in ("g", "o", "d", "B", "H", "T", "dh", "gn", "s")])
-    assert ro(g=0) == -1 and ro(d=0) == -1 and ro(gn=0) == -1
-    assert ro(dh=32) == -2 and ro(T=0) == -2 and ro(B=-1) == -2
+    ok_ro = dict(g_out=p, out=p, d_inv=p, B=1, H=8, T=4, dim_head=64, gn=p, stream=0)
+    ro = lambda **kw: abi_call("b2d_u2c_attn_readout_backward", dict(ok_ro, **kw))
+    assert ro(g_out=0) == -1 and ro(d_inv=0) == -1 and ro(gn=0) == -1
+    assert ro(dim_head=32) == -2 and ro(T=0) == -2 and ro(B=-1) == -2
     assert b"u2c_attn_readout_backward" in L.b2d_last_error()
-    ft = lambda **kw: L.b2d_u2c_softmax_features_backward(*[{**dict(g=p, f=p, x=p, v=p, sc=p, R=8, T=4, J=266, dh=64, q=1, e=1e-4,
-                                                                      gx=p, s=0), **kw}[k]
-                                                            for k in ("g", "f", "x", "v", "sc", "R", "T", "J", "dh", "q", "e", "gx", "s")])
-    assert ft(g=0) == -1 and ft(x=0) == -1 and ft(gx=0) == -1 and ft(sc=0) == -1
-    assert ft(dh=65) == -2 and ft(J=289) == -2 and ft(R=9) == -2 and ft(R=0) == -2
+    ok_ft = dict(g=p, features=p, data=p, vec=p, scal=p, rows=8, T=4, n_features=266, dim_head=64, is_query=1, eps=1e-4,
+                 gx=p, stream=0)
+    ft = lambda **kw: abi_call("b2d_u2c_softmax_features_backward", dict(ok_ft, **kw))
+    assert ft(g=0) == -1 and ft(data=0) == -1 and ft(gx=0) == -1 and ft(scal=0) == -1
+    assert ft(dim_head=65) == -2 and ft(n_features=289) == -2 and ft(rows=9) == -2 and ft(rows=0) == -2
     assert b"u2c_softmax_features_backward" in L.b2d_last_error()
-    qg = lambda **kw: L.b2d_u2c_qkv_gather_backward(*[{**dict(q=p, k=p, v=p, x=p, B=1, H=8, T=4, dh=64, n=1, o=p, s=0), **kw}[k]
-                                                      for k in ("q", "k", "v", "x", "B", "H", "T", "dh", "n", "o", "s")])
-    assert qg(q=0) == -1 and qg(o=0) == -1 and qg(x=0) == -1
-    assert qg(dh=128) == -2 and qg(H=0) == -2
+    ok_qg = dict(g_q=p, g_k=p, g_v=p, qkv=p, B=1, H=8, T=4, dim_head=64, normalized=1, g_qkv=p, stream=0)
+    qg = lambda **kw: abi_call("b2d_u2c_qkv_gather_backward", dict(ok_qg, **kw))
+    assert qg(g_q=0) == -1 and qg(g_qkv=0) == -1 and qg(qkv=0) == -1
+    assert qg(dim_head=128) == -2 and qg(H=0) == -2
     assert b"u2c_qkv_gather_backward" in L.b2d_last_error()
