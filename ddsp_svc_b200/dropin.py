@@ -90,7 +90,30 @@ def _patch_reflow(saved):
                 setattr(mod, name, getattr(own, name))
 
 
-def patch_reference(reflow=False):
+_DIFFUSION_MODULES = ("diffusion.vocoder", "diffusion.diffusion", "diffusion.wavenet", "diffusion.naive_v2_diff")
+_DIFFUSION_CLASSES = ("GaussianDiffusion", "WaveNet", "NaiveV2Diff")
+
+
+def _patch_diffusion(saved):
+    """rebind GaussianDiffusion / WaveNet / NaiveV2Diff in the reference's diffusion modules (those that import);
+    originals into saved["diffusion"] by module, since NaiveV2Diff also has a reflow original"""
+    import importlib
+    from . import diffusion as own
+    from . import reflow as own_reflow
+    ours = dict(GaussianDiffusion=own.GaussianDiffusion, WaveNet=own.WaveNet, NaiveV2Diff=own_reflow.NaiveV2Diff)
+    for modname in _DIFFUSION_MODULES:
+        try:
+            mod = importlib.import_module(modname)
+        except ImportError as e:
+            saved.setdefault("_not_patched", {})[modname] = "%s: %s" % (type(e).__name__, e)
+            continue
+        for name in _DIFFUSION_CLASSES:
+            if hasattr(mod, name):
+                saved.setdefault("diffusion", {}).setdefault(modname, {})[name] = getattr(mod, name)
+                setattr(mod, name, ours[name])
+
+
+def patch_reference(reflow=False, diffusion=False):
     """Swap the synthesizer classes inside the (importable) reference package.  Returns the dict
     of original classes so a caller can restore them; its keys say what was patched.  If the enhancer stack
     (nsf_hifigan.models) cannot be imported, only the synthesizers are patched and the reason is returned under
@@ -101,7 +124,13 @@ def patch_reference(reflow=False):
     import is reported under ``"_not_patched"``.  Off by default.  To run train_reflow.py on the kernels, also set
     ``ddsp_svc_b200.NaiveV2Diff.reflow_backward = True``: then ``RectifiedFlow(infer=False)`` returns the reflow loss
     with its backward, and Unit2Wav's training step trains every parameter (INTEGRATION.md section 3b); without it
-    infer=False and the sampler under grad raise NotImplementedError."""
+    infer=False and the sampler under grad raise NotImplementedError.
+
+    ``diffusion=True`` rebinds the diffusion models' sampler and denoisers (``GaussianDiffusion``, ``WaveNet``,
+    ``NaiveV2Diff``) in diffusion.vocoder, diffusion.diffusion, diffusion.wavenet and diffusion.naive_v2_diff, so
+    Unit2Mel / Unit2Wav / Unit2WavFast (main_diff.py) sample on the kernels; a module that does not import (diffusion.diffusion
+    imports librosa.sequence) is reported under ``"_not_patched"``.  Off by default.  Inference only: the training step
+    (train_diff.py) must run unpatched -- infer=False and calls under grad raise NotImplementedError."""
     import ddsp.vocoder as ref_vocoder          # the reference checkout must be on sys.path
     names = ("Sins", "CombSub", "CombSubSuperFast", "CombSubFast")
     saved = {name: getattr(ref_vocoder, name) for name in names}
@@ -129,6 +158,8 @@ def patch_reference(reflow=False):
         ref_nsf.SourceModuleHnNSF = sinegen.SourceModuleHnNSF
     if reflow:
         _patch_reflow(saved)
+    if diffusion:
+        _patch_diffusion(saved)
     return saved
 
 
@@ -151,3 +182,8 @@ def unpatch_reference(saved):
             for name in ("NaiveV2Diff", "RectifiedFlow"):
                 if mod is not None and name in saved and hasattr(mod, name):
                     setattr(mod, name, saved[name])
+    for modname, originals in saved.get("diffusion", {}).items():
+        mod = sys.modules.get(modname)
+        if mod is not None:
+            for name, cls in originals.items():
+                setattr(mod, name, cls)

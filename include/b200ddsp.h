@@ -458,6 +458,31 @@ int b2d_rf_layer_backward(const float* gz, float* gh, int B, int T, int D, int l
                           float* z, float* z_hi, float* z_lo, void* ws, size_t ws_bytes, void* stream);
 int b2d_rf_step_sums(const void* ws, size_t ws_bytes, int B, int T, int cols, float* out, void* stream);
 
+/* ---- diffusion models' sampler (diffusion.cu; GaussianDiffusion, diffusion/diffusion.py:216-384, around the WaveNet
+ * denoiser, diffusion/wavenet.py): the stages between the caller's library GEMMs.  Token-major [B, T, C] fp32, G a GEMM's
+ * output WITHOUT its bias, operand outputs (hi, lo) as for rf_* above.  Elementwise, one writer per element, no atomics:
+ * bit-identical from run to run.  The start and the finish are b2d_rf_start (its formula with t_start = sqrt(alpha_bar),
+ * one_minus_t_start = sqrt(1 - alpha_bar) is q_sample) and b2d_rf_finish (exactly denorm_spec).
+ * df_layer: stage 0: h [B T, C] = ReLU(G + bias); stage 1 / 2: r = G + bias over [B T, 2 C], h = (h + r[:C]) / sqrt 2 in
+ *   place, skip [B T, C] = r[C:] (1) or skip += r[C:] (2).  Then with step (row b at step + b step_stride, 0: one row for
+ *   every utterance): the k = 3 convolution's operand [B T, 3 C], row (b, t) = [y(t - 1) | y(t) | y(t + 1)] of
+ *   y = h + step[b], zero outside utterance b; step NULL: skip / skip_div into the [B T, C] operand.  C and step_stride
+ *   multiples of 4, buffers 16-byte aligned.
+ * df_gate: z = G + cond over [n_tokens, 2 C] (cond row n at cond + n cond_stride), sigmoid(z[:C]) tanh(z[C:]) into the
+ *   [n_tokens, C] operand.
+ * df_relu: ReLU(G + bias) [n_tokens, C] into the operand.
+ * df_update: over [B T, M]: eps = G + bias[m], d = a_x x + a_e eps, x' = c_x x + c_d d + c_1 h1 + c_2 h2 + c_3 h3 +
+ *   c_n noise with coef = {a_x, a_e, c_x, c_d, c_1, c_2, c_3, c_n} (8 floats on the device); h1..h3 [B T, M] or NULL,
+ *   noise [B, 1, M, T] channel-major or NULL.  d into d_out, x' into x_out and its operand into hi / lo, each optional
+ *   (NULL); d_out may be one of h1..h3 and x_out may be x (element-wise in place). */
+int b2d_df_layer(const float* g, const float* bias, float* h, float* skip, int stage, const float* step, int step_stride,
+                 float skip_div, int B, int T, int C, float* hi, float* lo, void* stream);
+int b2d_df_gate(const float* g, const float* cond, int cond_stride, int n_tokens, int C, float* hi, float* lo, void* stream);
+int b2d_df_relu(const float* g, const float* bias, int n_tokens, int C, float* hi, float* lo, void* stream);
+int b2d_df_update(const float* g, const float* bias, const float* coef, const float* x, float* d_out, const float* h1,
+                  const float* h2, const float* h3, const float* noise, int B, int T, int M, float* x_out, float* hi,
+                  float* lo, void* stream);
+
 /* ---- log-mel front end of the NSF-HiFiGAN vocoder: STFT.get_mel, nsf_hifigan/nvSTFT.py:73-117 (keyshift 0, speed 1) ----
  * audio [B, n_samples] -> mel [B, n_mels, n_frames], n_frames = b2d_mel_frames(...) (0 = signal too short):
  * reflect / constant padding by (win - hop)/2, frames of win_size = n_fft = 2048 at `hop`, periodic Hann `window` [2048],
