@@ -19,10 +19,11 @@
 #include "b2d_common.cuh"
 #endif
 #include "tf32_split.cuh"
+#include "token_slab.cuh"
 
 namespace {
 
-constexpr int kRfSlab = 32;      // frames of one utterance per slab of a token sum
+constexpr int kRfSlab = kTokenSlab;      // frames of one utterance per slab of a token sum
 
 __device__ __forceinline__ void rfb_emit(float v, float* __restrict__ hi, float* __restrict__ lo, size_t i) {
     if (!hi) return;

@@ -24,7 +24,14 @@ PNDM first denoise at k_step - speedup; the start's noise is randn_like of the t
 ``max(t - interval, 0)`` of a [B] tensor, which raises for B > 1 (and hands the network a Python int when the step is
 clipped to 0); here every B runs with the step clipped at 0.
 
-Training (infer=False, p_losses) is not built: it and every call under grad raise NotImplementedError.
+Training: with the denoiser's switch on (``WaveNet.diffusion_backward``; for NaiveV2Diff its own
+``reflow_backward``), ``GaussianDiffusion(infer=False)`` returns the reference's loss (p_losses, loss_type 'l2', with
+the reference's draws of t and the noise) and WaveNet's forward under grad its prediction, both differentiable with
+respect to the denoiser's parameters and the condition: ONE autograd Function each, whose forward is the inference
+forward (same launches, bit-identical) plus the saved activations and whose backward walks the layers in reverse on the
+kernels of csrc/diffusion_bwd.cu (and reflow_bwd.cu's loss and step sums) and library GEMMs at ``gemm_precision``.
+NaiveV2Diff's backward is reflow._network_backward.  With the switch off (the default) infer=False and every call under
+grad raise NotImplementedError; with it on, the samplers under grad still do.
 """
 import math
 
@@ -32,14 +39,21 @@ import numpy as np
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+from torch.autograd.function import once_differentiable
 
 from . import _lib
 from .ops import _need_cuda_f32, _stream
-from .reflow import NaiveV2Diff, _DiffusionEmbedding, _under_grad
+from .reflow import NaiveV2Diff, _DiffusionEmbedding, _network_backward, _under_grad
 from .unit2control import _Gemm, _k, _split
 
-_NO_TRAINING = ("%s: training (p_losses and the denoiser's gradients) is not built; run inference with infer=True under "
+_NO_TRAINING = ("%s: training (p_losses and the denoiser's gradients) is off; turn it on with WaveNet.diffusion_backward "
+                "= True (NaiveV2Diff.reflow_backward = True for that denoiser), or run inference with infer=True under "
                 "torch.no_grad()")
+
+
+def _training_switch(fn):
+    """the denoiser's training switch: WaveNet.diffusion_backward, or NaiveV2Diff's own reflow_backward"""
+    return fn.diffusion_backward if isinstance(fn, WaveNet) else fn.reflow_backward
 
 
 class _ResidualBlock(nn.Module):                 # wavenet.py:31-62 (dilation 1 in every configuration)
@@ -53,9 +67,177 @@ class _ResidualBlock(nn.Module):                 # wavenet.py:31-62 (dilation 1 
         self.output_projection = nn.Conv1d(residual_channels, 2 * residual_channels, 1)
 
 
+def _wavenet_backward(mod, g, S, gv, gvs, want_cond):
+    """WaveNet's backward from gv [B T, M], the cotangent of its output (fp32), and gvs, that cotangent as the operand of
+    the output projection's adjoints.  S: what _velocity / _step_rows / _cond_rows saved.  -> (dict of parameter
+    gradients by name, the condition's cotangent [B T, n_hidden] or None).
+
+    Output side: the output projection's adjoints, df_relu_backward at the skip projection, its adjoints; every layer's
+    skip output receives the same cotangent (g_p W_skip) / sqrt(n_layers).  Per layer, reversed: g_R = [g_h' / sqrt 2 |
+    g_skip] (df_layer_backward writes it), the output projection's adjoints, df_gate_backward into column block i of
+    G_Z, the convolution's adjoints over the saved [B T, 3 C] operand, then df_layer_backward (the adjoint of the
+    operand's scatter, g_h, the next g_R, the step sums).  Every layer's condition projection then takes ONE pair of
+    GEMMs over G_Z [B T, n_layers 2 C], whose column sums are both the condition projection's and the convolution's bias
+    gradients; the step projections take the per-utterance token sums of g_y; the step MLP's GEMMs have B rows."""
+    P, (B, T) = S["P"], S["BT"]
+    L, C, N, dev, nL = _lib.lib(), mod.dim, B * T, gv.device, len(S["P"]["layers"])
+    LC, Z2, split = nL * C, nL * 2 * C, g.mode == "3xtf32"
+    ws_bytes = L.b2d_u2c_backward_workspace_bytes(B, T, 2 * C, max(mod.mel_channels, 4 * C, Z2))
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    rws_bytes = L.b2d_rf_backward_workspace_bytes(B, T, LC)
+    rws = torch.empty(rws_bytes, dtype=torch.uint8, device=dev)
+    new = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)
+    operand = lambda n, c, fp32: mod._operand(g, n, c, dev) if split else fp32
+    halves = lambda ops: mod._ptrs(ops) if split else (0, 0)           # fp32 modes: the fp32 tensor is the operand
+    cols = lambda ops, blk: tuple(o[:, blk] for o in ops) if split else ops[:, blk]
+
+    def colsum(x):
+        out = new(x.shape[1])
+        _k(L.b2d_u2c_colsum(x.data_ptr(), x.shape[0], x.shape[1], out.data_ptr(), ws.data_ptr(), ws_bytes, _stream()),
+           "b2d_u2c_colsum")
+        return out
+
+    def relu_backward(gy, pre, bias):
+        """-> (fp32 cotangent of ReLU(pre + bias)'s input, its operand)"""
+        gx = new(*gy.shape)
+        ops = operand(gy.shape[0], gy.shape[1], gx)
+        hi, lo = halves(ops)
+        _k(L.b2d_df_relu_backward(gy.data_ptr(), pre.data_ptr(), bias.data_ptr(), gy.shape[0], gy.shape[1], gx.data_ptr(),
+                                  hi, lo, _stream()), "b2d_df_relu_backward")
+        return gx, ops
+
+    w3 = lambda x: x.unsqueeze(-1)
+    G = {"output_projection.weight": w3(g.grad_weight(gvs, S["q"])), "output_projection.bias": colsum(gv)}
+    gp, gps = relu_backward(g.grad_input(gvs, P["out_w"]), S["S"], P["skip_b"])
+    G["skip_projection.weight"], G["skip_projection.bias"] = w3(g.grad_weight(gps, S["sk"])), colsum(gp)
+    gsk = g.grad_input(gps, P["skip_w"])                                 # [B T, C]; / sqrt(n_layers) in df_layer_backward
+    skip_div = math.sqrt(nL)
+    gh = new(N, C)
+    gr = new(N, 2 * C)
+    grs = operand(N, 2 * C, gr)
+    gr_hi, gr_lo = halves(grs)
+    _k(L.b2d_df_layer_backward(0, gh.data_ptr(), gsk.data_ptr(), skip_div, B, T, C, nL - 1, nL, gr.data_ptr(), gr_hi, gr_lo,
+                               0, 0, _stream()), "b2d_df_layer_backward")       # h_L feeds nothing: g_R = [0 | g_skip]
+    z = new(N, Z2)                                                       # G_Z: every layer's g_z
+    zs = operand(N, Z2, z)
+    z_hi, z_lo = halves(zs)
+    crows = S["crows"]
+    for i in reversed(range(nL)):
+        us, Zi, vs = S["layers"][i]
+        Ly, pre = P["layers"][i], "residual_layers.%d." % i
+        G[pre + "output_projection.weight"] = w3(g.grad_weight(grs, vs))
+        G[pre + "output_projection.bias"] = colsum(gr)
+        ga = g.grad_input(grs, Ly["out_w"])                              # [B T, C]: cotangent of the gate's output
+        _k(L.b2d_df_gate_backward(ga.data_ptr(), Zi.data_ptr(), crows.data_ptr() + 4 * i * 2 * C, Z2, N, C, i, nL,
+                                  z.data_ptr(), z_hi, z_lo, _stream()), "b2d_df_gate_backward")
+        gzs = cols(zs, slice(i * 2 * C, (i + 1) * 2 * C))
+        dW = g.grad_weight(gzs, us)                                      # [2 C, 3 C]: column block k is tap k
+        G[pre + "dilated_conv.weight"] = dW.reshape(2 * C, 3, C).permute(0, 2, 1).contiguous()
+        gu = g.grad_input(gzs, Ly["conv_w"])                             # [B T, 3 C]
+        nxt = i > 0
+        _k(L.b2d_df_layer_backward(gu.data_ptr(), gh.data_ptr(), gsk.data_ptr(), skip_div, B, T, C, i, nL,
+                                   gr.data_ptr() if nxt else 0, gr_hi if nxt else 0, gr_lo if nxt else 0, rws.data_ptr(),
+                                   rws_bytes, _stream()), "b2d_df_layer_backward")
+    # input projection: h_0 = ReLU(in_proj(x_t)); x_t is data
+    gpre, gpres = relu_backward(gh, S["pre"], P["in_b"])
+    G["input_projection.weight"], G["input_projection.bias"] = w3(g.grad_weight(gpres, S["xs"])), colsum(gpre)
+    # every layer's condition projection at once; its bias and the convolution's share G_Z's column sums
+    dcw, dcb = g.grad_weight(zs, S["cond"]), colsum(z)
+    g_cond = g.grad_input(zs, P["cond_w"]) if want_cond else None
+    # step projections from the per-utterance sums of g_y, then the step MLP (the sinusoidal embedding is data)
+    gS = new(B, LC)
+    _k(L.b2d_rf_step_sums(rws.data_ptr(), rws_bytes, B, T, LC, gS.data_ptr(), _stream()), "b2d_rf_step_sums")
+    gSs = g.split(gS)
+    dsw, dsb = g.grad_weight(gSs, g.split(S["e2"])), colsum(gS)
+    ge2 = g.grad_input(gSs, P["step_w"])                                 # [B, C]
+    ge2s = g.split(ge2)
+    G["mlp.2.weight"], G["mlp.2.bias"] = g.grad_weight(ge2s, g.split(S["a1"])), colsum(ge2)
+    ga1 = g.grad_input(ge2s, P["mlp2_w"])                                # [B, 4 C]
+    ge1 = new(*ga1.shape)
+    _k(L.b2d_df_mish_backward(ga1.data_ptr(), S["e1"].data_ptr(), ga1.numel(), ge1.data_ptr(), 0, 0, _stream()),
+       "b2d_df_mish_backward")
+    G["mlp.0.weight"], G["mlp.0.bias"] = g.grad_weight(g.split(ge1), g.split(S["e0"])), colsum(ge1)
+    for i in range(nL):
+        pre, zr, sr = "residual_layers.%d." % i, slice(i * 2 * C, (i + 1) * 2 * C), slice(i * C, (i + 1) * C)
+        G[pre + "conditioner_projection.weight"] = w3(dcw[zr])
+        G[pre + "conditioner_projection.bias"] = dcb[zr]
+        G[pre + "dilated_conv.bias"] = dcb[zr].clone()
+        G[pre + "diffusion_projection.weight"], G[pre + "diffusion_projection.bias"] = dsw[sr], dsb[sr]
+    return G, g_cond
+
+
+class _WaveNetFunction(torch.autograd.Function):
+    """WaveNet as ONE differentiable op: (module, parameter names, x [B, M, T], steps [B], cond [B, n_hidden, T],
+    *parameters) -> the predicted noise [B T, M] token-major.  forward is WaveNet._run as it stands (same launches, same
+    bits) plus the saved activations; backward is _wavenet_backward.  x and steps are data.  Not differentiable twice."""
+
+    @staticmethod
+    def forward(ctx, mod, names, x, steps, cond, *params):
+        S = {}
+        with _Gemm(mod.gemm_precision) as g:
+            v = mod._run(g, x, steps, cond, save=S)
+        ctx.mod, ctx.names, ctx.saved, ctx.cond_shape = mod, names, S, cond.shape
+        ctx.set_materialize_grads(False)
+        return v
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gv):
+        if gv is None:
+            return (None,) * (5 + len(ctx.names))
+        mod, (B, Mc, T) = ctx.mod, ctx.cond_shape
+        with _Gemm(mod.gemm_precision) as g:
+            gv = gv.contiguous()
+            G, g_cond = _wavenet_backward(mod, g, ctx.saved, gv, g.split(gv), ctx.needs_input_grad[4])
+        g_cond = None if g_cond is None else g_cond.reshape(B, T, Mc).transpose(1, 2)
+        return (None, None, None, None, g_cond) + tuple(G.get(n) for n in ctx.names)
+
+
+class _DiffusionLossFunction(torch.autograd.Function):
+    """The diffusion loss with its denoiser (WaveNet or NaiveV2Diff) as ONE differentiable op: (diffusion, parameter
+    names, condition [B, T, M_cond], gt [B, T, M], t [B] int64, noise [B, T, M] token-major, *parameters) -> loss [].
+    forward is GaussianDiffusion._loss_forward (df_loss_input, the denoiser as its _velocity runs it, rf_loss with w = 1
+    and target = noise); backward is rf_loss_backward, which writes the output projection's operand directly, then
+    _wavenet_backward or reflow's _network_backward.  gt, t and noise are data.  Not differentiable twice."""
+
+    @staticmethod
+    def forward(ctx, diff, names, condition, gt, t, noise, *params):
+        S = {}
+        loss = diff._loss_forward(condition, gt, t, noise, save=S)
+        ctx.diff, ctx.names, ctx.saved = diff, names, S
+        ctx.set_materialize_grads(False)
+        return loss
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gl):
+        if gl is None:
+            return (None,) * (6 + len(ctx.names))
+        mod, S = ctx.diff.denoise_fn, ctx.saved
+        (B, T), M, dev = S["BT"], mod.mel_channels, gl.device
+        gl = gl.reshape(1).to(torch.float32).contiguous()
+        with _Gemm(mod.gemm_precision) as g:
+            gv = torch.empty(B * T, M, dtype=torch.float32, device=dev)
+            gvs = mod._operand(g, B * T, M, dev) if g.mode == "3xtf32" else gv
+            hi, lo = mod._ptrs(gvs) if g.mode == "3xtf32" else (0, 0)
+            _k(_lib.lib().b2d_rf_loss_backward(S["G"].data_ptr(), S["P"]["out_b"].data_ptr(), S["target"].data_ptr(),
+                                               S["w"].data_ptr(), gl.data_ptr(), B, T, M, gv.data_ptr(), hi, lo, _stream()),
+               "b2d_rf_loss_backward")
+            backward = _wavenet_backward if isinstance(mod, WaveNet) else _network_backward
+            G, g_cond = backward(mod, g, S, gv, gvs, ctx.needs_input_grad[2])
+        g_cond = None if g_cond is None else g_cond.reshape(B, T, -1)
+        return (None, None, g_cond, None, None, None) + tuple(G.get(n) for n in ctx.names)
+
+
 class WaveNet(nn.Module):
     #: precision of the library GEMMs, see unit2control._Gemm: "3xtf32" (default), "fp32", "tf32"
     gemm_precision = "3xtf32"
+    #: training: with grad mode on and a parameter (or cond) that requires grad, forward is differentiable with respect
+    #: to the parameters and cond, and GaussianDiffusion(infer=False) around this network returns the diffusion loss,
+    #: differentiable with respect to the parameters and condition (the backward of _WaveNetFunction /
+    #: _DiffusionLossFunction; the forward issues the same kernels with the same results).  Off by default: every call
+    #: under grad and infer=False raise.  Set it on the class (``WaveNet.diffusion_backward = True``) or per instance.
+    diffusion_backward = False
 
     def __init__(self, in_dims=128, n_layers=20, n_chans=384, n_hidden=256):
         super().__init__()
@@ -109,24 +291,34 @@ class WaveNet(nn.Module):
         return P
 
     # ---- the sampler's three operations (the same names and signatures as NaiveV2Diff's) ----
-    def _step_rows(self, g, P, steps):
-        """diffusion steps [E] -> every layer's step projection [E, n_layers C] (embedding, MLP, projections)"""
-        e1 = g.linear(self.diffusion_embedding(steps), P["mlp1_w"], P["mlp1_b"])
-        e2 = g.linear(F.mish(e1), P["mlp2_w"], P["mlp2_b"])
+    def _step_rows(self, g, P, steps, save=None):
+        """diffusion steps [E] -> every layer's step projection [E, n_layers C] (embedding, MLP, projections);
+        ``save``: a dict that receives the MLP's input, pre-activation and outputs"""
+        e0 = self.diffusion_embedding(steps)
+        e1 = g.linear(e0, P["mlp1_w"], P["mlp1_b"])
+        a1 = F.mish(e1)
+        e2 = g.linear(a1, P["mlp2_w"], P["mlp2_b"])
+        if save is not None:
+            save.update(e0=e0, e1=e1, a1=a1, e2=e2)
         return g.linear(e2, P["step_w"], P["step_b"])
 
-    def _cond_rows(self, g, P, cond_tm):
+    def _cond_rows(self, g, P, cond_tm, save=None):
         """condition [B, T, n_hidden] token-major -> every layer's condition projection plus both biases
-        [B T, n_layers 2 C] (one GEMM)"""
-        return g.mm(g.split(cond_tm.reshape(-1, cond_tm.shape[-1])), P["cond_w"], P["cond_b"])
+        [B T, n_layers 2 C] (one GEMM); ``save``: a dict that receives the condition's operand and the rows"""
+        cs = g.split(cond_tm.reshape(-1, cond_tm.shape[-1]))
+        rows = g.mm(cs, P["cond_w"], P["cond_b"])
+        if save is not None:
+            save.update(cond=cs, crows=rows)
+        return rows
 
     _operand = staticmethod(NaiveV2Diff._operand)
     _ptrs = staticmethod(NaiveV2Diff._ptrs)
 
-    def _velocity(self, g, P, xs, steps, step_stride, conds, B, T, out_bias=None):
+    def _velocity(self, g, P, xs, steps, step_stride, conds, B, T, out_bias=None, save=None):
         """one evaluation of the denoiser: xs the input operand [B T, M] -> output projection [B T, M] (+ out_bias);
         steps: the step rows of this evaluation ([B or 1, n_layers C] from row stride step_stride), conds
-        [B T, n_layers 2 C]"""
+        [B T, n_layers 2 C].  ``save``: a dict that receives what the backward needs (then every operand gets its own
+        buffer; same launches, same values)"""
         L, C, dev, N, nL = _lib.lib(), self.dim, conds.device, B * T, len(P["layers"])
         new = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)
         h, skip = new(N, C), new(N, C)
@@ -135,6 +327,8 @@ class WaveNet(nn.Module):
         G = g.mm(xs, P["in_w"])
         _k(L.b2d_df_layer(G.data_ptr(), P["in_b"].data_ptr(), h.data_ptr(), 0, 0, steps.data_ptr(), step_stride, 1.0, B, T,
                           C, uh, ul, _stream()), "b2d_df_layer")
+        if save is not None:
+            save.update(xs=xs, pre=G, layers=[])
         skip_div = math.sqrt(nL)
         for i, Ly in enumerate(P["layers"]):
             Z = g.mm(us, Ly["conv_w"])                                                   # [B T, 2 C]
@@ -142,19 +336,58 @@ class WaveNet(nn.Module):
                "b2d_df_gate")
             R = g.mm(vs, Ly["out_w"])                                                    # [B T, 2 C]: residual | skip
             last = i + 1 == nL
+            if save is not None:                     # the convolution operand, its product, the gate's operand
+                save["layers"].append((us, Z, vs))
+                if not last:
+                    us = self._operand(g, N, 3 * C, dev)
+                vs = self._operand(g, N, C, dev)
+                (uh, ul), (vh, vl) = self._ptrs(us), self._ptrs(vs)
             sp = 0 if last else steps.data_ptr() + 4 * (i + 1) * C
             oh, ol = (vh, vl) if last else (uh, ul)
             _k(L.b2d_df_layer(R.data_ptr(), Ly["out_b"].data_ptr(), h.data_ptr(), skip.data_ptr(), 1 if i == 0 else 2, sp,
                               step_stride, skip_div, B, T, C, oh, ol, _stream()), "b2d_df_layer")
         S = g.mm(vs, P["skip_w"])
+        if save is not None:                         # the skip projection's operand and product
+            save.update(sk=vs, S=S)
+            vs = self._operand(g, N, C, dev)
+            vh, vl = self._ptrs(vs)
         _k(L.b2d_df_relu(S.data_ptr(), P["skip_b"].data_ptr(), N, C, vh, vl, _stream()), "b2d_df_relu")
+        if save is not None:
+            save["q"] = vs
         return g.mm(vs, P["out_w"], out_bias)
+
+    def _run(self, g, x, steps, cond, save=None):
+        """x [B, M, T] contiguous, steps [B], cond [B, n_hidden, T] -> the predicted noise [B T, M] token-major (with the
+        output bias); ``save``: a dict that receives what the backward needs"""
+        B, M, T = x.shape
+        P = self._pack()
+        srows = self._step_rows(g, P, steps, save).contiguous()
+        crows = self._cond_rows(g, P, cond.transpose(1, 2).contiguous(), save)
+        xs = self._operand(g, B * T, M, x.device)
+        hi, lo = self._ptrs(xs)
+        _k(_lib.lib().b2d_rf_start(x.data_ptr(), 0, 0.0, 1.0, 0.0, 1.0, B, T, M, 0, hi, lo, _stream()), "b2d_rf_start")
+        if save is not None:
+            save.update(P=P, BT=(B, T))
+        return self._velocity(g, P, xs, srows, srows.shape[1], crows, B, T, out_bias=P["out_b"], save=save)
+
+    def _grad_params(self):
+        """(names, tensors) of the parameters the backward produces gradients for: all of them, in named_parameters order"""
+        items = list(self.named_parameters())
+        return tuple(n for n, _ in items), tuple(p for _, p in items)
 
     def forward(self, spec, diffusion_step, cond):
         """spec [B, 1, M, T] or [B, M, T], diffusion_step [B] (or one value for every utterance), cond [B, n_hidden, T]
-        -> the predicted noise [B, 1, M, T] (wavenet.py:84-108)"""
-        if _under_grad(self, spec, diffusion_step, cond):
+        -> the predicted noise [B, 1, M, T] (wavenet.py:84-108).  Under grad (``diffusion_backward`` on):
+        differentiable with respect to the parameters and cond, bit-identical to the no_grad call; spec and
+        diffusion_step are data."""
+        grad = _under_grad(self, spec, diffusion_step, cond)
+        if grad and not self.diffusion_backward:
             raise NotImplementedError(_NO_TRAINING % "WaveNet")
+        if grad:
+            for name, t in (("spec", spec), ("diffusion_step", diffusion_step)):
+                if torch.is_tensor(t) and t.requires_grad:
+                    raise NotImplementedError("WaveNet: no gradient with respect to %s (the diffusion loss does not need "
+                                              "it, so it is not built)" % name)
         x = spec[:, 0] if spec.dim() == 4 else spec
         _need_cuda_f32("spec", x)
         _need_cuda_f32("cond", cond)
@@ -163,15 +396,13 @@ class WaveNet(nn.Module):
             raise ValueError("WaveNet: spec [B, 1, %d, T] and cond [B, %d, T] expected, got %s and %s"
                              % (self.mel_channels, self.condition_dim, tuple(spec.shape), tuple(cond.shape)))
         steps = torch.as_tensor(diffusion_step, device=x.device).reshape(-1).expand(B)
-        with torch.no_grad(), _Gemm(self.gemm_precision) as g:
-            P = self._pack()
-            srows = self._step_rows(g, P, steps).contiguous()
-            crows = self._cond_rows(g, P, cond.transpose(1, 2).contiguous())
-            xs = self._operand(g, B * T, M, x.device)
-            hi, lo = self._ptrs(xs)
-            _k(_lib.lib().b2d_rf_start(x.contiguous().data_ptr(), 0, 0.0, 1.0, 0.0, 1.0, B, T, M, 0, hi, lo, _stream()),
-               "b2d_rf_start")
-            v = self._velocity(g, P, xs, srows, srows.shape[1], crows, B, T, out_bias=P["out_b"])
+        x = x.contiguous()
+        if grad:
+            names, params = self._grad_params()
+            v = _WaveNetFunction.apply(self, names, x, steps.detach(), cond, *params)
+        else:
+            with torch.no_grad(), _Gemm(self.gemm_precision) as g:
+                v = self._run(g, x, steps, cond)
         return v.reshape(B, T, M).transpose(1, 2).contiguous()[:, None]
 
 
@@ -368,11 +599,22 @@ class GaussianDiffusion(nn.Module):
         its noise drawn as randn_like of the transposed [B, 1, M, T] view, from t = k_step.  Then ``method``:
         'dpm-solver', 'unipc' (t // infer_speedup steps, at least 2), 'pndm', 'ddim'; None or infer_speedup 1: DDPM,
         one torch.randn((B, 1, M, T)) per step.  The draws happen on condition's device in the reference's order, so
-        seeded runs compare.  ``use_tqdm`` is accepted and ignored."""
+        seeded runs compare.  ``use_tqdm`` is accepted and ignored.
+
+        ``infer=False`` with the denoiser's switch on (``WaveNet.diffusion_backward``, ``NaiveV2Diff.reflow_backward``):
+        the reference's training loss (diffusion.py:194-238, loss_type 'l2') with its draws: t = torch.randint(0, t_max,
+        (B,)) with t_max = k_step, or self.k_step when k_step is None, then the noise as randn_like of the transposed
+        [B, 1, M, T] view of norm(gt_spec), which is token-major in memory.  Differentiable with respect to the
+        denoiser's parameters and condition; gt_spec is data."""
+        training = _training_switch(self.denoise_fn)
         if not infer:
-            raise NotImplementedError(_NO_TRAINING % "GaussianDiffusion")
+            if not training:
+                raise NotImplementedError(_NO_TRAINING % "GaussianDiffusion")
+            return self._training_loss(condition, gt_spec, k_step)
         if _under_grad(self, condition, gt_spec):
-            raise NotImplementedError(_NO_TRAINING % "GaussianDiffusion")
+            raise NotImplementedError(_NO_TRAINING % "GaussianDiffusion" if not training else
+                                      "GaussianDiffusion: the samplers (infer=True) are not differentiable; run them "
+                                      "under torch.no_grad()")
         _need_cuda_f32("condition", condition)
         fn, M, dev = self.denoise_fn, self.out_dims, condition.device
         B, T, Mc = condition.shape
@@ -444,3 +686,74 @@ class GaussianDiffusion(nn.Module):
             out = torch.empty(B, T, M, dtype=torch.float32, device=dev)
             _k(L.b2d_rf_finish(x.data_ptr(), spec_min, spec_range, N * M, out.data_ptr(), _stream()), "b2d_rf_finish")
         return out
+
+    # ---- training ----
+    def _training_loss(self, condition, gt_spec, k_step):
+        """forward(infer=False): the reference's draws (torch, on condition's device, in its order), then _loss"""
+        if gt_spec is None:
+            raise ValueError("GaussianDiffusion: infer=False needs gt_spec")
+        B, T, M, dev = condition.shape[0], condition.shape[1], self.out_dims, condition.device
+        t_max = self.k_step if k_step is None else k_step
+        if not 0 < t_max <= self.num_timesteps:
+            raise ValueError("GaussianDiffusion: k_step must be in [1, %d] (the schedule's length), got %r"
+                             % (self.num_timesteps, t_max))
+        t = torch.randint(0, t_max, (B,), device=dev).long()
+        # randn_like(x_start) of the transposed view keeps its strides (T M, T M, 1, M): the draw fills [B, T, M] in order
+        noise = torch.empty_strided((B, 1, M, T), (T * M, T * M, 1, M), device=dev).normal_()
+        return self._loss(condition, gt_spec, t, noise[:, 0].transpose(1, 2))
+
+    def _loss(self, condition, gt_spec, t, noise):
+        """the diffusion loss after the draws: condition [B, T, M_cond], gt_spec [B, T, M], t [B] int64 (steps in
+        [0, num_timesteps)), noise [B, T, M] token-major -> loss [] fp32, F.mse_loss(noise, denoise_fn(q_sample(...))).
+        Under grad: differentiable with respect to the denoiser's parameters and condition; otherwise the same value
+        without saving activations"""
+        fn, M = self.denoise_fn, self.out_dims
+        if not _training_switch(fn):
+            raise NotImplementedError(_NO_TRAINING % "GaussianDiffusion")
+        for name, v in (("condition", condition), ("gt_spec", gt_spec), ("noise", noise)):
+            _need_cuda_f32(name, v)
+        B, T, Mc = condition.shape
+        if M != fn.mel_channels or Mc != fn.condition_dim:
+            raise ValueError("GaussianDiffusion: out_dims / condition width do not match the denoiser")
+        if gt_spec.shape != (B, T, M) or noise.shape != (B, T, M) or t.shape != (B,):
+            raise ValueError("GaussianDiffusion: gt_spec and noise must be [B, T, %d] like condition, t [B]" % M)
+        if t.dtype != torch.int64 or t.device != condition.device:
+            raise ValueError("GaussianDiffusion: t must be an int64 tensor on condition's device")
+        for name, v in (("gt_spec", gt_spec), ("noise", noise)):
+            if v.requires_grad:
+                raise NotImplementedError("GaussianDiffusion: no gradient with respect to %s (data)" % name)
+        args = (condition.contiguous(), gt_spec.contiguous(), t.contiguous(), noise.contiguous())
+        if _under_grad(self, condition):
+            names, params = fn._grad_params()
+            return _DiffusionLossFunction.apply(self, names, *args, *params)
+        with torch.no_grad():
+            return self._loss_forward(*args)
+
+    def _loss_forward(self, condition, gt, t, noise, save=None):
+        """the loss on the kernels: df_loss_input (q_sample with the steps gathered on the device), the denoiser,
+        rf_loss with w = 1 and target = noise (its mean of (target - v)^2 is F.mse_loss).  ``save``: a dict that
+        receives what the backward needs"""
+        fn, (B, T, _), M, dev = self.denoise_fn, condition.shape, self.out_dims, condition.device
+        L, N = _lib.lib(), B * T
+        buf = self._host()
+        spec_min, spec_range = float(buf["spec_min"][0]), float(buf["spec_max"][0] - buf["spec_min"][0])
+        with _Gemm(fn.gemm_precision) as g:
+            P = fn._pack()
+            srows = fn._step_rows(g, P, t, save).contiguous()                              # [B, n_layers C]
+            crows = fn._cond_rows(g, P, condition, save)
+            xs = fn._operand(g, N, M, dev)
+            hi, lo = fn._ptrs(xs)
+            sa, s1m = self.sqrt_alphas_cumprod.contiguous(), self.sqrt_one_minus_alphas_cumprod.contiguous()
+            _k(L.b2d_df_loss_input(gt.data_ptr(), noise.data_ptr(), t.data_ptr(), sa.data_ptr(), s1m.data_ptr(), sa.numel(),
+                                   spec_min, spec_range, B, T, M, hi, lo, _stream()),
+               "b2d_df_loss_input")
+            G = fn._velocity(g, P, xs, srows, srows.shape[1], crows, B, T, save=save)
+            w = torch.ones(B, dtype=torch.float32, device=dev)
+            ws_bytes = L.b2d_rf_backward_workspace_bytes(B, T, M)
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+            loss = torch.empty((), dtype=torch.float32, device=dev)
+            _k(L.b2d_rf_loss(G.data_ptr(), P["out_b"].data_ptr(), noise.data_ptr(), w.data_ptr(), B, T, M, ws.data_ptr(),
+                             ws_bytes, loss.data_ptr(), _stream()), "b2d_rf_loss")
+        if save is not None:
+            save.update(P=P, BT=(B, T), G=G, target=noise, w=w)
+        return loss

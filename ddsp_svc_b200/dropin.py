@@ -129,8 +129,11 @@ def patch_reference(reflow=False, diffusion=False):
     ``diffusion=True`` rebinds the diffusion models' sampler and denoisers (``GaussianDiffusion``, ``WaveNet``,
     ``NaiveV2Diff``) in diffusion.vocoder, diffusion.diffusion, diffusion.wavenet and diffusion.naive_v2_diff, so
     Unit2Mel / Unit2Wav / Unit2WavFast (main_diff.py) sample on the kernels; a module that does not import (diffusion.diffusion
-    imports librosa.sequence) is reported under ``"_not_patched"``.  Off by default.  Inference only: the training step
-    (train_diff.py) must run unpatched -- infer=False and calls under grad raise NotImplementedError."""
+    imports librosa.sequence) is reported under ``"_not_patched"``.  Off by default.  To run train_diff.py on the kernels,
+    also set ``ddsp_svc_b200.WaveNet.diffusion_backward = True`` (diffusion.yaml, diffusion-new.yaml) or
+    ``ddsp_svc_b200.NaiveV2Diff.reflow_backward = True`` (diffusion-fast.yaml): then ``GaussianDiffusion(infer=False)``
+    returns the diffusion loss with its backward (DESIGN.md section 4.15b); without them infer=False and calls under
+    grad raise NotImplementedError.  The samplers under grad raise in any case."""
     import ddsp.vocoder as ref_vocoder          # the reference checkout must be on sys.path
     names = ("Sins", "CombSub", "CombSubSuperFast", "CombSubFast")
     saved = {name: getattr(ref_vocoder, name) for name in names}

@@ -483,6 +483,35 @@ int b2d_df_update(const float* g, const float* bias, const float* coef, const fl
                   const float* h2, const float* h3, const float* noise, int B, int T, int M, float* x_out, float* hi,
                   float* lo, void* stream);
 
+/* ---- diffusion training loss (diffusion/diffusion.py:194-238, q_sample + F.mse_loss, loss_type 'l2') and the WaveNet
+ * denoiser's backward (diffusion_bwd.cu): the stages between the caller's library GEMMs and their adjoints.  The loss and
+ * its backward are b2d_rf_loss / b2d_rf_loss_backward with w = 1 and target = noise; the step projection's cotangent is
+ * b2d_rf_step_sums over the slabs df_layer_backward writes.  Token-major [B, T, C] fp32, G a GEMM output WITHOUT its
+ * bias, operand outputs (hi, lo) as for rf_* above (optional where a fp32 output is also written).  No atomics, no
+ * shared memory: bit-identical from run to run and independent of the device.
+ * df_loss_input: the operand of x_t [B, T, M] = sqrt_ac[t_b] norm(gt) + sqrt_1m_ac[t_b] noise (norm as rf_start; fp32
+ *   products and sum, no contraction), gt and noise token-major, t [B] int64 on the device, the two tables [n_steps] on
+ *   the device (no host synchronisation); a t_b outside [0, n_steps) gives NaN.  hi required.
+ * df_relu_backward: gx [n_rows, C] = gy where pre + bias[c] > 0, else 0.
+ * df_mish_backward: gx [n] = gy mish'(x), mish(x) = x tanh(softplus(x)).
+ * df_gate_backward: ga [n_tokens, C] the cotangent of df_gate's output; z = G + cond recomputed as df_gate does (cond row
+ *   n at cond + n cond_stride) -> the cotangent of z [n_tokens, 2 C] into columns [layer 2 C, (layer + 1) 2 C) of
+ *   gz [n_tokens, n_layers 2 C] (operand into gz_hi / gz_lo).
+ * df_layer_backward: for layer `layer` of n_layers after its g_U GEMM, gu [B T, 3 C]: gh [B T, C] = gh / sqrt 2 + g_y in
+ *   place with g_y(t) = gu[t + 1, block 0] + gu[t, block 1] + gu[t - 1, block 2] inside utterance b (the adjoint of
+ *   df_layer's convolution operand), g_y's per-slab sums into ws (b2d_rf_backward_workspace_bytes(B, T, n_layers C)).
+ *   gu NULL (the start, before the last layer): gh = 0 and ws unused.  Then gr [B T, 2 C] (optional, gsk [B T, C] then
+ *   required) = [gh / sqrt 2 | gsk / skip_div], operand into gr_hi / gr_lo. */
+int b2d_df_loss_input(const float* gt, const float* noise, const int64_t* t, const float* sqrt_ac, const float* sqrt_1m_ac,
+                      int n_steps, float spec_min, float spec_range, int B, int T, int M, float* hi, float* lo, void* stream);
+int b2d_df_relu_backward(const float* gy, const float* pre, const float* bias, int n_rows, int C, float* gx, float* hi,
+                         float* lo, void* stream);
+int b2d_df_mish_backward(const float* gy, const float* x, int n, float* gx, float* hi, float* lo, void* stream);
+int b2d_df_gate_backward(const float* ga, const float* g, const float* cond, int cond_stride, int n_tokens, int C, int layer,
+                         int n_layers, float* gz, float* gz_hi, float* gz_lo, void* stream);
+int b2d_df_layer_backward(const float* gu, float* gh, const float* gsk, float skip_div, int B, int T, int C, int layer,
+                          int n_layers, float* gr, float* gr_hi, float* gr_lo, void* ws, size_t ws_bytes, void* stream);
+
 /* ---- log-mel front end of the NSF-HiFiGAN vocoder: STFT.get_mel, nsf_hifigan/nvSTFT.py:73-117 (keyshift 0, speed 1) ----
  * audio [B, n_samples] -> mel [B, n_mels, n_frames], n_frames = b2d_mel_frames(...) (0 = signal too short):
  * reflect / constant padding by (win - hop)/2, frames of win_size = n_fft = 2048 at `hop`, periodic Hann `window` [2048],
