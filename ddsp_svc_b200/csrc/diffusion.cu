@@ -23,19 +23,8 @@
 
 namespace {
 
-__device__ __forceinline__ void df_emit(float v, float* __restrict__ hi, float* __restrict__ lo, size_t i) {
-    if (lo) {
-        float h, l;
-        tf32_split(v, h, l);
-        hi[i] = h;
-        lo[i] = l;
-    } else {
-        hi[i] = v;
-    }
-}
-
 __device__ __forceinline__ void df_emit4(const float (&v)[4], float* __restrict__ hi, float* __restrict__ lo, size_t i) {
-    for (int k = 0; k < 4; ++k) df_emit(v[k], hi, lo, i + k);
+    for (int k = 0; k < 4; ++k) tf32_emit(v[k], hi, lo, i + k);
 }
 
 // G: [n_tokens, C] (stage 0) or [n_tokens, 2 C] (stages 1, 2: a layer's output projection); h, skip [n_tokens, C].
@@ -151,7 +140,7 @@ __global__ void __launch_bounds__(256) df_update_kernel(const float* __restrict_
         }
         if (d_out) d_out[i] = d;
         if (x_out) x_out[i] = v;
-        if (hi) df_emit(v, hi, lo, i);
+        if (hi) tf32_emit(v, hi, lo, i);
     }
 }
 

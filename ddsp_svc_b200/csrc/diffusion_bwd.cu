@@ -25,18 +25,6 @@ namespace {
 
 constexpr int kDfSlab = kTokenSlab;      // rf_step_sums reads these slabs: the same constant as reflow_bwd.cu's
 
-__device__ __forceinline__ void dfb_emit(float v, float* __restrict__ hi, float* __restrict__ lo, size_t i) {
-    if (!hi) return;
-    if (lo) {
-        float h, l;
-        tf32_split(v, h, l);
-        hi[i] = h;
-        lo[i] = l;
-    } else {
-        hi[i] = v;
-    }
-}
-
 // x_t over [B T, M] (gt and noise token-major, t [B] int64 on the device): the reference's fp32 association, norm as
 // rf_start computes it, then two products and a sum, no contraction.  A step outside [0, n_steps) gives NaN.
 __global__ void __launch_bounds__(256) df_loss_input_kernel(const float* __restrict__ gt, const float* __restrict__ noise,
@@ -52,7 +40,7 @@ __global__ void __launch_bounds__(256) df_loss_input_kernel(const float* __restr
             const float x0 = ((gt[i] - spec_min) / spec_range) * 2.0f - 1.0f;          // diffusion.py:62 (norm_spec)
             v = __fadd_rn(__fmul_rn(__ldg(sqrt_ac + s), x0), __fmul_rn(__ldg(sqrt_1m_ac + s), noise[i]));
         }
-        dfb_emit(v, hi, lo, i);
+        tf32_emit_opt(v, hi, lo, i);
     }
 }
 
@@ -65,7 +53,7 @@ __global__ void __launch_bounds__(256) df_relu_bwd_kernel(const float* __restric
         const float x = pre[i] + __ldg(bias + (int)(i % C));
         const float r = x > 0.f ? gy[i] : 0.f;
         gx[i] = r;
-        dfb_emit(r, hi, lo, i);
+        tf32_emit_opt(r, hi, lo, i);
     }
 }
 
@@ -79,7 +67,7 @@ __global__ void __launch_bounds__(256) df_mish_bwd_kernel(const float* __restric
         const float sg = 1.0f / (1.0f + expf(-v));
         const float r = gy[i] * (th + v * sg * (1.0f - th * th));
         gx[i] = r;
-        dfb_emit(r, hi, lo, i);
+        tf32_emit_opt(r, hi, lo, i);
     }
 }
 
@@ -100,8 +88,8 @@ __global__ void __launch_bounds__(256) df_gate_bwd_kernel(const float* __restric
         const size_t k = tok * zcols + (size_t)layer * 2 * C + c;
         gz[k] = ra;
         gz[k + C] = rb;
-        dfb_emit(ra, gz_hi, gz_lo, k);
-        dfb_emit(rb, gz_hi, gz_lo, k + C);
+        tf32_emit_opt(ra, gz_hi, gz_lo, k);
+        tf32_emit_opt(rb, gz_hi, gz_lo, k + C);
     }
 }
 
@@ -138,8 +126,8 @@ __global__ void __launch_bounds__(256) df_layer_bwd_kernel(const float* __restri
                     const float a = h / kSqrt2, sk = gsk[i] / skip_div;
                     gr[k] = a;
                     gr[k + C] = sk;
-                    dfb_emit(a, gr_hi, gr_lo, k);
-                    dfb_emit(sk, gr_hi, gr_lo, k + C);
+                    tf32_emit_opt(a, gr_hi, gr_lo, k);
+                    tf32_emit_opt(sk, gr_hi, gr_lo, k + C);
                 }
             }
             if (gu) part[(size_t)item * LC + (size_t)layer * C + c] = acc;

@@ -21,17 +21,6 @@
 
 namespace {
 
-__device__ __forceinline__ void rf_emit(float v, float* __restrict__ hi, float* __restrict__ lo, size_t i) {
-    if (lo) {
-        float h, l;
-        tf32_split(v, h, l);
-        hi[i] = h;
-        lo[i] = l;
-    } else {
-        hi[i] = v;
-    }
-}
-
 // exact-erf GELU with torch's association: x * 0.5 * (1 + erf(x / sqrt 2))
 __device__ __forceinline__ float rf_gelu(float x) { return (x * 0.5f) * (1.0f + erff(x * 0.70710678118654752f)); }
 
@@ -51,7 +40,7 @@ __global__ void __launch_bounds__(256) rf_start_kernel(const float* __restrict__
             v = t_start * nrm + one_minus_t_start * v;
         }
         if (x) x[i] = v;
-        rf_emit(v, hi, lo, i);
+        tf32_emit(v, hi, lo, i);
     }
 }
 
@@ -80,7 +69,7 @@ __global__ void __launch_bounds__(256) rf_layer_input_kernel(const float4* __res
             const float4 cv = *reinterpret_cast<const float4*>(cond + tok * cond_stride + 4 * c4);
             r[0] = (r[0] + sv.x) + cv.x; r[1] = (r[1] + sv.y) + cv.y; r[2] = (r[2] + sv.z) + cv.z; r[3] = (r[3] + sv.w) + cv.w;
         }
-        for (int k = 0; k < 4; ++k) rf_emit(r[k], hi, lo, 4 * i + k);
+        for (int k = 0; k < 4; ++k) tf32_emit(r[k], hi, lo, 4 * i + k);
     }
 }
 
@@ -105,7 +94,7 @@ __global__ void __launch_bounds__(256) rf_ode_kernel(const float* __restrict__ g
             acc[i] = stage == 0 ? v : acc[i] + 2.0f * v;
             out = xv + (stage == 2 ? v * dt : (0.5f * v) * dt);
         }
-        rf_emit(out, hi, lo, i);
+        tf32_emit(out, hi, lo, i);
     }
 }
 

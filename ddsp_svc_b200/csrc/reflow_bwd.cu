@@ -25,18 +25,6 @@ namespace {
 
 constexpr int kRfSlab = kTokenSlab;      // frames of one utterance per slab of a token sum
 
-__device__ __forceinline__ void rfb_emit(float v, float* __restrict__ hi, float* __restrict__ lo, size_t i) {
-    if (!hi) return;
-    if (lo) {
-        float h, l;
-        tf32_split(v, h, l);
-        hi[i] = h;
-        lo[i] = l;
-    } else {
-        hi[i] = v;
-    }
-}
-
 // one thread per element of [B T, M]; x_t and target keep the reference's fp32 association (no contraction)
 __global__ void __launch_bounds__(256) rf_loss_input_kernel(const float* __restrict__ gt, const float* __restrict__ x0,
                                                             const float* __restrict__ t, float spec_min, float spec_range,
@@ -47,7 +35,7 @@ __global__ void __launch_bounds__(256) rf_loss_input_kernel(const float* __restr
         const float x1 = ((gt[i] - spec_min) / spec_range) * 2.0f - 1.0f;          // reflow.py:107-108
         const float a = x0[i], d = __fsub_rn(x1, a);                               // reflow.py:22
         target[i] = d;
-        rfb_emit(__fadd_rn(a, __fmul_rn(__ldg(t + b), d)), hi, lo, i);
+        tf32_emit_opt(__fadd_rn(a, __fmul_rn(__ldg(t + b), d)), hi, lo, i);
     }
 }
 
@@ -109,7 +97,7 @@ __global__ void __launch_bounds__(256) rf_loss_bwd_kernel(const float* __restric
         const float v = __fadd_rn(g[i], __ldg(bias + m));
         const float r = c * __fsub_rn(v, target[i]);
         gv[i] = r;
-        rfb_emit(r, hi, lo, i);
+        tf32_emit_opt(r, hi, lo, i);
     }
 }
 
@@ -124,7 +112,7 @@ __global__ void __launch_bounds__(256) rf_gelu_bwd_kernel(const float* __restric
         const float pdf = 0.39894228040143268f * expf(-0.5f * x * x);
         const float r = gy[i] * (cdf + x * pdf);
         gx[i] = r;
-        rfb_emit(r, hi, lo, i);
+        tf32_emit_opt(r, hi, lo, i);
     }
 }
 
@@ -145,9 +133,9 @@ __global__ void __launch_bounds__(256) rf_layer_bwd_kernel(const float* __restri
                 const size_t n = (size_t)b * T + t, i = n * D + c, k = n * LD + (size_t)layer * D + c;
                 const float v = gz[i], h = __fadd_rn(gh[i], v);
                 gh[i] = h;
-                rfb_emit(h, gh_hi, gh_lo, i);
+                tf32_emit_opt(h, gh_hi, gh_lo, i);
                 z[k] = v;
-                rfb_emit(v, z_hi, z_lo, k);
+                tf32_emit_opt(v, z_hi, z_lo, k);
                 acc += (double)v;
             }
             part[(size_t)item * LD + (size_t)layer * D + c] = acc;

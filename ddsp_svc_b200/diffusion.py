@@ -27,11 +27,11 @@ clipped to 0); here every B runs with the step clipped at 0.
 Training: with the denoiser's switch on (``WaveNet.diffusion_backward``; for NaiveV2Diff its own
 ``reflow_backward``), ``GaussianDiffusion(infer=False)`` returns the reference's loss (p_losses, loss_type 'l2', with
 the reference's draws of t and the noise) and WaveNet's forward under grad its prediction, both differentiable with
-respect to the denoiser's parameters and the condition: ONE autograd Function each, whose forward is the inference
-forward (same launches, bit-identical) plus the saved activations and whose backward walks the layers in reverse on the
-kernels of csrc/diffusion_bwd.cu (and reflow_bwd.cu's loss and step sums) and library GEMMs at ``gemm_precision``.
-NaiveV2Diff's backward is reflow._network_backward.  With the switch off (the default) infer=False and every call under
-grad raise NotImplementedError; with it on, the samplers under grad still do.
+respect to the denoiser's parameters and the condition: ONE autograd Function each, shared with NaiveV2Diff
+(denoiser.py), whose forward is the inference forward (same launches, bit-identical) plus the saved activations and
+whose backward, the denoiser's _backward, walks the layers in reverse -- WaveNet's on the kernels of csrc/diffusion_bwd.cu
+(and reflow_bwd.cu's loss and step sums) and library GEMMs at ``gemm_precision``.  With the switch off (the default)
+infer=False and every call under grad raise NotImplementedError; with it on, the samplers under grad still do.
 """
 import math
 
@@ -39,21 +39,16 @@ import numpy as np
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
-from torch.autograd.function import once_differentiable
 
 from . import _lib
+from .denoiser import _Adjoint, _DiffusionEmbedding, _Denoiser, _LossFunction, _step_adjoint, _under_grad, _weighted_mse
 from .ops import _need_cuda_f32, _stream
-from .reflow import NaiveV2Diff, _DiffusionEmbedding, _network_backward, _under_grad
-from .unit2control import _Gemm, _k, _split
+from .reflow import NaiveV2Diff
+from .unit2control import _Gemm, _k
 
 _NO_TRAINING = ("%s: training (p_losses and the denoiser's gradients) is off; turn it on with WaveNet.diffusion_backward "
                 "= True (NaiveV2Diff.reflow_backward = True for that denoiser), or run inference with infer=True under "
                 "torch.no_grad()")
-
-
-def _training_switch(fn):
-    """the denoiser's training switch: WaveNet.diffusion_backward, or NaiveV2Diff's own reflow_backward"""
-    return fn.diffusion_backward if isinstance(fn, WaveNet) else fn.reflow_backward
 
 
 class _ResidualBlock(nn.Module):                 # wavenet.py:31-62 (dilation 1 in every configuration)
@@ -67,177 +62,14 @@ class _ResidualBlock(nn.Module):                 # wavenet.py:31-62 (dilation 1 
         self.output_projection = nn.Conv1d(residual_channels, 2 * residual_channels, 1)
 
 
-def _wavenet_backward(mod, g, S, gv, gvs, want_cond):
-    """WaveNet's backward from gv [B T, M], the cotangent of its output (fp32), and gvs, that cotangent as the operand of
-    the output projection's adjoints.  S: what _velocity / _step_rows / _cond_rows saved.  -> (dict of parameter
-    gradients by name, the condition's cotangent [B T, n_hidden] or None).
-
-    Output side: the output projection's adjoints, df_relu_backward at the skip projection, its adjoints; every layer's
-    skip output receives the same cotangent (g_p W_skip) / sqrt(n_layers).  Per layer, reversed: g_R = [g_h' / sqrt 2 |
-    g_skip] (df_layer_backward writes it), the output projection's adjoints, df_gate_backward into column block i of
-    G_Z, the convolution's adjoints over the saved [B T, 3 C] operand, then df_layer_backward (the adjoint of the
-    operand's scatter, g_h, the next g_R, the step sums).  Every layer's condition projection then takes ONE pair of
-    GEMMs over G_Z [B T, n_layers 2 C], whose column sums are both the condition projection's and the convolution's bias
-    gradients; the step projections take the per-utterance token sums of g_y; the step MLP's GEMMs have B rows."""
-    P, (B, T) = S["P"], S["BT"]
-    L, C, N, dev, nL = _lib.lib(), mod.dim, B * T, gv.device, len(S["P"]["layers"])
-    LC, Z2, split = nL * C, nL * 2 * C, g.mode == "3xtf32"
-    ws_bytes = L.b2d_u2c_backward_workspace_bytes(B, T, 2 * C, max(mod.mel_channels, 4 * C, Z2))
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    rws_bytes = L.b2d_rf_backward_workspace_bytes(B, T, LC)
-    rws = torch.empty(rws_bytes, dtype=torch.uint8, device=dev)
-    new = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)
-    operand = lambda n, c, fp32: mod._operand(g, n, c, dev) if split else fp32
-    halves = lambda ops: mod._ptrs(ops) if split else (0, 0)           # fp32 modes: the fp32 tensor is the operand
-    cols = lambda ops, blk: tuple(o[:, blk] for o in ops) if split else ops[:, blk]
-
-    def colsum(x):
-        out = new(x.shape[1])
-        _k(L.b2d_u2c_colsum(x.data_ptr(), x.shape[0], x.shape[1], out.data_ptr(), ws.data_ptr(), ws_bytes, _stream()),
-           "b2d_u2c_colsum")
-        return out
-
-    def relu_backward(gy, pre, bias):
-        """-> (fp32 cotangent of ReLU(pre + bias)'s input, its operand)"""
-        gx = new(*gy.shape)
-        ops = operand(gy.shape[0], gy.shape[1], gx)
-        hi, lo = halves(ops)
-        _k(L.b2d_df_relu_backward(gy.data_ptr(), pre.data_ptr(), bias.data_ptr(), gy.shape[0], gy.shape[1], gx.data_ptr(),
-                                  hi, lo, _stream()), "b2d_df_relu_backward")
-        return gx, ops
-
-    w3 = lambda x: x.unsqueeze(-1)
-    G = {"output_projection.weight": w3(g.grad_weight(gvs, S["q"])), "output_projection.bias": colsum(gv)}
-    gp, gps = relu_backward(g.grad_input(gvs, P["out_w"]), S["S"], P["skip_b"])
-    G["skip_projection.weight"], G["skip_projection.bias"] = w3(g.grad_weight(gps, S["sk"])), colsum(gp)
-    gsk = g.grad_input(gps, P["skip_w"])                                 # [B T, C]; / sqrt(n_layers) in df_layer_backward
-    skip_div = math.sqrt(nL)
-    gh = new(N, C)
-    gr = new(N, 2 * C)
-    grs = operand(N, 2 * C, gr)
-    gr_hi, gr_lo = halves(grs)
-    _k(L.b2d_df_layer_backward(0, gh.data_ptr(), gsk.data_ptr(), skip_div, B, T, C, nL - 1, nL, gr.data_ptr(), gr_hi, gr_lo,
-                               0, 0, _stream()), "b2d_df_layer_backward")       # h_L feeds nothing: g_R = [0 | g_skip]
-    z = new(N, Z2)                                                       # G_Z: every layer's g_z
-    zs = operand(N, Z2, z)
-    z_hi, z_lo = halves(zs)
-    crows = S["crows"]
-    for i in reversed(range(nL)):
-        us, Zi, vs = S["layers"][i]
-        Ly, pre = P["layers"][i], "residual_layers.%d." % i
-        G[pre + "output_projection.weight"] = w3(g.grad_weight(grs, vs))
-        G[pre + "output_projection.bias"] = colsum(gr)
-        ga = g.grad_input(grs, Ly["out_w"])                              # [B T, C]: cotangent of the gate's output
-        _k(L.b2d_df_gate_backward(ga.data_ptr(), Zi.data_ptr(), crows.data_ptr() + 4 * i * 2 * C, Z2, N, C, i, nL,
-                                  z.data_ptr(), z_hi, z_lo, _stream()), "b2d_df_gate_backward")
-        gzs = cols(zs, slice(i * 2 * C, (i + 1) * 2 * C))
-        dW = g.grad_weight(gzs, us)                                      # [2 C, 3 C]: column block k is tap k
-        G[pre + "dilated_conv.weight"] = dW.reshape(2 * C, 3, C).permute(0, 2, 1).contiguous()
-        gu = g.grad_input(gzs, Ly["conv_w"])                             # [B T, 3 C]
-        nxt = i > 0
-        _k(L.b2d_df_layer_backward(gu.data_ptr(), gh.data_ptr(), gsk.data_ptr(), skip_div, B, T, C, i, nL,
-                                   gr.data_ptr() if nxt else 0, gr_hi if nxt else 0, gr_lo if nxt else 0, rws.data_ptr(),
-                                   rws_bytes, _stream()), "b2d_df_layer_backward")
-    # input projection: h_0 = ReLU(in_proj(x_t)); x_t is data
-    gpre, gpres = relu_backward(gh, S["pre"], P["in_b"])
-    G["input_projection.weight"], G["input_projection.bias"] = w3(g.grad_weight(gpres, S["xs"])), colsum(gpre)
-    # every layer's condition projection at once; its bias and the convolution's share G_Z's column sums
-    dcw, dcb = g.grad_weight(zs, S["cond"]), colsum(z)
-    g_cond = g.grad_input(zs, P["cond_w"]) if want_cond else None
-    # step projections from the per-utterance sums of g_y, then the step MLP (the sinusoidal embedding is data)
-    gS = new(B, LC)
-    _k(L.b2d_rf_step_sums(rws.data_ptr(), rws_bytes, B, T, LC, gS.data_ptr(), _stream()), "b2d_rf_step_sums")
-    gSs = g.split(gS)
-    dsw, dsb = g.grad_weight(gSs, g.split(S["e2"])), colsum(gS)
-    ge2 = g.grad_input(gSs, P["step_w"])                                 # [B, C]
-    ge2s = g.split(ge2)
-    G["mlp.2.weight"], G["mlp.2.bias"] = g.grad_weight(ge2s, g.split(S["a1"])), colsum(ge2)
-    ga1 = g.grad_input(ge2s, P["mlp2_w"])                                # [B, 4 C]
-    ge1 = new(*ga1.shape)
-    _k(L.b2d_df_mish_backward(ga1.data_ptr(), S["e1"].data_ptr(), ga1.numel(), ge1.data_ptr(), 0, 0, _stream()),
-       "b2d_df_mish_backward")
-    G["mlp.0.weight"], G["mlp.0.bias"] = g.grad_weight(g.split(ge1), g.split(S["e0"])), colsum(ge1)
-    for i in range(nL):
-        pre, zr, sr = "residual_layers.%d." % i, slice(i * 2 * C, (i + 1) * 2 * C), slice(i * C, (i + 1) * C)
-        G[pre + "conditioner_projection.weight"] = w3(dcw[zr])
-        G[pre + "conditioner_projection.bias"] = dcb[zr]
-        G[pre + "dilated_conv.bias"] = dcb[zr].clone()
-        G[pre + "diffusion_projection.weight"], G[pre + "diffusion_projection.bias"] = dsw[sr], dsb[sr]
-    return G, g_cond
-
-
-class _WaveNetFunction(torch.autograd.Function):
-    """WaveNet as ONE differentiable op: (module, parameter names, x [B, M, T], steps [B], cond [B, n_hidden, T],
-    *parameters) -> the predicted noise [B T, M] token-major.  forward is WaveNet._run as it stands (same launches, same
-    bits) plus the saved activations; backward is _wavenet_backward.  x and steps are data.  Not differentiable twice."""
-
-    @staticmethod
-    def forward(ctx, mod, names, x, steps, cond, *params):
-        S = {}
-        with _Gemm(mod.gemm_precision) as g:
-            v = mod._run(g, x, steps, cond, save=S)
-        ctx.mod, ctx.names, ctx.saved, ctx.cond_shape = mod, names, S, cond.shape
-        ctx.set_materialize_grads(False)
-        return v
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, gv):
-        if gv is None:
-            return (None,) * (5 + len(ctx.names))
-        mod, (B, Mc, T) = ctx.mod, ctx.cond_shape
-        with _Gemm(mod.gemm_precision) as g:
-            gv = gv.contiguous()
-            G, g_cond = _wavenet_backward(mod, g, ctx.saved, gv, g.split(gv), ctx.needs_input_grad[4])
-        g_cond = None if g_cond is None else g_cond.reshape(B, T, Mc).transpose(1, 2)
-        return (None, None, None, None, g_cond) + tuple(G.get(n) for n in ctx.names)
-
-
-class _DiffusionLossFunction(torch.autograd.Function):
-    """The diffusion loss with its denoiser (WaveNet or NaiveV2Diff) as ONE differentiable op: (diffusion, parameter
-    names, condition [B, T, M_cond], gt [B, T, M], t [B] int64, noise [B, T, M] token-major, *parameters) -> loss [].
-    forward is GaussianDiffusion._loss_forward (df_loss_input, the denoiser as its _velocity runs it, rf_loss with w = 1
-    and target = noise); backward is rf_loss_backward, which writes the output projection's operand directly, then
-    _wavenet_backward or reflow's _network_backward.  gt, t and noise are data.  Not differentiable twice."""
-
-    @staticmethod
-    def forward(ctx, diff, names, condition, gt, t, noise, *params):
-        S = {}
-        loss = diff._loss_forward(condition, gt, t, noise, save=S)
-        ctx.diff, ctx.names, ctx.saved = diff, names, S
-        ctx.set_materialize_grads(False)
-        return loss
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, gl):
-        if gl is None:
-            return (None,) * (6 + len(ctx.names))
-        mod, S = ctx.diff.denoise_fn, ctx.saved
-        (B, T), M, dev = S["BT"], mod.mel_channels, gl.device
-        gl = gl.reshape(1).to(torch.float32).contiguous()
-        with _Gemm(mod.gemm_precision) as g:
-            gv = torch.empty(B * T, M, dtype=torch.float32, device=dev)
-            gvs = mod._operand(g, B * T, M, dev) if g.mode == "3xtf32" else gv
-            hi, lo = mod._ptrs(gvs) if g.mode == "3xtf32" else (0, 0)
-            _k(_lib.lib().b2d_rf_loss_backward(S["G"].data_ptr(), S["P"]["out_b"].data_ptr(), S["target"].data_ptr(),
-                                               S["w"].data_ptr(), gl.data_ptr(), B, T, M, gv.data_ptr(), hi, lo, _stream()),
-               "b2d_rf_loss_backward")
-            backward = _wavenet_backward if isinstance(mod, WaveNet) else _network_backward
-            G, g_cond = backward(mod, g, S, gv, gvs, ctx.needs_input_grad[2])
-        g_cond = None if g_cond is None else g_cond.reshape(B, T, -1)
-        return (None, None, g_cond, None, None, None) + tuple(G.get(n) for n in ctx.names)
-
-
-class WaveNet(nn.Module):
-    #: precision of the library GEMMs, see unit2control._Gemm: "3xtf32" (default), "fp32", "tf32"
-    gemm_precision = "3xtf32"
+class WaveNet(_Denoiser):
     #: training: with grad mode on and a parameter (or cond) that requires grad, forward is differentiable with respect
     #: to the parameters and cond, and GaussianDiffusion(infer=False) around this network returns the diffusion loss,
-    #: differentiable with respect to the parameters and condition (the backward of _WaveNetFunction /
-    #: _DiffusionLossFunction; the forward issues the same kernels with the same results).  Off by default: every call
-    #: under grad and infer=False raise.  Set it on the class (``WaveNet.diffusion_backward = True``) or per instance.
+    #: differentiable with respect to the parameters and condition (the backward of denoiser._NetworkFunction /
+    #: _LossFunction; the forward issues the same kernels with the same results).  Off by default: every call under
+    #: grad and infer=False raise.  Set it on the class (``WaveNet.diffusion_backward = True``) or per instance.
     diffusion_backward = False
+    _name, _switch, _out_4d = "WaveNet", "diffusion_backward", True
 
     def __init__(self, in_dims=128, n_layers=20, n_chans=384, n_hidden=256):
         super().__init__()
@@ -258,14 +90,9 @@ class WaveNet(nn.Module):
         self.output_projection = nn.Conv1d(n_chans, in_dims, 1)
         nn.init.zeros_(self.output_projection.weight)
         self.mel_channels, self.condition_dim, self.dim = in_dims, n_hidden, n_chans
-        self.__dict__["_packed"] = None
 
-    # ---- weights in the layouts the GEMMs want, rebuilt when a parameter changes (load_state_dict, .to) ----
-    def _pack(self):
-        key = (self.gemm_precision,) + tuple((p.data_ptr(), p._version) for p in self.parameters())
-        c = self.__dict__.get("_packed")
-        if c is not None and c[0] == key:
-            return c[1]
+    def _layout(self):
+        """the weights in the layouts the GEMMs want (_Denoiser._pack caches them)"""
         d = lambda t: t.detach().contiguous()
         w2 = lambda conv: conv.weight.detach()[:, :, 0].contiguous()
         layers = self.residual_layers
@@ -283,11 +110,6 @@ class WaveNet(nn.Module):
         P["layers"] = [dict(conv_w=Ly.dilated_conv.weight.detach().permute(0, 2, 1).reshape(2 * self.dim, 3 * self.dim)
                             .contiguous(), out_w=w2(Ly.output_projection), out_b=d(Ly.output_projection.bias))
                        for Ly in layers]
-        if self.gemm_precision == "3xtf32":          # weights of every GEMM as TF32-exact (hi, lo) pairs, once per checkpoint
-            for dd in [P] + P["layers"]:
-                for name in [n for n in dd if n.endswith("_w")]:
-                    dd[name] = _split(dd[name])
-        self.__dict__["_packed"] = (key, P)
         return P
 
     # ---- the sampler's three operations (the same names and signatures as NaiveV2Diff's) ----
@@ -310,9 +132,6 @@ class WaveNet(nn.Module):
         if save is not None:
             save.update(cond=cs, crows=rows)
         return rows
-
-    _operand = staticmethod(NaiveV2Diff._operand)
-    _ptrs = staticmethod(NaiveV2Diff._ptrs)
 
     def _velocity(self, g, P, xs, steps, step_stride, conds, B, T, out_bias=None, save=None):
         """one evaluation of the denoiser: xs the input operand [B T, M] -> output projection [B T, M] (+ out_bias);
@@ -356,54 +175,89 @@ class WaveNet(nn.Module):
             save["q"] = vs
         return g.mm(vs, P["out_w"], out_bias)
 
-    def _run(self, g, x, steps, cond, save=None):
-        """x [B, M, T] contiguous, steps [B], cond [B, n_hidden, T] -> the predicted noise [B T, M] token-major (with the
-        output bias); ``save``: a dict that receives what the backward needs"""
-        B, M, T = x.shape
-        P = self._pack()
-        srows = self._step_rows(g, P, steps, save).contiguous()
-        crows = self._cond_rows(g, P, cond.transpose(1, 2).contiguous(), save)
-        xs = self._operand(g, B * T, M, x.device)
-        hi, lo = self._ptrs(xs)
-        _k(_lib.lib().b2d_rf_start(x.data_ptr(), 0, 0.0, 1.0, 0.0, 1.0, B, T, M, 0, hi, lo, _stream()), "b2d_rf_start")
-        if save is not None:
-            save.update(P=P, BT=(B, T))
-        return self._velocity(g, P, xs, srows, srows.shape[1], crows, B, T, out_bias=P["out_b"], save=save)
+    def _backward(self, g, S, gv, gvs, want_cond):
+        """WaveNet's backward from gv [B T, M], the cotangent of its output (fp32), and gvs, that cotangent as the
+        operand of the output projection's adjoints.  S: what _velocity / _step_rows / _cond_rows saved.  -> (dict of
+        parameter gradients by name, the condition's cotangent [B T, n_hidden] or None).
 
-    def _grad_params(self):
-        """(names, tensors) of the parameters the backward produces gradients for: all of them, in named_parameters order"""
-        items = list(self.named_parameters())
-        return tuple(n for n, _ in items), tuple(p for _, p in items)
+        Output side: the output projection's adjoints, df_relu_backward at the skip projection, its adjoints; every
+        layer's skip output receives the same cotangent (g_p W_skip) / sqrt(n_layers).  Per layer, reversed: g_R =
+        [g_h' / sqrt 2 | g_skip] (df_layer_backward writes it), the output projection's adjoints, df_gate_backward into
+        column block i of G_Z, the convolution's adjoints over the saved [B T, 3 C] operand, then df_layer_backward
+        (the adjoint of the operand's scatter, g_h, the next g_R, the step sums).  Every layer's condition projection
+        then takes ONE pair of GEMMs over G_Z [B T, n_layers 2 C], whose column sums are both the condition
+        projection's and the convolution's bias gradients; the step projections take the per-utterance token sums of
+        g_y; the step MLP's GEMMs have B rows."""
+        P, (B, T) = S["P"], S["BT"]
+        C, N, nL = self.dim, B * T, len(P["layers"])
+        LC, Z2 = nL * C, nL * 2 * C
+        A = _Adjoint(self, g, B, T, gv.device, 2 * C, max(self.mel_channels, 4 * C, Z2), LC)
+        L, new, operand, halves, colsum = A.L, A.new, A.operand, A.halves, A.colsum
+        cols = lambda ops, blk: tuple(o[:, blk] for o in ops) if A.split else ops[:, blk]
 
-    def forward(self, spec, diffusion_step, cond):
-        """spec [B, 1, M, T] or [B, M, T], diffusion_step [B] (or one value for every utterance), cond [B, n_hidden, T]
-        -> the predicted noise [B, 1, M, T] (wavenet.py:84-108).  Under grad (``diffusion_backward`` on):
-        differentiable with respect to the parameters and cond, bit-identical to the no_grad call; spec and
-        diffusion_step are data."""
-        grad = _under_grad(self, spec, diffusion_step, cond)
-        if grad and not self.diffusion_backward:
-            raise NotImplementedError(_NO_TRAINING % "WaveNet")
-        if grad:
-            for name, t in (("spec", spec), ("diffusion_step", diffusion_step)):
-                if torch.is_tensor(t) and t.requires_grad:
-                    raise NotImplementedError("WaveNet: no gradient with respect to %s (the diffusion loss does not need "
-                                              "it, so it is not built)" % name)
-        x = spec[:, 0] if spec.dim() == 4 else spec
-        _need_cuda_f32("spec", x)
-        _need_cuda_f32("cond", cond)
-        B, M, T = x.shape
-        if M != self.mel_channels or cond.shape != (B, self.condition_dim, T):
-            raise ValueError("WaveNet: spec [B, 1, %d, T] and cond [B, %d, T] expected, got %s and %s"
-                             % (self.mel_channels, self.condition_dim, tuple(spec.shape), tuple(cond.shape)))
-        steps = torch.as_tensor(diffusion_step, device=x.device).reshape(-1).expand(B)
-        x = x.contiguous()
-        if grad:
-            names, params = self._grad_params()
-            v = _WaveNetFunction.apply(self, names, x, steps.detach(), cond, *params)
-        else:
-            with torch.no_grad(), _Gemm(self.gemm_precision) as g:
-                v = self._run(g, x, steps, cond)
-        return v.reshape(B, T, M).transpose(1, 2).contiguous()[:, None]
+        def relu_backward(gy, pre, bias):
+            """-> (fp32 cotangent of ReLU(pre + bias)'s input, its operand)"""
+            gx = new(*gy.shape)
+            ops = operand(gy.shape[0], gy.shape[1], gx)
+            hi, lo = halves(ops)
+            _k(L.b2d_df_relu_backward(gy.data_ptr(), pre.data_ptr(), bias.data_ptr(), gy.shape[0], gy.shape[1],
+                                      gx.data_ptr(), hi, lo, _stream()), "b2d_df_relu_backward")
+            return gx, ops
+
+        def mish_backward(gy, pre):
+            """-> (fp32 cotangent of Mish(pre)'s input, its operand)"""
+            gx = new(*gy.shape)
+            _k(L.b2d_df_mish_backward(gy.data_ptr(), pre.data_ptr(), gy.numel(), gx.data_ptr(), 0, 0, _stream()),
+               "b2d_df_mish_backward")
+            return gx, g.split(gx)
+
+        w3 = lambda x: x.unsqueeze(-1)
+        G = {"output_projection.weight": w3(g.grad_weight(gvs, S["q"])), "output_projection.bias": colsum(gv)}
+        gp, gps = relu_backward(g.grad_input(gvs, P["out_w"]), S["S"], P["skip_b"])
+        G["skip_projection.weight"], G["skip_projection.bias"] = w3(g.grad_weight(gps, S["sk"])), colsum(gp)
+        gsk = g.grad_input(gps, P["skip_w"])                             # [B T, C]; / sqrt(n_layers) in df_layer_backward
+        skip_div = math.sqrt(nL)
+        gh = new(N, C)
+        gr = new(N, 2 * C)
+        grs = operand(N, 2 * C, gr)
+        gr_hi, gr_lo = halves(grs)
+        _k(L.b2d_df_layer_backward(0, gh.data_ptr(), gsk.data_ptr(), skip_div, B, T, C, nL - 1, nL, gr.data_ptr(), gr_hi,
+                                   gr_lo, 0, 0, _stream()), "b2d_df_layer_backward")    # h_L feeds nothing: g_R = [0 | g_skip]
+        z = new(N, Z2)                                                   # G_Z: every layer's g_z
+        zs = operand(N, Z2, z)
+        z_hi, z_lo = halves(zs)
+        crows = S["crows"]
+        for i in reversed(range(nL)):
+            us, Zi, vs = S["layers"][i]
+            Ly, pre = P["layers"][i], "residual_layers.%d." % i
+            G[pre + "output_projection.weight"] = w3(g.grad_weight(grs, vs))
+            G[pre + "output_projection.bias"] = colsum(gr)
+            ga = g.grad_input(grs, Ly["out_w"])                          # [B T, C]: cotangent of the gate's output
+            _k(L.b2d_df_gate_backward(ga.data_ptr(), Zi.data_ptr(), crows.data_ptr() + 4 * i * 2 * C, Z2, N, C, i, nL,
+                                      z.data_ptr(), z_hi, z_lo, _stream()), "b2d_df_gate_backward")
+            gzs = cols(zs, slice(i * 2 * C, (i + 1) * 2 * C))
+            dW = g.grad_weight(gzs, us)                                  # [2 C, 3 C]: column block k is tap k
+            G[pre + "dilated_conv.weight"] = dW.reshape(2 * C, 3, C).permute(0, 2, 1).contiguous()
+            gu = g.grad_input(gzs, Ly["conv_w"])                         # [B T, 3 C]
+            nxt = i > 0
+            _k(L.b2d_df_layer_backward(gu.data_ptr(), gh.data_ptr(), gsk.data_ptr(), skip_div, B, T, C, i, nL,
+                                       gr.data_ptr() if nxt else 0, gr_hi if nxt else 0, gr_lo if nxt else 0,
+                                       A.rws.data_ptr(), A.rws_bytes, _stream()), "b2d_df_layer_backward")
+        # input projection: h_0 = ReLU(in_proj(x_t)); x_t is data
+        gpre, gpres = relu_backward(gh, S["pre"], P["in_b"])
+        G["input_projection.weight"], G["input_projection.bias"] = w3(g.grad_weight(gpres, S["xs"])), colsum(gpre)
+        # every layer's condition projection at once; its bias and the convolution's share G_Z's column sums
+        dcw, dcb = g.grad_weight(zs, S["cond"]), colsum(z)
+        g_cond = g.grad_input(zs, P["cond_w"]) if want_cond else None
+        # step projections from the per-utterance sums of g_y, then the step MLP
+        dsw, dsb = _step_adjoint(A, S, P, G, mish_backward, ("mlp.0", "mlp.2"))
+        for i in range(nL):
+            pre, zr, sr = "residual_layers.%d." % i, slice(i * 2 * C, (i + 1) * 2 * C), slice(i * C, (i + 1) * C)
+            G[pre + "conditioner_projection.weight"] = w3(dcw[zr])
+            G[pre + "conditioner_projection.bias"] = dcb[zr]
+            G[pre + "dilated_conv.bias"] = dcb[zr].clone()
+            G[pre + "diffusion_projection.weight"], G[pre + "diffusion_projection.bias"] = dsw[sr], dsb[sr]
+        return G, g_cond
 
 
 # ---- the samplers' schedules and coefficients (host, float64 from the reference's fp32 tables) -----------------------------
@@ -606,7 +460,7 @@ class GaussianDiffusion(nn.Module):
         (B,)) with t_max = k_step, or self.k_step when k_step is None, then the noise as randn_like of the transposed
         [B, 1, M, T] view of norm(gt_spec), which is token-major in memory.  Differentiable with respect to the
         denoiser's parameters and condition; gt_spec is data."""
-        training = _training_switch(self.denoise_fn)
+        training = self.denoise_fn._trains()
         if not infer:
             if not training:
                 raise NotImplementedError(_NO_TRAINING % "GaussianDiffusion")
@@ -708,7 +562,7 @@ class GaussianDiffusion(nn.Module):
         Under grad: differentiable with respect to the denoiser's parameters and condition; otherwise the same value
         without saving activations"""
         fn, M = self.denoise_fn, self.out_dims
-        if not _training_switch(fn):
+        if not fn._trains():
             raise NotImplementedError(_NO_TRAINING % "GaussianDiffusion")
         for name, v in (("condition", condition), ("gt_spec", gt_spec), ("noise", noise)):
             _need_cuda_f32(name, v)
@@ -725,7 +579,7 @@ class GaussianDiffusion(nn.Module):
         args = (condition.contiguous(), gt_spec.contiguous(), t.contiguous(), noise.contiguous())
         if _under_grad(self, condition):
             names, params = fn._grad_params()
-            return _DiffusionLossFunction.apply(self, names, *args, *params)
+            return _LossFunction.apply(self, fn, names, args[0], args[1:], *params)
         with torch.no_grad():
             return self._loss_forward(*args)
 
@@ -749,11 +603,7 @@ class GaussianDiffusion(nn.Module):
                "b2d_df_loss_input")
             G = fn._velocity(g, P, xs, srows, srows.shape[1], crows, B, T, save=save)
             w = torch.ones(B, dtype=torch.float32, device=dev)
-            ws_bytes = L.b2d_rf_backward_workspace_bytes(B, T, M)
-            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-            loss = torch.empty((), dtype=torch.float32, device=dev)
-            _k(L.b2d_rf_loss(G.data_ptr(), P["out_b"].data_ptr(), noise.data_ptr(), w.data_ptr(), B, T, M, ws.data_ptr(),
-                             ws_bytes, loss.data_ptr(), _stream()), "b2d_rf_loss")
+            loss = _weighted_mse(G, P["out_b"], noise, w, B, T, M)
         if save is not None:
             save.update(P=P, BT=(B, T), G=G, target=noise, w=w)
         return loss

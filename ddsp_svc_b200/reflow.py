@@ -17,42 +17,23 @@ at ``gemm_precision`` (unit2control._Gemm: "3xtf32" default, "fp32", "tf32").
 
 Training: with ``NaiveV2Diff.reflow_backward`` on, ``RectifiedFlow(infer=False)`` returns the reference's reflow loss
 (loss_type 'l2_lognorm', the reference's draws of t and x_0) and NaiveV2Diff's forward under grad its velocity, both
-differentiable with respect to the velocity network's parameters and the condition: ONE autograd Function each, whose
-forward is the inference forward (same launches, bit-identical) plus the saved activations and whose backward walks the
-layers in reverse on the kernels of csrc/reflow_bwd.cu and unit2control_bwd.cu and library GEMMs at ``gemm_precision``.
+differentiable with respect to the velocity network's parameters and the condition: ONE autograd Function each, shared
+with WaveNet (denoiser.py), whose forward is the inference forward (same launches, bit-identical) plus the saved
+activations and whose backward, NaiveV2Diff._backward, walks the layers in reverse on the kernels of csrc/reflow_bwd.cu
+and unit2control_bwd.cu and library GEMMs at ``gemm_precision``.
 With the switch off (the default) infer=False and every call under grad raise NotImplementedError; with it on, the
 sampler under grad still does.
 """
-import math
-
 import torch
 import torch.nn as nn
-from torch.autograd.function import once_differentiable
 
 from . import _lib
+from .denoiser import _Adjoint, _DiffusionEmbedding, _Denoiser, _LossFunction, _step_adjoint, _under_grad, _weighted_mse
 from .ops import _need_cuda_f32, _stream
-from .unit2control import _ConvModule, _Gemm, _k, _split
+from .unit2control import _ConvModule, _Gemm, _k
 
 _NO_TRAINING = ("%s: training (the reflow loss and its gradients) is not built; run inference with infer=True under "
                 "torch.no_grad()")
-
-
-class _DiffusionEmbedding(nn.Module):
-    """parameter-free sinusoidal embedding (naive_v2_diff.py:15-29): index 0 of ``diffusion_embedding``"""
-
-    def __init__(self, dim):
-        super().__init__()
-        self.dim = dim
-
-    def forward(self, x):
-        """x [E] diffusion steps -> [E, dim] fp32.  The frequencies are the reference's fp32 values (it builds them from
-        an integer arange); argument, sin and cos are float64: the argument reaches 1000 rad, where an fp32 product alone
-        is off by up to 3e-5 rad.  A few hundred values per sampling call."""
-        half = self.dim // 2
-        scale = math.log(10000) / (half - 1)
-        freq = torch.exp(torch.arange(half, device=x.device) * -scale)
-        arg = x.double()[:, None] * freq.double()[None, :]
-        return torch.cat((arg.sin(), arg.cos()), dim=-1).float()
 
 
 class _Layer(nn.Module):                          # naive_v2_diff.py:32-98 with conv_only, no wavenet skip
@@ -64,166 +45,14 @@ class _Layer(nn.Module):                          # naive_v2_diff.py:32-98 with 
         self.condition_projection = nn.Conv1d(dim_cond, dim, 1)
 
 
-def _under_grad(module, *inputs):
-    return torch.is_grad_enabled() and (any(p.requires_grad for p in module.parameters()) or
-                                        any(torch.is_tensor(t) and t.requires_grad for t in inputs))
-
-
-def _network_backward(mod, g, S, gv, gvs, want_cond):
-    """The velocity network's backward from gv [B T, M], the cotangent of its output (fp32), and gvs, that cotangent as
-    the operand of the output projection's adjoints.  S: what _velocity / _step_rows / _cond_rows saved.  -> (dict of
-    parameter gradients by name, the condition's cotangent [B T, M_cond] or None).
-
-    Per layer, reversed: pw2's adjoints, the GLU-conv-SiLU backward recomputed from the saved pw1 output, pw1's adjoints,
-    then rf_layer_backward adds g_z into the residual stream's cotangent and into column block i of G_Z.  Every layer's
-    condition projection then takes ONE pair of GEMMs over G_Z [B T, n_layers dim], and the step projections the
-    per-utterance token sums of G_Z; the step MLP's GEMMs have B rows."""
-    P, (B, T) = S["P"], S["BT"]
-    L, D, N, dev, nL = _lib.lib(), mod.dim, B * T, gv.device, len(S["P"]["layers"])
-    LD, inner, split = nL * D, 2 * D, g.mode == "3xtf32"
-    ws_bytes = L.b2d_u2c_backward_workspace_bytes(B, T, inner, max(mod.mel_channels, 4 * D, LD))
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    rws_bytes = L.b2d_rf_backward_workspace_bytes(B, T, LD)
-    rws = torch.empty(rws_bytes, dtype=torch.uint8, device=dev)
-    new = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)
-    halves = lambda ops: mod._ptrs(ops) if split else (0, 0)       # fp32 modes: the fp32 tensor is the operand
-
-    def colsum(x):
-        out = new(x.shape[1])
-        _k(L.b2d_u2c_colsum(x.data_ptr(), x.shape[0], x.shape[1], out.data_ptr(), ws.data_ptr(), ws_bytes, _stream()),
-           "b2d_u2c_colsum")
-        return out
-
-    def gelu_backward(gy, pre, bias):
-        """-> (fp32 cotangent of GELU's input, its operand)"""
-        gx = new(*gy.shape)
-        ops = mod._operand(g, gy.shape[0], gy.shape[1], dev) if split else gx
-        hi, lo = halves(ops)
-        _k(L.b2d_rf_gelu_backward(gy.data_ptr(), pre.data_ptr(), 0 if bias is None else bias.data_ptr(), gy.shape[0],
-                                  gy.shape[1], gx.data_ptr(), hi, lo, _stream()), "b2d_rf_gelu_backward")
-        return gx, ops
-
-    G = {"output_projection.weight": g.grad_weight(gvs, S["hL"]).unsqueeze(-1), "output_projection.bias": colsum(gv)}
-    gh = g.grad_input(gvs, P["out_w"])                                   # [B T, dim]: cotangent of h_L
-    ghs = g.split(gh)
-    gh_hi, gh_lo = halves(ghs)
-    z = new(N, LD)                                                       # G_Z: every layer's g_z
-    zs = mod._operand(g, N, LD, dev) if split else z
-    z_hi, z_lo = halves(zs)
-    for i in reversed(range(nL)):
-        us, hh, ss = S["layers"][i]
-        Ly, net = P["layers"][i], "residual_layers.%d.conformer.net." % i
-        G[net + "6.weight"] = g.grad_weight(ghs, ss).unsqueeze(-1)
-        G[net + "6.bias"] = colsum(gh)
-        gs = g.grad_input(ghs, Ly["pw2_w"])                              # [B T, 2 dim]
-        ghh, dwb = new(N, 2 * inner), new(inner, 32)
-        _k(L.b2d_u2c_glu_dwconv_silu_backward(hh.data_ptr(), Ly["dw_w"].data_ptr(), Ly["dw_b"].data_ptr(), gs.data_ptr(),
-                                              ghh.data_ptr(), dwb.data_ptr(), B, T, inner, Ly["dw_w"].shape[1], ws.data_ptr(),
-                                              ws_bytes, _stream()), "b2d_u2c_glu_dwconv_silu_backward")
-        G[net + "4.weight"], G[net + "4.bias"] = dwb[:, :31].unsqueeze(1).contiguous(), dwb[:, 31].contiguous()
-        ghhs = g.split(ghh)
-        G[net + "2.weight"] = g.grad_weight(ghhs, us).unsqueeze(-1)
-        G[net + "2.bias"] = colsum(ghh)
-        gz = g.grad_input(ghhs, Ly["pw1_w"])                             # [B T, dim]: cotangent of z_i
-        _k(L.b2d_rf_layer_backward(gz.data_ptr(), gh.data_ptr(), B, T, D, i, nL, gh_hi, gh_lo, z.data_ptr(), z_hi, z_lo,
-                                   rws.data_ptr(), rws_bytes, _stream()), "b2d_rf_layer_backward")
-    # input projection: h_0 = GELU(in_proj(x_t)); x_t is data
-    gpre, gpres = gelu_backward(gh, S["pre"], P["in_b"])
-    G["input_projection.weight"] = g.grad_weight(gpres, S["xs"]).unsqueeze(-1)
-    G["input_projection.bias"] = colsum(gpre)
-    # every layer's condition projection at once
-    dcw, dcb = g.grad_weight(zs, S["cond"]), colsum(z)
-    g_cond = g.grad_input(zs, P["cond_w"]) if want_cond else None
-    # step projections from the per-utterance sums of G_Z, then the step MLP (the sinusoidal embedding is data)
-    gS = new(B, LD)
-    _k(L.b2d_rf_step_sums(rws.data_ptr(), rws_bytes, B, T, LD, gS.data_ptr(), _stream()), "b2d_rf_step_sums")
-    gSs = g.split(gS)
-    dsw, dsb = g.grad_weight(gSs, g.split(S["e2"])), colsum(gS)
-    ge2 = g.grad_input(gSs, P["step_w"])                                 # [B, dim]
-    ge2s = g.split(ge2)
-    G["diffusion_embedding.3.weight"] = g.grad_weight(ge2s, g.split(S["a1"]))
-    G["diffusion_embedding.3.bias"] = colsum(ge2)
-    ge1, ge1s = gelu_backward(g.grad_input(ge2s, P["mlp2_w"]), S["e1"], None)
-    G["diffusion_embedding.1.weight"] = g.grad_weight(ge1s, g.split(S["e0"]))
-    G["diffusion_embedding.1.bias"] = colsum(ge1)
-    for i in range(nL):
-        pre, rows = "residual_layers.%d." % i, slice(i * D, (i + 1) * D)
-        G[pre + "condition_projection.weight"], G[pre + "condition_projection.bias"] = dcw[rows].unsqueeze(-1), dcb[rows]
-        G[pre + "diffusion_step_projection.weight"] = dsw[rows].unsqueeze(-1)
-        G[pre + "diffusion_step_projection.bias"] = dsb[rows]
-    return G, g_cond
-
-
-class _VelocityFunction(torch.autograd.Function):
-    """NaiveV2Diff as ONE differentiable op: (module, parameter names, x [B, M, T], steps [B], cond [B, M_cond, T],
-    *parameters) -> v [B T, M] token-major.  forward is NaiveV2Diff._run as it stands (same launches, same bits) plus
-    the saved activations; backward is _network_backward.  x and steps are data.  Not differentiable twice."""
-
-    @staticmethod
-    def forward(ctx, mod, names, x, steps, cond, *params):
-        S = {}
-        with _Gemm(mod.gemm_precision) as g:
-            v = mod._run(g, x, steps, cond, save=S)
-        ctx.mod, ctx.names, ctx.saved, ctx.cond_shape = mod, names, S, cond.shape
-        ctx.set_materialize_grads(False)
-        return v
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, gv):
-        if gv is None:
-            return (None,) * (5 + len(ctx.names))
-        mod, (B, Mc, T) = ctx.mod, ctx.cond_shape
-        with _Gemm(mod.gemm_precision) as g:
-            gv = gv.contiguous()
-            G, g_cond = _network_backward(mod, g, ctx.saved, gv, g.split(gv), ctx.needs_input_grad[4])
-        g_cond = None if g_cond is None else g_cond.reshape(B, T, Mc).transpose(1, 2)
-        return (None, None, None, None, g_cond) + tuple(G.get(n) for n in ctx.names)
-
-
-class _ReflowLossFunction(torch.autograd.Function):
-    """The reflow loss with its velocity network as ONE differentiable op: (flow, parameter names, condition [B, T, M_cond],
-    gt [B, T, M], t [B], x0 [B, T, M], w [B], *parameters) -> loss [].  forward is RectifiedFlow._loss_forward (rf_loss_input,
-    the velocity network as NaiveV2Diff._velocity runs it, rf_loss); backward is rf_loss_backward, which writes the
-    output projection's operand directly, then _network_backward.  gt, t, x0 and w are data.  Not differentiable twice."""
-
-    @staticmethod
-    def forward(ctx, flow, names, condition, gt, t, x0, w, *params):
-        S = {}
-        loss = flow._loss_forward(condition, gt, t, x0, w, save=S)
-        ctx.flow, ctx.names, ctx.saved, ctx.w = flow, names, S, w
-        ctx.set_materialize_grads(False)
-        return loss
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, gl):
-        if gl is None:
-            return (None,) * (7 + len(ctx.names))
-        mod, S = ctx.flow.velocity_fn, ctx.saved
-        (B, T), M, dev = S["BT"], mod.mel_channels, gl.device
-        gl = gl.reshape(1).to(torch.float32).contiguous()
-        with _Gemm(mod.gemm_precision) as g:
-            gv = torch.empty(B * T, M, dtype=torch.float32, device=dev)
-            gvs = mod._operand(g, B * T, M, dev) if g.mode == "3xtf32" else gv
-            hi, lo = mod._ptrs(gvs) if g.mode == "3xtf32" else (0, 0)
-            _k(_lib.lib().b2d_rf_loss_backward(S["G"].data_ptr(), S["P"]["out_b"].data_ptr(), S["target"].data_ptr(),
-                                               ctx.w.data_ptr(), gl.data_ptr(), B, T, M, gv.data_ptr(), hi, lo, _stream()),
-               "b2d_rf_loss_backward")
-            G, g_cond = _network_backward(mod, g, S, gv, gvs, ctx.needs_input_grad[2])
-        g_cond = None if g_cond is None else g_cond.reshape(B, T, -1)
-        return (None, None, g_cond, None, None, None, None) + tuple(G.get(n) for n in ctx.names)
-
-
-class NaiveV2Diff(nn.Module):
-    #: precision of the library GEMMs, see unit2control._Gemm: "3xtf32" (default), "fp32", "tf32"
-    gemm_precision = "3xtf32"
+class NaiveV2Diff(_Denoiser):
     #: training: with grad mode on and a parameter (or cond) that requires grad, forward is differentiable with respect
     #: to the parameters and cond, and RectifiedFlow(infer=False) returns the reflow loss, differentiable with respect to
-    #: the parameters and condition (the backward of _VelocityFunction / _ReflowLossFunction; the forward issues the same
-    #: kernels with the same results).  Off by default: every call under grad and infer=False raise, and tests pin that.
-    #: Set it on the class (``NaiveV2Diff.reflow_backward = True``) or per instance.
+    #: the parameters and condition (the backward of denoiser._NetworkFunction / _LossFunction; the forward issues the
+    #: same kernels with the same results).  Off by default: every call under grad and infer=False raise, and tests pin
+    #: that.  Set it on the class (``NaiveV2Diff.reflow_backward = True``) or per instance.
     reflow_backward = False
+    _name, _switch = "NaiveV2Diff", "reflow_backward"
 
     def __init__(self, mel_channels=128, dim=512, use_mlp=True, mlp_factor=4, condition_dim=256, num_layers=20,
                  expansion_factor=2, kernel_size=31, conv_only=True, wavenet_like=False, use_norm=False,
@@ -252,14 +81,9 @@ class NaiveV2Diff(nn.Module):
         self.output_projection = nn.Conv1d(dim, mel_channels, 1)
         nn.init.zeros_(self.output_projection.weight)
         self.dim, self.mel_channels, self.condition_dim = dim, mel_channels, condition_dim
-        self.__dict__["_packed"] = None
 
-    # ---- weights in the layouts the GEMMs want, rebuilt when a parameter changes (load_state_dict, .to) ----
-    def _pack(self):
-        key = (self.gemm_precision,) + tuple((p.data_ptr(), p._version) for p in self.parameters())
-        c = self.__dict__.get("_packed")
-        if c is not None and c[0] == key:
-            return c[1]
+    def _layout(self):
+        """the weights in the layouts the GEMMs want (_Denoiser._pack caches them)"""
         w2 = lambda conv: conv.weight.detach()[:, :, 0].contiguous()
         layers = self.residual_layers
         P = dict(in_w=w2(self.input_projection), in_b=self.input_projection.bias.detach().contiguous(),
@@ -276,12 +100,12 @@ class NaiveV2Diff(nn.Module):
             P["layers"].append(dict(pw1_w=w2(net[2]), pw1_b=net[2].bias.detach(), dw_w=net[4].weight.detach()[:, 0, :].contiguous(),
                                     dw_b=net[4].bias.detach().contiguous(), pw2_w=w2(net[6]),
                                     pw2_b=net[6].bias.detach().contiguous()))
-        if self.gemm_precision == "3xtf32":          # weights of every GEMM as TF32-exact (hi, lo) pairs, once per checkpoint
-            for d in [P] + P["layers"]:
-                for name in [n for n in d if n.endswith("_w") and n != "dw_w"]:
-                    d[name] = _split(d[name].contiguous())
-        self.__dict__["_packed"] = (key, P)
         return P
+
+    def _has_grad(self, name):
+        """all but the layers' LayerNorms (in the reference's state dict, never used when conv_only: their gradients
+        stay None)"""
+        return not (name.startswith("residual_layers.") and ".norm." in name)
 
     # ---- building blocks ----
     def _step_rows(self, g, P, steps, save=None):
@@ -302,16 +126,6 @@ class NaiveV2Diff(nn.Module):
         if save is not None:
             save["cond"] = cs
         return g.mm(cs, P["cond_w"], P["cond_b"])
-
-    @staticmethod
-    def _operand(g, n, c, dev):
-        """a [n, c] GEMM operand buffer: (hi, lo) in 3xtf32 mode, one fp32 tensor otherwise"""
-        new = lambda: torch.empty(n, c, dtype=torch.float32, device=dev)
-        return (new(), new()) if g.mode == "3xtf32" else new()
-
-    @staticmethod
-    def _ptrs(xs):
-        return (xs[0].data_ptr(), xs[1].data_ptr()) if isinstance(xs, tuple) else (xs.data_ptr(), 0)
 
     def _velocity(self, g, P, xs, steps, step_stride, conds, B, T, out_bias=None, save=None):
         """one evaluation of the network: xs the input operand [B T, M] -> output projection [B T, M] (+ out_bias);
@@ -350,58 +164,71 @@ class NaiveV2Diff(nn.Module):
             save["hL"] = us
         return g.mm(us, P["out_w"], out_bias)
 
-    def _run(self, g, x, steps, cond, save=None):
-        """x [B, M, T] contiguous, steps [B], cond [B, M_cond, T] -> the velocity [B T, M] token-major (with the output
-        bias); ``save``: a dict that receives what the backward needs"""
-        B, M, T = x.shape
-        P = self._pack()
-        srows = self._step_rows(g, P, steps, save).contiguous()                          # [B, n_layers dim]
-        crows = self._cond_rows(g, P, cond.transpose(1, 2).contiguous(), save)
-        xs = self._operand(g, B * T, M, x.device)
-        hi, lo = self._ptrs(xs)
-        _k(_lib.lib().b2d_rf_start(x.data_ptr(), 0, 0.0, 1.0, 0.0, 1.0, B, T, M, 0, hi, lo, _stream()), "b2d_rf_start")
-        if save is not None:
-            save.update(P=P, BT=(B, T))
-        return self._velocity(g, P, xs, srows, srows.shape[1], crows, B, T, out_bias=P["out_b"], save=save)
+    def _backward(self, g, S, gv, gvs, want_cond):
+        """The velocity network's backward from gv [B T, M], the cotangent of its output (fp32), and gvs, that
+        cotangent as the operand of the output projection's adjoints.  S: what _velocity / _step_rows / _cond_rows
+        saved.  -> (dict of parameter gradients by name, the condition's cotangent [B T, M_cond] or None).
 
-    def _grad_params(self):
-        """(names, tensors) of the parameters the backward produces gradients for, in named_parameters order: all but the
-        layers' LayerNorms (in the reference's state dict, never used when conv_only: their gradients stay None)"""
-        items = [(n, p) for n, p in self.named_parameters() if not (n.startswith("residual_layers.") and ".norm." in n)]
-        return tuple(n for n, _ in items), tuple(p for _, p in items)
+        Per layer, reversed: pw2's adjoints, the GLU-conv-SiLU backward recomputed from the saved pw1 output, pw1's
+        adjoints, then rf_layer_backward adds g_z into the residual stream's cotangent and into column block i of G_Z.
+        Every layer's condition projection then takes ONE pair of GEMMs over G_Z [B T, n_layers dim], and the step
+        projections the per-utterance token sums of G_Z; the step MLP's GEMMs have B rows."""
+        P, (B, T) = S["P"], S["BT"]
+        D, N, nL = self.dim, B * T, len(P["layers"])
+        LD, inner = nL * D, 2 * D
+        A = _Adjoint(self, g, B, T, gv.device, inner, max(self.mel_channels, 4 * D, LD), LD)
+        L, new, halves, colsum = A.L, A.new, A.halves, A.colsum
 
-    def forward(self, spec, diffusion_step, cond):
-        """spec [B, 1, M, T] or [B, M, T], diffusion_step [B] (one step per utterance), cond [B, M_cond, T] -> the
-        velocity in the layout of spec.  Under grad (``reflow_backward`` on): differentiable with respect to the
-        parameters and cond, bit-identical to the no_grad call; spec and diffusion_step are data."""
-        grad = _under_grad(self, spec, diffusion_step, cond)
-        if grad and not self.reflow_backward:
-            raise NotImplementedError(_NO_TRAINING % "NaiveV2Diff")
-        if grad:
-            for name, t in (("spec", spec), ("diffusion_step", diffusion_step)):
-                if torch.is_tensor(t) and t.requires_grad:
-                    raise NotImplementedError("NaiveV2Diff: no gradient with respect to %s (the reflow loss does not need "
-                                              "it, so it is not built)" % name)
-        four = spec.dim() == 4
-        x = spec[:, 0] if four else spec
-        if x.dim() != 3:
-            raise ValueError("mel must be 3 dim tensor, but got %d" % x.dim())
-        _need_cuda_f32("spec", x)
-        _need_cuda_f32("cond", cond)
-        B, M, T = x.shape
-        if M != self.mel_channels or cond.shape != (B, self.condition_dim, T):
-            raise ValueError("NaiveV2Diff: spec [B, %d, T] and cond [B, %d, T] expected, got %s and %s"
-                             % (self.mel_channels, self.condition_dim, tuple(x.shape), tuple(cond.shape)))
-        steps = torch.as_tensor(diffusion_step, device=x.device).reshape(-1).expand(B)
-        x = x.contiguous()
-        if grad:
-            names, params = self._grad_params()
-            v = _VelocityFunction.apply(self, names, x, steps.detach(), cond, *params)
-        else:
-            with torch.no_grad(), _Gemm(self.gemm_precision) as g:
-                v = self._run(g, x, steps, cond)
-        v = v.reshape(B, T, M).transpose(1, 2).contiguous()
-        return v[:, None] if four else v
+        def gelu_backward(gy, pre, bias):
+            """-> (fp32 cotangent of GELU's input, its operand)"""
+            gx = new(*gy.shape)
+            ops = A.operand(gy.shape[0], gy.shape[1], gx)
+            hi, lo = halves(ops)
+            _k(L.b2d_rf_gelu_backward(gy.data_ptr(), pre.data_ptr(), 0 if bias is None else bias.data_ptr(), gy.shape[0],
+                                      gy.shape[1], gx.data_ptr(), hi, lo, _stream()), "b2d_rf_gelu_backward")
+            return gx, ops
+
+        G = {"output_projection.weight": g.grad_weight(gvs, S["hL"]).unsqueeze(-1), "output_projection.bias": colsum(gv)}
+        gh = g.grad_input(gvs, P["out_w"])                                   # [B T, dim]: cotangent of h_L
+        ghs = g.split(gh)
+        gh_hi, gh_lo = halves(ghs)
+        z = new(N, LD)                                                       # G_Z: every layer's g_z
+        zs = A.operand(N, LD, z)
+        z_hi, z_lo = halves(zs)
+        for i in reversed(range(nL)):
+            us, hh, ss = S["layers"][i]
+            Ly, net = P["layers"][i], "residual_layers.%d.conformer.net." % i
+            G[net + "6.weight"] = g.grad_weight(ghs, ss).unsqueeze(-1)
+            G[net + "6.bias"] = colsum(gh)
+            gs = g.grad_input(ghs, Ly["pw2_w"])                              # [B T, 2 dim]
+            ghh, dwb = new(N, 2 * inner), new(inner, 32)
+            _k(L.b2d_u2c_glu_dwconv_silu_backward(hh.data_ptr(), Ly["dw_w"].data_ptr(), Ly["dw_b"].data_ptr(),
+                                                  gs.data_ptr(), ghh.data_ptr(), dwb.data_ptr(), B, T, inner,
+                                                  Ly["dw_w"].shape[1], A.ws.data_ptr(), A.ws_bytes, _stream()),
+               "b2d_u2c_glu_dwconv_silu_backward")
+            G[net + "4.weight"], G[net + "4.bias"] = dwb[:, :31].unsqueeze(1).contiguous(), dwb[:, 31].contiguous()
+            ghhs = g.split(ghh)
+            G[net + "2.weight"] = g.grad_weight(ghhs, us).unsqueeze(-1)
+            G[net + "2.bias"] = colsum(ghh)
+            gz = g.grad_input(ghhs, Ly["pw1_w"])                             # [B T, dim]: cotangent of z_i
+            _k(L.b2d_rf_layer_backward(gz.data_ptr(), gh.data_ptr(), B, T, D, i, nL, gh_hi, gh_lo, z.data_ptr(), z_hi,
+                                       z_lo, A.rws.data_ptr(), A.rws_bytes, _stream()), "b2d_rf_layer_backward")
+        # input projection: h_0 = GELU(in_proj(x_t)); x_t is data
+        gpre, gpres = gelu_backward(gh, S["pre"], P["in_b"])
+        G["input_projection.weight"] = g.grad_weight(gpres, S["xs"]).unsqueeze(-1)
+        G["input_projection.bias"] = colsum(gpre)
+        # every layer's condition projection at once
+        dcw, dcb = g.grad_weight(zs, S["cond"]), colsum(z)
+        g_cond = g.grad_input(zs, P["cond_w"]) if want_cond else None
+        # step projections from the per-utterance sums of G_Z, then the step MLP
+        dsw, dsb = _step_adjoint(A, S, P, G, lambda gy, pre: gelu_backward(gy, pre, None),
+                                 ("diffusion_embedding.1", "diffusion_embedding.3"))
+        for i in range(nL):
+            pre, rows = "residual_layers.%d." % i, slice(i * D, (i + 1) * D)
+            G[pre + "condition_projection.weight"], G[pre + "condition_projection.bias"] = dcw[rows].unsqueeze(-1), dcb[rows]
+            G[pre + "diffusion_step_projection.weight"] = dsw[rows].unsqueeze(-1)
+            G[pre + "diffusion_step_projection.bias"] = dsb[rows]
+        return G, g_cond
 
 
 class RectifiedFlow(nn.Module):
@@ -522,7 +349,7 @@ class RectifiedFlow(nn.Module):
         args = (condition.contiguous(), gt_spec.contiguous(), t.contiguous(), x0.contiguous(), w.contiguous())
         if _under_grad(self, condition):
             names, params = fn._grad_params()
-            return _ReflowLossFunction.apply(self, names, *args, *params)
+            return _LossFunction.apply(self, fn, names, args[0], args[1:], *params)
         with torch.no_grad():
             return self._loss_forward(*args)
 
@@ -542,11 +369,7 @@ class RectifiedFlow(nn.Module):
                                    float(self.spec_max - self.spec_min), B, T, M, target.data_ptr(), hi, lo, _stream()),
                "b2d_rf_loss_input")
             G = fn._velocity(g, P, xs, srows, srows.shape[1], crows, B, T, save=save)
-            ws_bytes = L.b2d_rf_backward_workspace_bytes(B, T, M)
-            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-            loss = torch.empty((), dtype=torch.float32, device=dev)
-            _k(L.b2d_rf_loss(G.data_ptr(), P["out_b"].data_ptr(), target.data_ptr(), w.data_ptr(), B, T, M, ws.data_ptr(),
-                             ws_bytes, loss.data_ptr(), _stream()), "b2d_rf_loss")
+            loss = _weighted_mse(G, P["out_b"], target, w, B, T, M)
         if save is not None:
-            save.update(P=P, BT=(B, T), G=G, target=target)
+            save.update(P=P, BT=(B, T), G=G, target=target, w=w)
         return loss

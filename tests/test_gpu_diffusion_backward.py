@@ -1,5 +1,5 @@
 """The diffusion loss and the WaveNet denoiser's CUDA backward (csrc/diffusion_bwd.cu + reflow_bwd.cu's loss + library
-GEMMs, ddsp_svc_b200/diffusion.py: _DiffusionLossFunction, _WaveNetFunction) on the GPU:
+GEMMs, ddsp_svc_b200/diffusion.py and denoiser.py: _LossFunction, _NetworkFunction) on the GPU:
 
 * the diffusion-new.yaml network (WaveNet(128, 20, 512, 256)) at its training batch (36 x 172) and at 1 x 861, and the
   diffusion-fast.yaml denoiser (NaiveV2Diff(512, 6 layers)) inside GaussianDiffusion at 48 x 172, against float64

@@ -1,5 +1,5 @@
-"""The reflow loss and the velocity network's CUDA backward (csrc/reflow_bwd.cu + library GEMMs, ddsp_svc_b200/reflow.py:
-_ReflowLossFunction, _VelocityFunction) on the GPU:
+"""The reflow loss and the velocity network's CUDA backward (csrc/reflow_bwd.cu + library GEMMs, ddsp_svc_b200/reflow.py
+and denoiser.py: _LossFunction, _NetworkFunction) on the GPU:
 
 * the reference's own loss and float64 gradients replayed (tests/golden/reflow_grad_*.npz) in the three GEMM modes;
 * the 512-wide, 6-layer network of configs/reflow.yaml at its training batch (48 x 172) and at 1 x 861, against float64
