@@ -388,3 +388,46 @@ extern "C" int b2d_combsub_synth(const float* f0_frames, const double* frame_pha
     return b2d::ltv_fir_launch(allp, ir_h, Lh, harmonic, nullptr, nullptr, 0, nullptr, nbuf, signal, seed,
                                utterance_offset, B, n_frames, block, st);
 }
+
+// ---------------------------------------------------------------------------------------
+// NSF-HiFiGAN generator (nsf_hifigan/models.py:207-273): the kernels of hifigan.cu
+// ---------------------------------------------------------------------------------------
+namespace b2d {
+int hifigan_conv_launch(const float* x, int64_t sb, int64_t st, int64_t sc, int B, int T, int Cin, const float* w,
+                        const float* bias, int k, int dil, int N, int lrelu, const float* residual, const float* accum,
+                        float div, int up, const float* src, const float* wn, const float* bn, int n_k, int n_stride,
+                        int n_pad, float* out, cudaStream_t stream);
+int hifigan_post_launch(const float* x, const float* w, const float* bias, int B, int T, int C, float* out, cudaStream_t stream);
+}  // namespace b2d
+
+extern "C" int b2d_hifigan_conv(const float* x, int64_t x_stride_b, int64_t x_stride_t, int64_t x_stride_c, int B, int T,
+                                int C_in, const float* w, const float* bias, int k, int dilation, int N, int lrelu,
+                                const float* residual, const float* accum, float div, int up, const float* source,
+                                const float* noise_w, const float* noise_b, int noise_k, int noise_stride, int noise_pad,
+                                float* out, void* stream) {
+    if (!x || !w || !bias || !out || (source && (!noise_w || !noise_b)))
+        return b2d::fail(B2D_ERR_NULL, "hifigan_conv: null pointer");
+    if (B <= 0 || T <= 0 || C_in <= 0 || N <= 0 || k <= 0 || dilation <= 0 || !(div > 0.f) || up < 0 ||
+        (up && N % up) || (source && (noise_k <= 0 || noise_stride <= 0 || noise_pad < 0)))
+        return b2d::fail(B2D_ERR_SHAPE, "hifigan_conv: bad shape");
+    if (k % 2 == 0 || C_in % 16 || N % 16 || (up && ((N / up) % 2 || residual || accum)) || (!up && source) ||
+        B > 65535 || (long long)dilation * (k - 1) / 2 > 256)
+        return b2d::fail(B2D_ERR_UNSUPPORTED, "hifigan_conv: needs odd k, a halo of <= 256 rows, C_in and N multiples of "
+                                              "16, an even C_out, no residual / accum with up, no source without");
+    if (x_stride_c == 1 && (!b2d::aligned16(x) || x_stride_t % 4 || x_stride_b % 4))
+        return b2d::fail(B2D_ERR_ALIGN, "hifigan_conv: a unit channel stride needs 16-byte aligned x and strides");
+    if (!b2d::aligned16(w) || (reinterpret_cast<uintptr_t>(bias) & 7u) || (reinterpret_cast<uintptr_t>(out) & 7u) ||
+        (residual && (reinterpret_cast<uintptr_t>(residual) & 7u)) || (accum && (reinterpret_cast<uintptr_t>(accum) & 7u)))
+        return b2d::fail(B2D_ERR_ALIGN, "hifigan_conv: w 16-byte, bias / out / residual / accum 8-byte aligned");
+    return b2d::hifigan_conv_launch(x, x_stride_b, x_stride_t, x_stride_c, B, T, C_in, w, bias, k, dilation, N, lrelu,
+                                    residual, accum, div, up, source, noise_w, noise_b, noise_k, noise_stride, noise_pad,
+                                    out, (cudaStream_t)stream);
+}
+
+extern "C" int b2d_hifigan_post(const float* x, const float* w, const float* bias, int B, int T, int C, float* out, void* stream) {
+    if (!x || !w || !bias || !out) return b2d::fail(B2D_ERR_NULL, "hifigan_post: null pointer");
+    if (B <= 0 || T <= 0 || C <= 0) return b2d::fail(B2D_ERR_SHAPE, "hifigan_post: bad shape");
+    if (C % 4 || C > 4096) return b2d::fail(B2D_ERR_UNSUPPORTED, "hifigan_post: C must be a multiple of 4, <= 4096");
+    if (!b2d::aligned16(x)) return b2d::fail(B2D_ERR_ALIGN, "hifigan_post: x must be 16-byte aligned");
+    return b2d::hifigan_post_launch(x, w, bias, B, T, C, out, (cudaStream_t)stream);
+}

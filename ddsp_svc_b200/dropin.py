@@ -113,7 +113,7 @@ def _patch_diffusion(saved):
                 setattr(mod, name, ours[name])
 
 
-def patch_reference(reflow=False, diffusion=False):
+def patch_reference(reflow=False, diffusion=False, hifigan=False):
     """Swap the synthesizer classes inside the (importable) reference package.  Returns the dict
     of original classes so a caller can restore them; its keys say what was patched.  If the enhancer stack
     (nsf_hifigan.models) cannot be imported, only the synthesizers are patched and the reason is returned under
@@ -133,7 +133,12 @@ def patch_reference(reflow=False, diffusion=False):
     also set ``ddsp_svc_b200.WaveNet.diffusion_backward = True`` (diffusion.yaml, diffusion-new.yaml) or
     ``ddsp_svc_b200.NaiveV2Diff.reflow_backward = True`` (diffusion-fast.yaml): then ``GaussianDiffusion(infer=False)``
     returns the diffusion loss with its backward (DESIGN.md section 4.15b); without them infer=False and calls under
-    grad raise NotImplementedError.  The samplers under grad raise in any case."""
+    grad raise NotImplementedError.  The samplers under grad raise in any case.
+
+    ``hifigan=True`` rebinds ``nsf_hifigan.models.Generator`` to ``ddsp_svc_b200.Generator``.  ``load_model`` looks the
+    name up when it is called, so the enhancer (enhancer.py) and the diffusion and reflow vocoders (diffusion/vocoder.py,
+    reflow/vocoder.py), which import ``load_model`` by name, all build the package's generator and vocode on the kernels.
+    Off by default; needs nsf_hifigan.models to import (reported under ``"_not_patched"`` otherwise)."""
     import ddsp.vocoder as ref_vocoder          # the reference checkout must be on sys.path
     names = ("Sins", "CombSub", "CombSubSuperFast", "CombSubFast")
     saved = {name: getattr(ref_vocoder, name) for name in names}
@@ -159,6 +164,10 @@ def patch_reference(reflow=False, diffusion=False):
         saved["SourceModuleHnNSF"] = ref_nsf.SourceModuleHnNSF
         ref_nsf.SineGen = sinegen.SineGen
         ref_nsf.SourceModuleHnNSF = sinegen.SourceModuleHnNSF
+        if hifigan:
+            from .hifigan import Generator
+            saved["Generator"] = ref_nsf.Generator
+            ref_nsf.Generator = Generator
     if reflow:
         _patch_reflow(saved)
     if diffusion:
@@ -179,6 +188,8 @@ def unpatch_reference(saved):
         ref_nsf.SineGen = saved["SineGen"]
         if "SourceModuleHnNSF" in saved:
             ref_nsf.SourceModuleHnNSF = saved["SourceModuleHnNSF"]
+        if "Generator" in saved:
+            ref_nsf.Generator = saved["Generator"]
     if "NaiveV2Diff" in saved or "RectifiedFlow" in saved:
         for modname in _REFLOW_MODULES:
             mod = sys.modules.get(modname)

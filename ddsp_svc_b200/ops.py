@@ -755,3 +755,62 @@ def set_sins_impl(name):
     global _sins_impl
     _lib.check(_lib.lib().b2d_set_sins_impl({"auto": 0, "split": 1, "fused": 2, "spectrum": 3}[name]), "b2d_set_sins_impl")
     _sins_impl = name
+
+
+def hifigan_conv(x, w, bias, k, dilation, n_out, lrelu, residual=None, accum=None, div=1.0, up=0, source=None,
+                 noise_w=None, noise_b=None, noise_stride=1, noise_pad=0, out=None):
+    """One NSF-HiFiGAN convolution (b2d_hifigan_conv): x a [B, T, C_in] view with any strides -> out [B, T, n_out]
+    = (conv(leaky_relu(x, 0.1) if lrelu else x) + bias (+ residual) (+ accum)) / div, or with up = u the polyphase
+    transposed convolution -> [B, T u, n_out / u] plus the noise_convs term of ``source`` [B, T u noise_stride, 1].
+    ``w`` is packed by hifigan.pack_conv / pack_transposed; ``out`` may be residual or accum."""
+    _need_cuda_f32("x", x)
+    B, T, Cin = x.shape
+    for name, t in (("w", w), ("bias", bias), ("residual", residual), ("accum", accum), ("source", source),
+                    ("noise_w", noise_w), ("noise_b", noise_b), ("out", out)):
+        if t is not None:
+            _need_cuda_f32(name, t)
+            if not t.is_contiguous():
+                raise ValueError("%s must be contiguous" % name)
+    if w.numel() != 2 * k * Cin * n_out:
+        raise ValueError("w must hold 2 k C_in N = %d floats, got %d" % (2 * k * Cin * n_out, w.numel()))
+    shape = (B, T, n_out) if not up else (B, T * up, n_out // up)
+    for name, t in (("residual", residual), ("accum", accum)):
+        if t is not None and tuple(t.shape) != shape:
+            raise ValueError("%s must be %s, got %s" % (name, shape, tuple(t.shape)))
+    noise_k = 0
+    if source is not None:
+        if source.numel() != B * shape[1] * noise_stride:
+            raise ValueError("source must hold B T_out noise_stride = %d samples" % (B * shape[1] * noise_stride))
+        noise_k = noise_w.shape[-1]
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float32, device=x.device)
+    elif tuple(out.shape) != shape:
+        raise ValueError("out must be %s, got %s" % (shape, tuple(out.shape)))
+    # the stride of a size-1 dimension is never followed; 0 keeps it from failing the kernel's alignment rule
+    sb, st, sc = (0 if n == 1 else s for n, s in zip(x.shape, x.stride()))
+    if sc == 1 and (x.data_ptr() % 16 or st % 4 or sb % 4):
+        x = x.contiguous()
+        sb, st, sc = T * Cin, Cin, 1
+    rc = _lib.lib().b2d_hifigan_conv(x.data_ptr(), sb, st, sc, B, T, Cin, w.data_ptr(), bias.data_ptr(), int(k),
+                                     int(dilation), int(n_out), int(bool(lrelu)), _ptr(residual), _ptr(accum),
+                                     float(div), int(up), _ptr(source), _ptr(noise_w), _ptr(noise_b), int(noise_k),
+                                     int(noise_stride), int(noise_pad), out.data_ptr(), _stream())
+    _lib.check(rc, "b2d_hifigan_conv")
+    _count(1)
+    return out
+
+
+def hifigan_post(x, w, bias):
+    """tanh(Conv1d(C -> 1, 7, padding 3)(leaky_relu(x, 0.01)) + bias): x [B, T, C] token-major, w [7, C] tap-major,
+    bias [1] on the device -> [B, 1, T] (b2d_hifigan_post)."""
+    _need_cuda_f32("x", x)
+    _need_cuda_f32("w", w)
+    _need_cuda_f32("bias", bias)
+    B, T, C = x.shape
+    if not x.is_contiguous() or not w.is_contiguous() or w.numel() != 7 * C:
+        raise ValueError("x must be a contiguous [B, T, C] tensor and w a contiguous [7, C] one")
+    out = torch.empty(B, 1, T, dtype=torch.float32, device=x.device)
+    _lib.check(_lib.lib().b2d_hifigan_post(x.data_ptr(), w.data_ptr(), bias.data_ptr(), B, T, C, out.data_ptr(),
+                                           _stream()), "b2d_hifigan_post")
+    _count(1)
+    return out

@@ -554,6 +554,28 @@ int b2d_rss_loss_backward(const float* x_pred, const float* x_true, int B, int n
                           const float* const* tables, float alpha, float eps, const double* norms, const float* grad_loss,
                           float* grad_pred, void* stream);
 
+/* ---- NSF-HiFiGAN generator (nsf_hifigan/models.py:207-273), inference (hifigan.cu) -------------------------------------
+ * b2d_hifigan_conv: one Conv1d(C_in -> N, k, dilation, padding dilation (k - 1) / 2) as an implicit GEMM on the tensor
+ *   cores, 3xTF32.  x element (b, t, c) at x[b x_stride_b + t x_stride_t + c x_stride_c] (token-major [B, T, C_in], or
+ *   any strided view such as a channel-major mel), zero padding at each utterance's edges.  w: the weights split into
+ *   TF32 (hi, lo) in mma.sync B-fragment order, [k][C_in / 8][N / 8][32 lanes][4] with lane 4 g + t holding the hi
+ *   halves of W[8 nb + g, 8 kb + t, j] and W[8 nb + g, 8 kb + t + 4, j], then their lo halves
+ *   (ddsp_svc_b200.hifigan.pack_conv).  lrelu != 0: leaky_relu(x, 0.1) first.
+ *   up == 0: out [B, T, N] = (conv + bias[N] (+ residual) (+ accum)) / div; out may alias residual or accum.
+ *   up == u > 0: the polyphase form of ConvTranspose1d(C_in, C_out = N / u, 2u, u, u / 2) (hifigan.pack_transposed):
+ *   out [B, T u, C_out], element (t u + r, co) = column r C_out + co + bias[co], plus with source [B, T u noise_stride]
+ *   the strided dot noise_b[co] + sum_{q < noise_k} noise_w[co, q] source[(t u + r) noise_stride - noise_pad + q]
+ *   (zero outside), i.e. noise_convs[i](har_source).  k odd, C_in and N multiples of 16, C_out even, halo
+ *   dilation (k - 1) / 2 <= 256; a unit channel stride needs x and its strides 16-byte aligned.
+ * b2d_hifigan_post: out [B, 1, T] = tanh(bias[0] + Conv1d(C -> 1, 7, padding 3)(leaky_relu(x, 0.01))), x [B, T, C]
+ *   token-major (16-byte aligned, C a multiple of 4), w [7][C] (tap-major).
+ * No atomics: bit-identical from run to run. */
+int b2d_hifigan_conv(const float* x, int64_t x_stride_b, int64_t x_stride_t, int64_t x_stride_c, int B, int T, int C_in,
+                     const float* w, const float* bias, int k, int dilation, int N, int lrelu, const float* residual,
+                     const float* accum, float div, int up, const float* source, const float* noise_w,
+                     const float* noise_b, int noise_k, int noise_stride, int noise_pad, float* out, void* stream);
+int b2d_hifigan_post(const float* x, const float* w, const float* bias, int B, int T, int C, float* out, void* stream);
+
 /* b2d_sins_synth variants.  0 (default) = 1 = oscillator-bank kernel next to the impulse-response builds, then the FIR
  * kernel transforms the impulse responses itself.  2 = the bank is evaluated inside the FFT-domain FIR kernel (additionally <= 128 harmonics):
  * no [B, T] sinusoid tensor, one launch less, kept as a tested alternative (see api.cu).
