@@ -431,3 +431,98 @@ extern "C" int b2d_hifigan_post(const float* x, const float* w, const float* bia
     if (!b2d::aligned16(x)) return b2d::fail(B2D_ERR_ALIGN, "hifigan_post: x must be 16-byte aligned");
     return b2d::hifigan_post_launch(x, w, bias, B, T, C, out, (cudaStream_t)stream);
 }
+
+// ---------------------------------------------------------------------------------------------------------------------
+// RMVPE pitch extractor (encoder/rmvpe/), inference: the kernels of rmvpe.cu
+// ---------------------------------------------------------------------------------------------------------------------
+namespace b2d {
+int rmvpe_conv_launch(const float* x, int ldx, int B, int T, int F, int Cin, const float* w, const float* bias, int k,
+                      int N, int n_valid, int act, int up, const float* res, int ldr, float* out, int ldo,
+                      cudaStream_t stream);
+int rmvpe_conv_small_launch(const float* x, int64_t sb, int64_t st, int64_t sf, int64_t sc, int B, int T, int F, int Cin,
+                            const float* in_scale, const float* in_shift, const float* w, const float* bias, int k,
+                            int Cout, int act, int head, float* out, int ldo, cudaStream_t stream);
+int rmvpe_pool_launch(const float* x, int ldx, int B, int T, int F, int C, float* out, cudaStream_t stream);
+int rmvpe_gru_launch(const float* xg, const float* whh, const float* bhh, int B, int T, float* out, cudaStream_t stream);
+int rmvpe_resample_launch(const float* x, int B, int N, const float* table, int new_freq, int orig_freq, int taps,
+                          int width, int n_out, float* out, cudaStream_t stream);
+int rmvpe_mel_launch(const float* y, int B, int N, const float* window, const float* basis, const int* lohi, int hop,
+                     int n_frames, int t_pad, float* out, cudaStream_t stream);
+int rmvpe_decode_launch(const float* sal, int B, int t_pad, int n_frames, float thred, float* f0, cudaStream_t stream);
+}  // namespace b2d
+
+namespace {
+bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7u) == 0; }
+bool pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
+}  // namespace
+
+extern "C" int b2d_rmvpe_conv(const float* x, int ldx, int B, int T, int F, int C_in, const float* w, const float* bias,
+                              int k, int N, int n_valid, int act, int up, const float* residual, int ldr, float* out,
+                              int ldo, void* stream) {
+    if (!x || !w || !bias || !out) return b2d::fail(B2D_ERR_NULL, "rmvpe_conv: null pointer");
+    if (B <= 0 || T <= 0 || F <= 0 || C_in <= 0 || N <= 0 || n_valid <= 0 || n_valid > N || ldx < C_in ||
+        ldo < (up ? N / 4 : n_valid) || (residual && ldr < n_valid) || act < 0 || act > 2)
+        return b2d::fail(B2D_ERR_SHAPE, "rmvpe_conv: bad shape");
+    if (k < 1 || k > 3 || C_in % 16 || N % 16 || n_valid % 2 || !pow2(F) || B > 65535 || N / 16 > 65535 ||
+        (up && (k != 2 || N % 8 || n_valid != N || residual)))
+        return b2d::fail(B2D_ERR_UNSUPPORTED, "rmvpe_conv: needs k in 1..3, C_in and N multiples of 16, an even n_valid, "
+                                              "F a power of two; up needs k = 2, N = 4 C_out with C_out even, no residual");
+    if (!b2d::aligned16(x) || ldx % 4 || !b2d::aligned16(w) || !aligned8(bias) || !aligned8(out) || ldo % 2 ||
+        (residual && (!aligned8(residual) || ldr % 2)))
+        return b2d::fail(B2D_ERR_ALIGN, "rmvpe_conv: x / w 16-byte aligned with ldx % 4 == 0; bias / out / residual "
+                                        "8-byte aligned with even strides");
+    return b2d::rmvpe_conv_launch(x, ldx, B, T, F, C_in, w, bias, k, N, n_valid, act, up, residual, ldr, out, ldo,
+                                  (cudaStream_t)stream);
+}
+
+extern "C" int b2d_rmvpe_conv_small(const float* x, int64_t x_stride_b, int64_t x_stride_t, int64_t x_stride_f,
+                                    int64_t x_stride_c, int B, int T, int F, int C_in, const float* in_scale,
+                                    const float* in_shift, const float* w, const float* bias, int k, int C_out, int relu,
+                                    int head, float* out, int ldo, void* stream) {
+    if (!x || !w || !out || (!in_scale != !in_shift)) return b2d::fail(B2D_ERR_NULL, "rmvpe_conv_small: null pointer");
+    if (B <= 0 || T <= 0 || F <= 0 || C_in <= 0 || C_out <= 0 || (!head && ldo < C_out))
+        return b2d::fail(B2D_ERR_SHAPE, "rmvpe_conv_small: bad shape");
+    if ((k != 1 && k != 3) || C_out > 16 || C_in * C_out * k * k > 4096)
+        return b2d::fail(B2D_ERR_UNSUPPORTED, "rmvpe_conv_small: k 1 or 3, C_out <= 16, C_in C_out k^2 <= 4096");
+    return b2d::rmvpe_conv_small_launch(x, x_stride_b, x_stride_t, x_stride_f, x_stride_c, B, T, F, C_in, in_scale,
+                                        in_shift, w, bias, k, C_out, relu, head, out, ldo, (cudaStream_t)stream);
+}
+
+extern "C" int b2d_rmvpe_pool(const float* x, int ldx, int B, int T, int F, int C, float* out, void* stream) {
+    if (!x || !out) return b2d::fail(B2D_ERR_NULL, "rmvpe_pool: null pointer");
+    if (B <= 0 || T <= 0 || F <= 0 || C <= 0 || ldx < C || T % 2 || F % 2)
+        return b2d::fail(B2D_ERR_SHAPE, "rmvpe_pool: bad shape (T and F must be even)");
+    return b2d::rmvpe_pool_launch(x, ldx, B, T, F, C, out, (cudaStream_t)stream);
+}
+
+extern "C" int b2d_rmvpe_gru(const float* xg, const float* w_hh, const float* b_hh, int B, int T, float* out,
+                             void* stream) {
+    if (!xg || !w_hh || !b_hh || !out) return b2d::fail(B2D_ERR_NULL, "rmvpe_gru: null pointer");
+    if (B <= 0 || T <= 0 || B > 4 * 65535) return b2d::fail(B2D_ERR_SHAPE, "rmvpe_gru: bad shape");
+    return b2d::rmvpe_gru_launch(xg, w_hh, b_hh, B, T, out, (cudaStream_t)stream);
+}
+
+extern "C" int b2d_rmvpe_resample(const float* x, int B, int N, const float* table, int new_freq, int orig_freq,
+                                  int taps, int width, int n_out, float* out, void* stream) {
+    if (!x || !table || !out) return b2d::fail(B2D_ERR_NULL, "rmvpe_resample: null pointer");
+    if (B <= 0 || N <= 0 || new_freq <= 0 || orig_freq <= 0 || taps <= 0 || width < 0 || n_out <= 0)
+        return b2d::fail(B2D_ERR_SHAPE, "rmvpe_resample: bad shape");
+    return b2d::rmvpe_resample_launch(x, B, N, table, new_freq, orig_freq, taps, width, n_out, out, (cudaStream_t)stream);
+}
+
+extern "C" int b2d_rmvpe_mel(const float* audio, int B, int N, const float* window, const float* basis, const int* lohi,
+                             int hop, int n_frames, int t_pad, float* out, void* stream) {
+    if (!audio || !window || !basis || !lohi || !out) return b2d::fail(B2D_ERR_NULL, "rmvpe_mel: null pointer");
+    if (B <= 0 || B > 65535 || hop <= 0 || n_frames <= 0 || t_pad < n_frames)
+        return b2d::fail(B2D_ERR_SHAPE, "rmvpe_mel: bad shape");
+    if (N <= 512 || n_frames != 1 + N / hop)
+        return b2d::fail(B2D_ERR_SHAPE, "rmvpe_mel: needs N > 512 samples (reflect padding) and n_frames = 1 + N / hop");
+    return b2d::rmvpe_mel_launch(audio, B, N, window, basis, lohi, hop, n_frames, t_pad, out, (cudaStream_t)stream);
+}
+
+extern "C" int b2d_rmvpe_decode(const float* salience, int B, int t_pad, int n_frames, float thred, float* f0,
+                                void* stream) {
+    if (!salience || !f0) return b2d::fail(B2D_ERR_NULL, "rmvpe_decode: null pointer");
+    if (B <= 0 || n_frames <= 0 || t_pad < n_frames) return b2d::fail(B2D_ERR_SHAPE, "rmvpe_decode: bad shape");
+    return b2d::rmvpe_decode_launch(salience, B, t_pad, n_frames, thred, f0, (cudaStream_t)stream);
+}

@@ -24,6 +24,7 @@
 // No atomics and no global mutable state: every output element has one writer and a fixed summation order, so results
 // are bit-identical from run to run, and concurrent calls from several host threads are independent.
 #include "b2d_common.cuh"
+#include "mma_sync.cuh"
 #include "tf32_split.cuh"
 
 namespace {
@@ -51,20 +52,6 @@ struct HgConvParams {
     int n_k, n_stride, n_pad;
     float* out;                    // [B, T, N] or [B, T u, C_out]
 };
-
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
-
-__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
-                 "{%0, %1, %2, %3};\n"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 
 // BM time rows (4 warps of BM / 4 rows, MT m16 tiles each) x BN output columns (NT n8 tiles) per CTA.
 // Grid: (ceil(T / BM), N / BN, B).

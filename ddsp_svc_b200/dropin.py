@@ -113,7 +113,31 @@ def _patch_diffusion(saved):
                 setattr(mod, name, ours[name])
 
 
-def patch_reference(reflow=False, diffusion=False, hifigan=False):
+_RMVPE_MODULES = ("encoder.rmvpe", "encoder.rmvpe.inference", "encoder.rmvpe.model")
+
+
+def _patch_rmvpe(saved):
+    """rebind RMVPE / E2E0 in the reference's encoder.rmvpe modules; originals into saved["rmvpe"] by module"""
+    import importlib
+    from . import rmvpe as own
+    try:
+        mods = [importlib.import_module(m) for m in _RMVPE_MODULES]
+    except ImportError as e:                    # encoder.rmvpe imports librosa
+        saved.setdefault("_not_patched", {})["encoder.rmvpe"] = "%s: %s" % (type(e).__name__, e)
+        return
+    import ddsp.vocoder as ref_vocoder
+    cached = getattr(ref_vocoder, "F0_KERNEL", {}).get("rmvpe")
+    if cached is not None and not isinstance(cached, own.RMVPE):
+        saved.setdefault("_not_patched", {})["ddsp.vocoder.F0_KERNEL['rmvpe']"] = (
+            "already holds a reference RMVPE instance; F0_Extractor keeps using it")
+    for modname, mod in zip(_RMVPE_MODULES, mods):
+        for name in ("RMVPE", "E2E0"):
+            if hasattr(mod, name):
+                saved.setdefault("rmvpe", {}).setdefault(modname, {})[name] = getattr(mod, name)
+                setattr(mod, name, getattr(own, name))
+
+
+def patch_reference(reflow=False, diffusion=False, hifigan=False, rmvpe=False):
     """Swap the synthesizer classes inside the (importable) reference package.  Returns the dict
     of original classes so a caller can restore them; its keys say what was patched.  If the enhancer stack
     (nsf_hifigan.models) cannot be imported, only the synthesizers are patched and the reason is returned under
@@ -138,7 +162,13 @@ def patch_reference(reflow=False, diffusion=False, hifigan=False):
     ``hifigan=True`` rebinds ``nsf_hifigan.models.Generator`` to ``ddsp_svc_b200.Generator``.  ``load_model`` looks the
     name up when it is called, so the enhancer (enhancer.py) and the diffusion and reflow vocoders (diffusion/vocoder.py,
     reflow/vocoder.py), which import ``load_model`` by name, all build the package's generator and vocode on the kernels.
-    Off by default; needs nsf_hifigan.models to import (reported under ``"_not_patched"`` otherwise)."""
+    Off by default; needs nsf_hifigan.models to import (reported under ``"_not_patched"`` otherwise).
+
+    ``rmvpe=True`` rebinds ``RMVPE`` and ``E2E0`` in encoder.rmvpe, encoder.rmvpe.inference and encoder.rmvpe.model to
+    ``ddsp_svc_b200.RMVPE`` / ``ddsp_svc_b200.E2E0``.  F0_Extractor imports ``RMVPE`` from encoder.rmvpe when it first
+    builds the 'rmvpe' extractor, so it then extracts f0 on the kernels.  Off by default.  If encoder.rmvpe does not
+    import (it imports librosa), or ddsp.vocoder.F0_KERNEL['rmvpe'] already holds a reference instance (which
+    F0_Extractor would keep using), that is reported under ``"_not_patched"``."""
     import ddsp.vocoder as ref_vocoder          # the reference checkout must be on sys.path
     names = ("Sins", "CombSub", "CombSubSuperFast", "CombSubFast")
     saved = {name: getattr(ref_vocoder, name) for name in names}
@@ -172,6 +202,8 @@ def patch_reference(reflow=False, diffusion=False, hifigan=False):
         _patch_reflow(saved)
     if diffusion:
         _patch_diffusion(saved)
+    if rmvpe:
+        _patch_rmvpe(saved)
     return saved
 
 
@@ -196,7 +228,7 @@ def unpatch_reference(saved):
             for name in ("NaiveV2Diff", "RectifiedFlow"):
                 if mod is not None and name in saved and hasattr(mod, name):
                     setattr(mod, name, saved[name])
-    for modname, originals in saved.get("diffusion", {}).items():
+    for modname, originals in list(saved.get("diffusion", {}).items()) + list(saved.get("rmvpe", {}).items()):
         mod = sys.modules.get(modname)
         if mod is not None:
             for name, cls in originals.items():

@@ -33,13 +33,22 @@ def _mel_to_hz(m):
     return np.where(m >= min_log_mel, min_log_hz * np.exp(logstep * (m - min_log_mel)), f_sp * m)
 
 
-def mel_filterbank(sr, n_fft, n_mels=128, fmin=0.0, fmax=None):
-    """librosa.filters.mel(sr=, n_fft=, n_mels=, fmin=, fmax=) with its defaults (htk=False, norm='slaney'):
-    triangular filters with corners equally spaced on the Slaney mel scale, each normalised to unit area -> float32
-    [n_mels, 1 + n_fft // 2]."""
+def _hz_to_mel_htk(f):
+    return 2595.0 * np.log10(1.0 + np.asarray(f, dtype=np.float64) / 700.0)
+
+
+def _mel_to_hz_htk(m):
+    return 700.0 * (10.0 ** (np.asarray(m, dtype=np.float64) / 2595.0) - 1.0)
+
+
+def mel_filterbank(sr, n_fft, n_mels=128, fmin=0.0, fmax=None, htk=False):
+    """librosa.filters.mel(sr=, n_fft=, n_mels=, fmin=, fmax=, htk=) with norm='slaney': triangular filters with
+    corners equally spaced on the Slaney (htk=False, librosa's default) or HTK (2595 log10(1 + f / 700)) mel scale, each
+    normalised to unit area -> float32 [n_mels, 1 + n_fft // 2]."""
+    to_mel, to_hz = (_hz_to_mel_htk, _mel_to_hz_htk) if htk else (_hz_to_mel, _mel_to_hz)
     fmax = float(sr) / 2 if fmax is None else float(fmax)
     fftfreqs = np.linspace(0.0, float(sr) / 2, 1 + n_fft // 2)
-    mel_f = _mel_to_hz(np.linspace(_hz_to_mel(fmin), _hz_to_mel(fmax), n_mels + 2))
+    mel_f = to_hz(np.linspace(to_mel(fmin), to_mel(fmax), n_mels + 2))
     fdiff = np.diff(mel_f)
     ramps = mel_f[:, None] - fftfreqs[None, :]
     lower = -ramps[:-2] / fdiff[:-1, None]

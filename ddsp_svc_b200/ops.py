@@ -814,3 +814,158 @@ def hifigan_post(x, w, bias):
                                            _stream()), "b2d_hifigan_post")
     _count(1)
     return out
+
+
+def _rows(name, t, C):
+    """a [..., C] channel slice of a channel-contiguous activation -> its pixel stride ld: element (..., c) of pixel
+    index p (row-major over the leading dims) at p ld + c"""
+    _need_cuda_f32(name, t)
+    if t.shape[-1] != C or t.stride(-1) != 1:
+        raise ValueError("%s must be a [..., %d] view with unit channel stride" % (name, C))
+    lead = [d for d in range(t.dim() - 1) if t.shape[d] > 1]
+    if not lead:
+        return C
+    inner = 1
+    for d in range(lead[-1] + 1, t.dim() - 1):
+        inner *= t.shape[d]
+    ld = t.stride(lead[-1]) // inner
+    for d in lead:
+        span = 1
+        for e in range(d + 1, t.dim() - 1):
+            span *= t.shape[e]
+        if t.stride(d) != ld * span:
+            raise ValueError("%s must be dense apart from its channel slice" % name)
+    return ld
+
+
+def rmvpe_conv(x, w, bias, k, n_out, act=0, up=False, residual=None, out=None, n_valid=None):
+    """One RMVPE convolution (b2d_rmvpe_conv): x a [B, T, F, C_in] channel slice -> out [B, T, F, n_valid] (or
+    [B, 2T, 2F, n_out / 4] with up) = act(conv + bias) (+ residual); act 0 none, 1 relu, 2 sigmoid.  ``out`` and
+    ``residual`` may be channel slices of wider buffers; ``w`` is packed by hifigan.pack_conv."""
+    B, T, F, Cin = x.shape
+    n_valid = n_out if n_valid is None else n_valid
+    ldx = _rows("x", x, Cin)
+    for name, t in (("w", w), ("bias", bias)):
+        _need_cuda_f32(name, t)
+    if w.numel() != 2 * k * k * Cin * n_out:
+        raise ValueError("w must hold 2 k^2 C_in N = %d floats, got %d" % (2 * k * k * Cin * n_out, w.numel()))
+    shape = (B, 2 * T, 2 * F, n_out // 4) if up else (B, T, F, n_valid)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float32, device=x.device)
+    if tuple(out.shape) != shape:
+        raise ValueError("out must be %s, got %s" % (shape, tuple(out.shape)))
+    ldo = _rows("out", out, shape[-1])
+    ldr = 0
+    if residual is not None:
+        if tuple(residual.shape) != shape:
+            raise ValueError("residual must be %s, got %s" % (shape, tuple(residual.shape)))
+        ldr = _rows("residual", residual, shape[-1])
+    _lib.check(_lib.lib().b2d_rmvpe_conv(x.data_ptr(), ldx, B, T, F, Cin, w.data_ptr(), bias.data_ptr(), int(k),
+                                         int(n_out), int(n_valid), int(act), int(bool(up)), _ptr(residual), ldr,
+                                         out.data_ptr(), ldo, _stream()), "b2d_rmvpe_conv")
+    _count(1)
+    return out
+
+
+def rmvpe_conv_small(x, w, bias, relu=False, in_scale=None, in_shift=None, head=False, out=None):
+    """Direct fp32 convolution (b2d_rmvpe_conv_small): x a [B, T, F, C_in] view with any strides, w [C_out, C_in, k, k]
+    (k 1 or 3, padding k // 2), optional input affine on the real pixels -> out [B, T, F, C_out] (a channel slice is
+    fine), or with head [B, T, C_out F] (feature c F + f)."""
+    _need_cuda_f32("x", x)
+    _need_cuda_f32("w", w)
+    B, T, F, Cin = x.shape
+    Cout, k = w.shape[0], w.shape[-1]
+    if tuple(w.shape) != (Cout, Cin, k, k) or not w.is_contiguous():
+        raise ValueError("w must be a contiguous [C_out, %d, k, k] tensor" % Cin)
+    for name, t in (("bias", bias), ("in_scale", in_scale), ("in_shift", in_shift)):
+        if t is not None:
+            _need_cuda_f32(name, t)
+    shape = (B, T, Cout * F) if head else (B, T, F, Cout)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float32, device=x.device)
+    if tuple(out.shape) != shape:
+        raise ValueError("out must be %s, got %s" % (shape, tuple(out.shape)))
+    if head:
+        if not out.is_contiguous():
+            raise ValueError("out must be contiguous")
+        ldo = Cout
+    else:
+        ldo = _rows("out", out, Cout)
+    s = x.stride()
+    _lib.check(_lib.lib().b2d_rmvpe_conv_small(x.data_ptr(), s[0], s[1], s[2], s[3], B, T, F, Cin, _ptr(in_scale),
+                                               _ptr(in_shift), w.data_ptr(), _ptr(bias), int(k), int(Cout),
+                                               int(bool(relu)), int(bool(head)), out.data_ptr(), ldo, _stream()),
+               "b2d_rmvpe_conv_small")
+    _count(1)
+    return out
+
+
+def rmvpe_pool(x):
+    """AvgPool2d(2) of a [B, T, F, C] channel slice -> a new [B, T / 2, F / 2, C] tensor (b2d_rmvpe_pool)"""
+    B, T, F, C = x.shape
+    ldx = _rows("x", x, C)
+    out = torch.empty(B, T // 2, F // 2, C, dtype=torch.float32, device=x.device)
+    _lib.check(_lib.lib().b2d_rmvpe_pool(x.data_ptr(), ldx, B, T, F, C, out.data_ptr(), _stream()), "b2d_rmvpe_pool")
+    _count(1)
+    return out
+
+
+def rmvpe_gru(xg, w_hh, b_hh):
+    """BiGRU(384 -> 256) recurrence (b2d_rmvpe_gru): xg [B, T, 1536] = W_ih x + b_ih of both directions, w_hh
+    [2, 768, 256], b_hh [2, 768] -> [B, T, 512] = [forward | backward]"""
+    for name, t in (("xg", xg), ("w_hh", w_hh), ("b_hh", b_hh)):
+        _need_cuda_f32(name, t)
+        if not t.is_contiguous():
+            raise ValueError("%s must be contiguous" % name)
+    B, T, G = xg.shape
+    if G != 1536 or w_hh.numel() != 2 * 768 * 256 or b_hh.numel() != 2 * 768:
+        raise ValueError("xg must be [B, T, 1536], w_hh [2, 768, 256], b_hh [2, 768]")
+    out = torch.empty(B, T, 512, dtype=torch.float32, device=xg.device)
+    _lib.check(_lib.lib().b2d_rmvpe_gru(xg.data_ptr(), w_hh.data_ptr(), b_hh.data_ptr(), B, T, out.data_ptr(),
+                                        _stream()), "b2d_rmvpe_gru")
+    _count(1)
+    return out
+
+
+def rmvpe_resample(x, table, new_freq, orig_freq, width, n_out):
+    """x [B, N] -> [B, n_out] through the polyphase table [new_freq, taps] (b2d_rmvpe_resample)"""
+    _need_cuda_f32("x", x)
+    _need_cuda_f32("table", table)
+    if x.dim() != 2 or not x.is_contiguous() or not table.is_contiguous() or table.shape[0] != new_freq:
+        raise ValueError("x must be a contiguous [B, N] tensor and table a contiguous [new_freq, taps] one")
+    B, N = x.shape
+    out = torch.empty(B, n_out, dtype=torch.float32, device=x.device)
+    _lib.check(_lib.lib().b2d_rmvpe_resample(x.data_ptr(), B, N, table.data_ptr(), int(new_freq), int(orig_freq),
+                                             int(table.shape[1]), int(width), int(n_out), out.data_ptr(), _stream()),
+               "b2d_rmvpe_resample")
+    _count(1)
+    return out
+
+
+def rmvpe_mel(audio, window, basis, lohi, hop, t_pad):
+    """audio [B, N] at 16 kHz -> log-mel [B, t_pad, 128] (frames past 1 + N // hop are zero) (b2d_rmvpe_mel)"""
+    _need_cuda_f32("audio", audio)
+    _need_cuda_f32("window", window)
+    _need_cuda_f32("basis", basis)
+    _need_cuda_f32("lohi", lohi, torch.int32)
+    if audio.dim() != 2 or not audio.is_contiguous():
+        raise ValueError("audio must be a contiguous [B, N] tensor")
+    B, N = audio.shape
+    out = torch.empty(B, t_pad, 128, dtype=torch.float32, device=audio.device)
+    _lib.check(_lib.lib().b2d_rmvpe_mel(audio.data_ptr(), B, N, window.data_ptr(), basis.data_ptr(), lohi.data_ptr(),
+                                        int(hop), 1 + N // hop, int(t_pad), out.data_ptr(), _stream()), "b2d_rmvpe_mel")
+    _count(1)
+    return out
+
+
+def rmvpe_decode(salience, n_frames, thred):
+    """salience [B, t_pad, 360] -> f0 [B, n_frames] in Hz, 0 where unvoiced (b2d_rmvpe_decode)"""
+    _need_cuda_f32("salience", salience)
+    if salience.dim() != 3 or salience.shape[-1] != 360 or not salience.is_contiguous():
+        raise ValueError("salience must be a contiguous [B, T, 360] tensor")
+    B, t_pad, _ = salience.shape
+    out = torch.empty(B, n_frames, dtype=torch.float32, device=salience.device)
+    _lib.check(_lib.lib().b2d_rmvpe_decode(salience.data_ptr(), B, t_pad, int(n_frames), float(thred), out.data_ptr(),
+                                           _stream()), "b2d_rmvpe_decode")
+    _count(1)
+    return out

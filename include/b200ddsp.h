@@ -604,6 +604,44 @@ int b2d_set_overlap(int mode);
  * pass BigCrush; 11 % faster; Kolmogorov-Smirnov / correlation tests in tests/test_gpu_combsub_sinegen.py). */
 int b2d_set_sinegen_impl(int impl);
 
+/* ---- RMVPE pitch extractor (encoder/rmvpe/), inference (rmvpe.cu) ---------------------------------------------------
+ * Activations are channel-contiguous [B, T, F, C]: element (b, t, f, c) at x[((b T + t) F + f) ld + c].
+ * b2d_rmvpe_conv: a k x k convolution (k = 3: padding 1; k = 1; k = 2 with up) as an implicit GEMM on the tensor cores,
+ *   3xTF32, zero padding at the T and F edges.  w: [k k][C_in / 8][N / 8][32][4] in mma.sync B-fragment order, TF32
+ *   (hi, lo) halves (ddsp_svc_b200.hifigan.pack_conv of the [N, C_in, k k] weight).  out[pixel ldo + col] =
+ *   act(conv + bias[col]) (+ residual[pixel ldr + col]) for col < n_valid; act 0 none, 1 relu, 2 sigmoid.  up = 1: the
+ *   polyphase form of ConvTranspose2d(3x3, stride 2, padding 1, output_padding 1) (ddsp_svc_b200.rmvpe.polyphase2d):
+ *   column r C_out + co (N = 4 C_out) goes to channel co of pixel (2t + r / 2, 2f + r % 2) of the [B, 2T, 2F] output,
+ *   plus bias[co].  C_in and N multiples of 16, F a power of two, x and w 16-byte aligned.
+ * b2d_rmvpe_conv_small: direct fp32 k x k convolution (k = 1 or 3, padding k / 2), x element (b, t, f, c) at
+ *   x[b x_stride_b + t x_stride_t + f x_stride_f + c x_stride_c], optionally x in_scale[c] + in_shift[c] on every real
+ *   input (before the zero padding), w [C_out][C_in][k][k], bias [C_out] or NULL, relu, C_out <= 16.  head = 0:
+ *   out[pixel ldo + co]; head = 1: out[((b T + t) C_out + co) F + f] (the head's features c F + f).
+ * b2d_rmvpe_pool: out [B, T / 2, F / 2, C] = AvgPool2d(2) of x (row stride ldx).
+ * b2d_rmvpe_gru: the bidirectional GRU(384 -> 256) recurrence.  xg [B, T, 2][3][256] = W_ih x + b_ih of both
+ *   directions (gates r, z, n), w_hh [2][768][256], b_hh [2][768] -> out [B, T, 512] = [forward | backward].  One
+ *   8-CTA cluster per direction and group of 4 utterances.
+ * b2d_rmvpe_resample: torchaudio Resample with the [new_freq, taps] table of ddsp_svc_b200.rmvpe.resample_table
+ *   (rates divided by their gcd): out[b, j new_freq + p] = sum_k table[p, k] x[b, j orig_freq + k - width], zero
+ *   outside, for the first n_out samples.
+ * b2d_rmvpe_mel: log(clamp(basis @ |stft(audio, 1024, hop, hann window, center, reflect)|, 1e-5)), basis [128, 513]
+ *   with lohi [128][2] the support of each row -> out [B, t_pad, 128], zeros for frames n_frames .. t_pad - 1.
+ *   Needs N > 512 and n_frames = 1 + N / hop.
+ * b2d_rmvpe_decode: salience [B, t_pad, 360] -> f0 [B, n_frames] (to_local_average_f0).
+ * No atomics: bit-identical from run to run. */
+int b2d_rmvpe_conv(const float* x, int ldx, int B, int T, int F, int C_in, const float* w, const float* bias, int k,
+                   int N, int n_valid, int act, int up, const float* residual, int ldr, float* out, int ldo, void* stream);
+int b2d_rmvpe_conv_small(const float* x, int64_t x_stride_b, int64_t x_stride_t, int64_t x_stride_f, int64_t x_stride_c,
+                         int B, int T, int F, int C_in, const float* in_scale, const float* in_shift, const float* w,
+                         const float* bias, int k, int C_out, int relu, int head, float* out, int ldo, void* stream);
+int b2d_rmvpe_pool(const float* x, int ldx, int B, int T, int F, int C, float* out, void* stream);
+int b2d_rmvpe_gru(const float* xg, const float* w_hh, const float* b_hh, int B, int T, float* out, void* stream);
+int b2d_rmvpe_resample(const float* x, int B, int N, const float* table, int new_freq, int orig_freq, int taps,
+                       int width, int n_out, float* out, void* stream);
+int b2d_rmvpe_mel(const float* audio, int B, int N, const float* window, const float* basis, const int* lohi, int hop,
+                  int n_frames, int t_pad, float* out, void* stream);
+int b2d_rmvpe_decode(const float* salience, int B, int t_pad, int n_frames, float thred, float* f0, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
