@@ -526,3 +526,82 @@ extern "C" int b2d_rmvpe_decode(const float* salience, int B, int t_pad, int n_f
     if (B <= 0 || n_frames <= 0 || t_pad < n_frames) return b2d::fail(B2D_ERR_SHAPE, "rmvpe_decode: bad shape");
     return b2d::rmvpe_decode_launch(salience, B, t_pad, n_frames, thred, f0, (cudaStream_t)stream);
 }
+
+// ---------------------------------------------------------------------------------------------------------------------
+// HuBERT / ContentVec units encoder, inference: the kernels of hubert.cu
+// ---------------------------------------------------------------------------------------------------------------------
+namespace b2d {
+int hubert_conv0_launch(const float* x, int B, int N, int pad, const float* w, int L0, int La, float* y, double* part,
+                        cudaStream_t stream);
+int hubert_gn_finalize_launch(const double* part, int B, int n_tiles, int L0, const float* gamma, const float* beta,
+                              float eps, float* scale, float* shift, cudaStream_t stream);
+int hubert_act_launch(const float* x, int rows, int C, int rows_per_b, const float* scale, const float* shift, float* hi,
+                      float* lo, cudaStream_t stream);
+int hubert_ln_launch(const float* x, const float* y, int rows, int T, int rows_per_b, int C, int gelu,
+                     const float* gamma, const float* beta, float eps, float* h, float* hi, float* lo,
+                     cudaStream_t stream);
+int hubert_posconv_launch(const float* x, int B, int T, const float* w, const float* bias, float* y,
+                          cudaStream_t stream);
+int hubert_attention_launch(const float* qkv, int B, int T, float* hi, float* lo, cudaStream_t stream);
+int hubert_align_launch(const float* units, int B, int T, int C, float ratio, int n_frames, float* out,
+                        cudaStream_t stream);
+}  // namespace b2d
+
+extern "C" int b2d_hubert_conv0(const float* x, int B, int N, int pad, const float* w, int La, float* y, double* part,
+                                void* stream) {
+    if (!x || !w || !y || !part) return b2d::fail(B2D_ERR_NULL, "hubert_conv0: null pointer");
+    if (B <= 0 || B > 65535 || N <= 0 || pad < 0 || (long long)N + 2LL * pad < 10)
+        return b2d::fail(B2D_ERR_SHAPE, "hubert_conv0: bad shape (N + 2 pad must be >= 10)");
+    const int L0 = (N + 2 * pad - 10) / 5 + 1;
+    if (La < L0) return b2d::fail(B2D_ERR_SHAPE, "hubert_conv0: La %d < L0 %d", La, L0);
+    return b2d::hubert_conv0_launch(x, B, N, pad, w, L0, La, y, part, (cudaStream_t)stream);
+}
+
+extern "C" int b2d_hubert_gn_finalize(const double* part, int B, int n_tiles, int L0, const float* gamma,
+                                      const float* beta, float eps, float* scale, float* shift, void* stream) {
+    if (!part || !gamma || !beta || !scale || !shift) return b2d::fail(B2D_ERR_NULL, "hubert_gn_finalize: null pointer");
+    if (B <= 0 || n_tiles <= 0 || L0 <= 0 || L0 > 64LL * n_tiles || !(eps > 0.f))
+        return b2d::fail(B2D_ERR_SHAPE, "hubert_gn_finalize: bad shape");
+    return b2d::hubert_gn_finalize_launch(part, B, n_tiles, L0, gamma, beta, eps, scale, shift, (cudaStream_t)stream);
+}
+
+extern "C" int b2d_hubert_act(const float* x, int rows, int C, int rows_per_b, const float* scale, const float* shift,
+                              float* hi, float* lo, void* stream) {
+    if (!x || !hi || (scale && !shift) || (shift && !scale)) return b2d::fail(B2D_ERR_NULL, "hubert_act: null pointer");
+    if (rows <= 0 || C <= 0 || rows_per_b <= 0 || rows % rows_per_b)
+        return b2d::fail(B2D_ERR_SHAPE, "hubert_act: bad shape (rows must be a multiple of rows_per_b)");
+    return b2d::hubert_act_launch(x, rows, C, rows_per_b, scale, shift, hi, lo, (cudaStream_t)stream);
+}
+
+extern "C" int b2d_hubert_ln(const float* x, const float* y, int rows, int T, int rows_per_b, int C, int gelu,
+                             const float* gamma, const float* beta, float eps, float* h, float* hi, float* lo,
+                             void* stream) {
+    if (!x || !gamma || !beta || (!h && !hi) || (lo && !hi)) return b2d::fail(B2D_ERR_NULL, "hubert_ln: null pointer");
+    if (rows <= 0 || T <= 0 || rows % T || rows_per_b < T || !(eps > 0.f))
+        return b2d::fail(B2D_ERR_SHAPE, "hubert_ln: bad shape");
+    if (C != 512 && C != 768) return b2d::fail(B2D_ERR_UNSUPPORTED, "hubert_ln: C must be 512 or 768, got %d", C);
+    if (h == x && rows_per_b != T) return b2d::fail(B2D_ERR_SHAPE, "hubert_ln: h may alias x only when rows_per_b = T");
+    return b2d::hubert_ln_launch(x, y, rows, T, rows_per_b, C, gelu, gamma, beta, eps, h, hi, lo, (cudaStream_t)stream);
+}
+
+extern "C" int b2d_hubert_posconv(const float* x, int B, int T, const float* w, const float* bias, float* y,
+                                  void* stream) {
+    if (!x || !w || !bias || !y) return b2d::fail(B2D_ERR_NULL, "hubert_posconv: null pointer");
+    if (B <= 0 || B > 65535 || T <= 0) return b2d::fail(B2D_ERR_SHAPE, "hubert_posconv: bad shape");
+    if (!b2d::aligned16(w)) return b2d::fail(B2D_ERR_ALIGN, "hubert_posconv: w must be 16-byte aligned");
+    return b2d::hubert_posconv_launch(x, B, T, w, bias, y, (cudaStream_t)stream);
+}
+
+extern "C" int b2d_hubert_attention(const float* qkv, int B, int T, float* hi, float* lo, void* stream) {
+    if (!qkv || !hi) return b2d::fail(B2D_ERR_NULL, "hubert_attention: null pointer");
+    if (B <= 0 || B > 65535 || T <= 0) return b2d::fail(B2D_ERR_SHAPE, "hubert_attention: bad shape");
+    return b2d::hubert_attention_launch(qkv, B, T, hi, lo, (cudaStream_t)stream);
+}
+
+extern "C" int b2d_hubert_align(const float* units, int B, int T, int C, float ratio, int n_frames, float* out,
+                                void* stream) {
+    if (!units || !out) return b2d::fail(B2D_ERR_NULL, "hubert_align: null pointer");
+    if (B <= 0 || T <= 0 || C <= 0 || n_frames <= 0 || !(ratio >= 0.f) || !(ratio < 1e30f))
+        return b2d::fail(B2D_ERR_SHAPE, "hubert_align: bad shape");
+    return b2d::hubert_align_launch(units, B, T, C, ratio, n_frames, out, (cudaStream_t)stream);
+}

@@ -137,7 +137,25 @@ def _patch_rmvpe(saved):
                 setattr(mod, name, getattr(own, name))
 
 
-def patch_reference(reflow=False, diffusion=False, hifigan=False, rmvpe=False):
+def _patch_units(saved):
+    """rebind Units_Encoder in ddsp.vocoder and HubertSoft in encoder.hubert.model and ddsp.vocoder; originals into
+    saved["units"] by module"""
+    import ddsp.vocoder as ref_vocoder
+    from . import hubert as own
+    targets = [(ref_vocoder, ("Units_Encoder", "HubertSoft"))]
+    try:
+        import encoder.hubert.model as ref_hubert
+        targets.append((ref_hubert, ("HubertSoft",)))
+    except ImportError as e:                    # encoder.hubert.model imports sklearn
+        saved.setdefault("_not_patched", {})["encoder.hubert.model"] = "%s: %s" % (type(e).__name__, e)
+    for mod, names in targets:
+        for name in names:
+            if hasattr(mod, name):
+                saved.setdefault("units", {}).setdefault(mod.__name__, {})[name] = getattr(mod, name)
+                setattr(mod, name, getattr(own, name))
+
+
+def patch_reference(reflow=False, diffusion=False, hifigan=False, rmvpe=False, units=False):
     """Swap the synthesizer classes inside the (importable) reference package.  Returns the dict
     of original classes so a caller can restore them; its keys say what was patched.  If the enhancer stack
     (nsf_hifigan.models) cannot be imported, only the synthesizers are patched and the reason is returned under
@@ -168,7 +186,13 @@ def patch_reference(reflow=False, diffusion=False, hifigan=False, rmvpe=False):
     ``ddsp_svc_b200.RMVPE`` / ``ddsp_svc_b200.E2E0``.  F0_Extractor imports ``RMVPE`` from encoder.rmvpe when it first
     builds the 'rmvpe' extractor, so it then extracts f0 on the kernels.  Off by default.  If encoder.rmvpe does not
     import (it imports librosa), or ddsp.vocoder.F0_KERNEL['rmvpe'] already holds a reference instance (which
-    F0_Extractor would keep using), that is reported under ``"_not_patched"``."""
+    F0_Extractor would keep using), that is reported under ``"_not_patched"``.
+
+    ``units=True`` rebinds ``Units_Encoder`` in ddsp.vocoder and ``HubertSoft`` in ddsp.vocoder and encoder.hubert.model
+    to ``ddsp_svc_b200.Units_Encoder`` / ``ddsp_svc_b200.HubertSoft``, so main.py, the GUIs, the APIs and preprocess.py
+    encode units on the kernels ('hubertsoft', the 'hubertbase*' and the 'contentvec*' encoders; fairseq checkpoints
+    load without fairseq).  Off by default.  If encoder.hubert.model does not import, that is reported under
+    ``"_not_patched"``."""
     import ddsp.vocoder as ref_vocoder          # the reference checkout must be on sys.path
     names = ("Sins", "CombSub", "CombSubSuperFast", "CombSubFast")
     saved = {name: getattr(ref_vocoder, name) for name in names}
@@ -204,6 +228,8 @@ def patch_reference(reflow=False, diffusion=False, hifigan=False, rmvpe=False):
         _patch_diffusion(saved)
     if rmvpe:
         _patch_rmvpe(saved)
+    if units:
+        _patch_units(saved)
     return saved
 
 
@@ -228,7 +254,8 @@ def unpatch_reference(saved):
             for name in ("NaiveV2Diff", "RectifiedFlow"):
                 if mod is not None and name in saved and hasattr(mod, name):
                     setattr(mod, name, saved[name])
-    for modname, originals in list(saved.get("diffusion", {}).items()) + list(saved.get("rmvpe", {}).items()):
+    for modname, originals in (list(saved.get("diffusion", {}).items()) + list(saved.get("rmvpe", {}).items())
+                               + list(saved.get("units", {}).items())):
         mod = sys.modules.get(modname)
         if mod is not None:
             for name, cls in originals.items():

@@ -969,3 +969,144 @@ def rmvpe_decode(salience, n_frames, thred):
                                            _stream()), "b2d_rmvpe_decode")
     _count(1)
     return out
+
+
+# ---- HuBERT / ContentVec units encoder (b2d_hubert_*) ------------------------------------------------------------------
+def _contig(name, t, dtype=torch.float32):
+    _need_cuda_f32(name, t, dtype)
+    if not t.is_contiguous():
+        raise ValueError("%s must be contiguous" % name)
+
+
+def _operand(shape, device, split):
+    """an output a library GEMM reads: (hi, lo) TF32 halves when split, else one fp32 tensor"""
+    if split:
+        return (torch.empty(shape, dtype=torch.float32, device=device),
+                torch.empty(shape, dtype=torch.float32, device=device))
+    return torch.empty(shape, dtype=torch.float32, device=device)
+
+
+def _operand_ptrs(op):
+    return (op[0].data_ptr(), op[1].data_ptr()) if isinstance(op, tuple) else (op.data_ptr(), 0)
+
+
+def hubert_conv0(x, w, pad, La):
+    """Conv1d(1 -> 512, 10, stride 5) of x [B, N] zero-padded by `pad` -> (y [B, La, 512], part [B, La / 64, 2, 512]
+    fp64, L0) (b2d_hubert_conv0): y zero past the L0 valid frames, part the per-tile GroupNorm sums"""
+    _contig("x", x)
+    _contig("w", w)
+    if x.dim() != 2 or w.numel() != 512 * 10:
+        raise ValueError("x must be [B, N] and w [512, 1, 10]")
+    B, N = x.shape
+    y = torch.empty(B, La, 512, dtype=torch.float32, device=x.device)
+    part = torch.empty(B, -(-La // 64), 2, 512, dtype=torch.float64, device=x.device)
+    _lib.check(_lib.lib().b2d_hubert_conv0(x.data_ptr(), B, N, int(pad), w.data_ptr(), int(La), y.data_ptr(),
+                                           part.data_ptr(), _stream()), "b2d_hubert_conv0")
+    _count(1)
+    return y, part, (N + 2 * pad - 10) // 5 + 1
+
+
+def hubert_gn_finalize(part, L0, gamma, beta, eps=1e-5):
+    """per-tile sums [B, n_tiles, 2, 512] -> GroupNorm(512, 512) (scale, shift) [B, 512] (b2d_hubert_gn_finalize)"""
+    _contig("part", part, torch.float64)
+    _contig("gamma", gamma)
+    _contig("beta", beta)
+    B, n_tiles = part.shape[:2]
+    scale = torch.empty(B, 512, dtype=torch.float32, device=part.device)
+    shift = torch.empty_like(scale)
+    _lib.check(_lib.lib().b2d_hubert_gn_finalize(part.data_ptr(), B, n_tiles, int(L0), gamma.data_ptr(),
+                                                 beta.data_ptr(), float(eps), scale.data_ptr(), shift.data_ptr(),
+                                                 _stream()), "b2d_hubert_gn_finalize")
+    _count(1)
+    return scale, shift
+
+
+def hubert_act(x, scale=None, shift=None, split=True):
+    """GELU(x scale[b] + shift[b]) of x [B, L, C] (or [rows, C] without the affine) as a GEMM operand of the same
+    shape (b2d_hubert_act)"""
+    _contig("x", x)
+    C = x.shape[-1]
+    rows = x.numel() // C
+    per_b = x.shape[1] if scale is not None else rows
+    if scale is not None:
+        _contig("scale", scale)
+        _contig("shift", shift)
+        if x.dim() != 3 or scale.shape != (x.shape[0], C) or shift.shape != scale.shape:
+            raise ValueError("with an affine, x must be [B, L, C] and scale, shift [B, C]")
+    out = _operand(x.shape, x.device, split)
+    hi, lo = _operand_ptrs(out)
+    _lib.check(_lib.lib().b2d_hubert_act(x.data_ptr(), rows, C, per_b, _ptr(scale), _ptr(shift), hi, lo, _stream()),
+               "b2d_hubert_act")
+    _count(1)
+    return out
+
+
+def hubert_ln(x, gamma, beta, T, y=None, gelu=False, eps=1e-5, h=None, operand=True, split=True):
+    """LayerNorm(C) of rows of x [B, rows_per_b, C] (the first T of each utterance; x [B T, C] when rows_per_b = T)
+    (+ y [B T, C]), GELU first when `gelu` -> (h [B T, C] or None, operand or None) (b2d_hubert_ln).  Pass h = x to
+    normalize in place; h=False skips the fp32 output."""
+    _contig("x", x)
+    _contig("gamma", gamma)
+    _contig("beta", beta)
+    C = x.shape[-1]
+    n_in = x.numel() // C
+    B = x.shape[0] if x.dim() == 3 else n_in // T
+    per_b = n_in // B
+    rows = B * T
+    if y is not None:
+        _contig("y", y)
+        if y.numel() != rows * C:
+            raise ValueError("y must hold B T rows of %d" % C)
+    if h is None:
+        h = torch.empty(rows, C, dtype=torch.float32, device=x.device)
+    elif h is False:
+        h = None
+    else:
+        _contig("h", h)
+    op = _operand((rows, C), x.device, split) if operand else None
+    hi, lo = _operand_ptrs(op) if operand else (0, 0)
+    _lib.check(_lib.lib().b2d_hubert_ln(x.data_ptr(), _ptr(y), rows, int(T), per_b, C, int(bool(gelu)),
+                                        gamma.data_ptr(), beta.data_ptr(), float(eps), _ptr(h), hi, lo, _stream()),
+               "b2d_hubert_ln")
+    _count(1)
+    return h, op
+
+
+def hubert_posconv(x, w, bias, T):
+    """GELU(grouped positional convolution + bias) of x [B T, 768] -> [B T, 768] (b2d_hubert_posconv); w the folded
+    weight packed [16, 128, 48, 48]"""
+    _contig("x", x)
+    _contig("w", w)
+    _contig("bias", bias)
+    if x.shape[-1] != 768 or (x.numel() // 768) % T or w.numel() != 16 * 128 * 48 * 48:
+        raise ValueError("x must be [B T, 768] and w [16, 128, 48, 48]")
+    B = x.numel() // 768 // T
+    y = torch.empty(B * T, 768, dtype=torch.float32, device=x.device)
+    _lib.check(_lib.lib().b2d_hubert_posconv(x.data_ptr(), B, int(T), w.data_ptr(), bias.data_ptr(), y.data_ptr(),
+                                             _stream()), "b2d_hubert_posconv")
+    _count(1)
+    return y
+
+
+def hubert_attention(qkv, T, split=True):
+    """12-head softmax attention of qkv [B T, 2304] -> the out-projection's operand [B T, 768] (b2d_hubert_attention)"""
+    _contig("qkv", qkv)
+    if qkv.shape[-1] != 2304 or (qkv.numel() // 2304) % T:
+        raise ValueError("qkv must be [B T, 2304]")
+    B = qkv.numel() // 2304 // T
+    out = _operand((B * T, 768), qkv.device, split)
+    hi, lo = _operand_ptrs(out)
+    _lib.check(_lib.lib().b2d_hubert_attention(qkv.data_ptr(), B, int(T), hi, lo, _stream()), "b2d_hubert_attention")
+    _count(1)
+    return out
+
+
+def hubert_align(units, ratio, n_frames):
+    """units [B, T, C] -> [B, n_frames, C] at rows min(rint(float32(ratio) f), T - 1) (b2d_hubert_align)"""
+    _contig("units", units)
+    B, T, C = units.shape
+    out = torch.empty(B, n_frames, C, dtype=torch.float32, device=units.device)
+    _lib.check(_lib.lib().b2d_hubert_align(units.data_ptr(), B, T, C, float(ratio), int(n_frames), out.data_ptr(),
+                                           _stream()), "b2d_hubert_align")
+    _count(1)
+    return out

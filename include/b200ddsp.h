@@ -642,6 +642,39 @@ int b2d_rmvpe_mel(const float* audio, int B, int N, const float* window, const f
                   int n_frames, int t_pad, float* out, void* stream);
 int b2d_rmvpe_decode(const float* salience, int B, int t_pad, int n_frames, float thred, float* f0, void* stream);
 
+/* ---- HuBERT / ContentVec units encoder (encoder/hubert/model.py, fairseq HubertModel), inference (hubert.cu) ---------
+ * Activations are token-major [B, T, C], C contiguous.  Outputs named (hi, lo) are a library GEMM's operand: fp32 into
+ * `hi` when `lo` is NULL, else the TF32-exact halves of b2d_split_tf32.
+ * b2d_hubert_conv0: Conv1d(1 -> 512, kernel 10, stride 5, no bias) of x [B, N] zero-padded by `pad` on the left (and
+ *   as far as needed on the right) -> y [B, La, 512] for the L0 = (N + 2 pad - 10) / 5 + 1 valid frames, zeros for
+ *   frames L0 .. La - 1; w [512][10].  part [B, ceil(La / 64), 2, 512] (fp64): the per-tile sums of y and y^2 over the
+ *   valid frames, for b2d_hubert_gn_finalize (n_tiles = ceil(La / 64)).
+ * b2d_hubert_gn_finalize: GroupNorm(512, 512) over the L0 frames -> scale, shift [B, 512] with y scale + shift the
+ *   normalized, affine output.
+ * b2d_hubert_act: GELU(x scale[b, c] + shift[b, c]) (the affine only when scale is non-NULL) of x [B rows_per_b, C]
+ *   -> (hi, lo) of the same shape.
+ * b2d_hubert_ln: row r < rows (= B T) reads x[(r / T) rows_per_b + r % T] (+ y[r] when y is non-NULL), optionally
+ *   GELU, LayerNorm(C) with gamma, beta, eps -> h[r] (when non-NULL) and (hi, lo)[r] (when hi is non-NULL).  C = 512 or
+ *   768; h may be x itself when rows_per_b = T.
+ * b2d_hubert_posconv: y [B T, 768] = GELU(Conv1d(768, 768, 128, padding 64, groups 16)(x)[..., :T] + bias) of x
+ *   [B T, 768]; w [16][128][48 in][48 out] (weight norm folded), 16-byte aligned.
+ * b2d_hubert_attention: per head of qkv [B T, 2304] (q | k | v, head h at columns 64 h of each) -> (hi, lo) [B T, 768]
+ *   = softmax(q k^T / 8) v, non-causal, over the T keys.
+ * b2d_hubert_align: out [B, n_frames, C] = units [B, T, C] at row min(rint(ratio f), T - 1) of frame f, the product
+ *   ratio f in float32 and rounded half to even.
+ * No atomics: bit-identical from run to run. */
+int b2d_hubert_conv0(const float* x, int B, int N, int pad, const float* w, int La, float* y, double* part,
+                     void* stream);
+int b2d_hubert_gn_finalize(const double* part, int B, int n_tiles, int L0, const float* gamma, const float* beta,
+                           float eps, float* scale, float* shift, void* stream);
+int b2d_hubert_act(const float* x, int rows, int C, int rows_per_b, const float* scale, const float* shift, float* hi,
+                   float* lo, void* stream);
+int b2d_hubert_ln(const float* x, const float* y, int rows, int T, int rows_per_b, int C, int gelu, const float* gamma,
+                  const float* beta, float eps, float* h, float* hi, float* lo, void* stream);
+int b2d_hubert_posconv(const float* x, int B, int T, const float* w, const float* bias, float* y, void* stream);
+int b2d_hubert_attention(const float* qkv, int B, int T, float* hi, float* lo, void* stream);
+int b2d_hubert_align(const float* units, int B, int T, int C, float ratio, int n_frames, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
