@@ -21,11 +21,14 @@
 #ifndef B2D_HOST_EMU               // tests/emu/ runs the kernels' source on the CPU (host_emu.h provides the shims)
 #include "b2d_common.cuh"
 #endif
-#include "fft_smem.cuh"
+#include "bluestein.cuh"
 
 using namespace b2d_fft;
+using namespace b2d_bluestein;
 using b2d_fft_smem::kThreads;
 using b2d_fft_smem::padi;
+
+extern "C" int b2d_mel_frames(int n_samples, int n_fft, int win_size, int hop);
 
 namespace {
 
@@ -152,6 +155,103 @@ __global__ void __launch_bounds__(kThreads, 3) mel_kernel(MelParams p) {
         const int m = i / kFramesPerCta, c = i - m * kFramesPerCta;
         if (c < nfr) p.out[((size_t)b * p.n_mels + m) * p.n_frames + f0 + c] = stage[m * (kFramesPerCta + 1) + c];
     }
+}
+
+// ---- keyshift: STFT.get_mel(y, keyshift) for keyshift != 0 (nvSTFT.py:73-117, speed 1, center False) ----
+// n' = round(2048 * 2^(keyshift / 12)) is both the transform and the window length, any integer in [hop, 3072]:
+//   y_pad  = pad(y, (n' - hop) / 2 left, max((n' - hop + 1) / 2, n' - T - left) right, reflect | constant)
+//   X      = n'-point DFT of hann(n') frames, bins k < K = min(1025, n' / 2 + 1)
+//   mag    = sqrt(Re^2 + Im^2 + 1e-9) * 2048 / n' for k < K, exactly 0 for K <= k < 1025 (the pad follows the sqrt)
+//   mel    = log(clamp(mel_basis [n_mels, 1025] @ mag, clip_val))   (the unshifted 2048-point basis)
+// The DFT is Bluestein's (bluestein.cuh) for the K bins only, so M >= n' + K - 1: 4096 up to n' = 3072.  One CTA owns
+// two consecutive frames of one utterance, transformed side by side in one batched FFT.  They are not packed as a + j b
+// like mel_kernel's pairs: separating the two spectra needs bins n' - k beyond K, which an M-point convolution this
+// small does not produce.  A CTA owns one pair and no loop over pairs: the 4096-point transforms need nearly all 255
+// registers, and a frame loop lets the compiler hoist their index arithmetic out of it and spill.
+// The table (bluestein.cuh's layout, window hann(n')) is per n'.  The projection is mel_kernel's.
+struct MelKeyshiftParams {
+    const float* y;            // [B, T]
+    const float* table;        // bluestein.cuh table of n (window, chirp, FFT_M(h) / M)
+    const float* basis;        // [n_mels, 1025]
+    const int* lohi;           // [n_mels, 2]
+    float* out;                // [B, n_mels, n_frames]
+    int T, hop, n, K, n_frames, n_mels, pad_left, reflect;
+    float clip;
+};
+
+constexpr int kKeyshiftMaxN = 3072;
+
+template <int M> constexpr size_t keyshift_smem_bytes() {
+    return (size_t)2 * b2d_fft_smem::Plan<M>::kPad * sizeof(float2) +
+           (size_t)(b2d_fft_smem::Plan<M>::kTw2 + b2d_fft_smem::Plan<M>::kTw3) * sizeof(float2) +
+           (size_t)2 * kMagStride * sizeof(float);
+}
+
+// ZU: n <= M / 2, the first FFT skips the zero upper half of its input
+template <int M, bool ZU>
+__global__ void __launch_bounds__(kThreads) mel_keyshift_kernel(MelKeyshiftParams p) {
+    constexpr int kPadM = b2d_fft_smem::Plan<M>::kPad;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    float2* z = reinterpret_cast<float2*>(smem_raw);          // [2][kPadM] frames fa, fa + 1
+    float2* tw2 = z + 2 * kPadM;
+    float2* tw3 = tw2 + b2d_fft_smem::Plan<M>::kTw2;
+    float* mag = reinterpret_cast<float*>(tw3 + b2d_fft_smem::Plan<M>::kTw3);        // [2][kMagStride]
+    const int tid = threadIdx.x, b = blockIdx.y, n = p.n, fa = 2 * blockIdx.x;
+    const bool has_b = fa + 1 < p.n_frames;
+    const float* y = p.y + (size_t)b * p.T;
+    const float* window = p.table + kWinOff;
+    const float2* chirp = reinterpret_cast<const float2*>(p.table + chirp_off(n));
+
+    b2d_fft_smem::init_twiddles<M>(tw2, tw3, tid);
+    // ---- windowed, chirped frames fa and fa + 1: w y conj(c) on [0, n), zero above ----
+    const int s0 = fa * p.hop - p.pad_left;
+    for (int m = tid; m < (ZU ? M / 2 : M); m += kThreads) {
+        float2 va = make_float2(0.f, 0.f), vb = va;
+        if (m < n) {
+            const float w = __ldg(window + m);
+            const float2 ch = __ldg(chirp + m);
+            const float a = w * sample_at(y, p.T, s0 + m, p.reflect);
+            const float c = has_b ? w * sample_at(y, p.T, s0 + p.hop + m, p.reflect) : 0.f;
+            va = make_float2(a * ch.x, -a * ch.y);
+            vb = make_float2(c * ch.x, -c * ch.y);
+        }
+        z[padi(m)] = va;
+        z[kPadM + padi(m)] = vb;
+    }
+    __syncthreads();
+    bluestein_core<M, 2, ZU>(z, reinterpret_cast<const float2*>(p.table + hspec_off(n)), tw2, tw3, tid);
+    // ---- magnitudes of bins k < K, scaled by 2048 / n; zero above ----
+    for (int k = tid; k < kBins; k += kThreads) {
+        float ma = 0.f, mb = 0.f;
+        if (k < p.K) {
+            const float2 xa = bluestein_out<M>(z, chirp, k), xb = bluestein_out<M>(z + kPadM, chirp, k);
+            ma = sqrtf(xa.x * xa.x + xa.y * xa.y + 1e-9f) * 2048.f / (float)n;
+            mb = sqrtf(xb.x * xb.x + xb.y * xb.y + 1e-9f) * 2048.f / (float)n;
+        }
+        mag[k] = ma;
+        mag[kMagStride + k] = mb;
+    }
+    __syncthreads();
+    // ---- mel projection and log: thread m, both frames ----
+    if (tid < p.n_mels) {
+        float sa, sb;
+        project_pair(mag, p.basis + (size_t)tid * kBins, __ldg(p.lohi + 2 * tid), __ldg(p.lohi + 2 * tid + 1), sa, sb);
+        float* row = p.out + ((size_t)b * p.n_mels + tid) * p.n_frames + fa;
+        row[0] = logf(fmaxf(sa, p.clip));
+        if (has_b) row[1] = logf(fmaxf(sb, p.clip));
+    }
+}
+
+// the shape fields of p for n_samples, n' = n_fft, hop (nvSTFT.py:97-104); returns n_frames (0: no frame)
+int keyshift_setup(MelKeyshiftParams& p, int n_samples, int n_fft, int hop) {
+    p.T = n_samples; p.n = n_fft; p.hop = hop;
+    p.K = min(kBins, n_fft / 2 + 1);
+    p.pad_left = (n_fft - hop) / 2;
+    int pad_right = (n_fft - hop + 1) / 2;
+    if (n_fft - n_samples - p.pad_left > pad_right) pad_right = n_fft - n_samples - p.pad_left;
+    p.reflect = pad_right < n_samples ? 1 : 0;                  // then pad_left <= pad_right < n_samples as well
+    p.n_frames = b2d_mel_frames(n_samples, n_fft, n_fft, hop);
+    return p.n_frames;
 }
 
 // ---- backward: dL/dy for g = dL/dmel [B, n_mels, n_frames] (any element strides) ----
@@ -310,7 +410,47 @@ extern "C" int b2d_mel_frames(int n_samples, int n_fft, int win_size, int hop) {
     return padded < n_fft ? 0 : (int)(1 + (padded - n_fft) / hop);
 }
 
+extern "C" int b2d_mel_keyshift_table_floats(int n_fft) {
+    if (n_fft < 1 || n_fft > kKeyshiftMaxN) return 0;
+    return bluestein_table_floats(n_fft, min(kBins, n_fft / 2 + 1));
+}
+
 #ifndef B2D_HOST_EMU
+
+namespace {
+template <int M, bool ZU> int launch_keyshift(const MelKeyshiftParams& p, int B, cudaStream_t st) {
+    constexpr size_t smem = keyshift_smem_bytes<M>();
+    cudaError_t e = cudaFuncSetAttribute(mel_keyshift_kernel<M, ZU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return b2d::fail((int)e, "mel_spectrogram_keyshift: smem attr: %s", cudaGetErrorString(e));
+    mel_keyshift_kernel<M, ZU><<<dim3((p.n_frames + 1) / 2, B), kThreads, smem, st>>>(p);
+    return b2d::check_launch("mel_spectrogram_keyshift");
+}
+}  // namespace
+
+extern "C" int b2d_mel_spectrogram_keyshift(const float* audio, const float* table, const float* mel_basis,
+                                            const int* filter_lohi, int B, int n_samples, int n_fft, int hop, int n_mels,
+                                            float clip_val, float* mel, void* stream) {
+    if (!audio || !table || !mel_basis || !filter_lohi || !mel)
+        return b2d::fail(B2D_ERR_NULL, "mel_spectrogram_keyshift: null pointer");
+    if ((uintptr_t)table & 7) return b2d::fail(B2D_ERR_ALIGN, "mel_spectrogram_keyshift: table not 8-byte aligned");
+    if (B <= 0 || B > 65535 || n_samples <= 0 || hop <= 0 || n_mels <= 0 || n_mels > 128)
+        return b2d::fail(B2D_ERR_SHAPE, "mel_spectrogram_keyshift: bad shape B=%d T=%d hop=%d n_mels=%d (n_mels <= 128)",
+                         B, n_samples, hop, n_mels);
+    if (n_fft < hop || n_fft > kKeyshiftMaxN)
+        return b2d::fail(B2D_ERR_UNSUPPORTED, "mel_spectrogram_keyshift: n_fft %d outside [hop = %d, %d]", n_fft, hop,
+                         kKeyshiftMaxN);
+    MelKeyshiftParams p;
+    p.y = audio; p.table = table; p.basis = mel_basis; p.lohi = filter_lohi; p.out = mel;
+    p.n_mels = n_mels; p.clip = clip_val;
+    if (keyshift_setup(p, n_samples, n_fft, hop) <= 0)
+        return b2d::fail(B2D_ERR_SHAPE, "mel_spectrogram_keyshift: signal too short");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int M = bluestein_size(n_fft, p.K);
+    const bool zu = 2 * n_fft <= M;
+    if (M == 1024) return zu ? launch_keyshift<1024, true>(p, B, st) : launch_keyshift<1024, false>(p, B, st);
+    if (M == 2048) return zu ? launch_keyshift<2048, true>(p, B, st) : launch_keyshift<2048, false>(p, B, st);
+    return zu ? launch_keyshift<4096, true>(p, B, st) : launch_keyshift<4096, false>(p, B, st);
+}
 
 extern "C" int b2d_mel_spectrogram(const float* audio, const float* window, const float* mel_basis, const int* filter_lohi,
                                    int B, int n_samples, int n_fft, int win_size, int hop, int n_mels, float clip_val,

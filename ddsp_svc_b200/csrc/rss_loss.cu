@@ -6,12 +6,8 @@
 //   loss_n   = mean_b ||S_t - S_p||_F / ||S_t + S_p||_F + alpha mean |log S_t - log S_p|
 //   loss     = sum_n loss_n / n_scale
 //
-// Any n in [256, 2047] (primes included) goes through Bluestein's chirp z-transform on the shared-memory Stockham FFT
-// of fft_smem.cuh, size M = 1024 / 2048 / 4096 (the smallest >= 2n - 1):
-//   X[k] = conj(c[k]) * (u (*) h)[k],   u[m] = z[m] conj(c[m]) (m < n, zero to M),   c[m] = exp(+i pi (m^2 mod 2n) / n)
-//   h    = c on [0, n) and its mirror on (M - n, M);  u (*) h = IFFT_M(FFT_M(u) * FFT_M(h))
-// FFT_M(h) / M and the chirp come from a per-n table built on the host in float64 (rounded once to fp32).  The inverse
-// FFT is a forward FFT read at (M - k) mod M.  The first FFT skips the zero upper half of u (n <= M / 2).
+// Any n in [256, 2047] (primes included) goes through Bluestein's chirp z-transform (bluestein.cuh) for all n bins: size
+// M = 1024 / 2048 / 4096, the smallest >= 2n - 1, so the first FFT skips the zero upper half of u (n <= M / 2).
 //
 // One CTA (128 threads) owns one frame of one row and runs two transforms side by side: the prediction's frame and the
 // target's (see transform_frames for why frames are not packed two to a transform).  Both signals go through the same
@@ -32,9 +28,10 @@
 #ifndef B2D_HOST_EMU               // tests/emu/ runs the kernels' source on the CPU (host_emu.h provides the shims)
 #include "b2d_common.cuh"
 #endif
-#include "fft_smem.cuh"
+#include "bluestein.cuh"
 
 using namespace b2d_fft;
+using namespace b2d_bluestein;
 using b2d_fft_smem::kThreads;
 using b2d_fft_smem::padi;
 
@@ -42,12 +39,8 @@ namespace {
 
 constexpr int kNMin = 256, kNMax = 2047, kMaxScales = 64;
 
-// per-n table (floats): [0] c = sqrt(sum w^2); window at kWinOff; chirp (n float2) at chirp_off(n); FFT_M(h) / M
-// (M float2) at hspec_off(n)
-constexpr int kWinOff = 4;
-__host__ __device__ __forceinline__ int chirp_off(int n) { return kWinOff + ((n + 3) & ~3); }
-__host__ __device__ __forceinline__ int hspec_off(int n) { return chirp_off(n) + 2 * n; }
-__host__ __device__ __forceinline__ int bluestein_size(int n) { return 2 * n - 1 <= 1024 ? 1024 : 2 * n - 1 <= 2048 ? 2048 : 4096; }
+// per-n table (bluestein.cuh's layout): [0] c = sqrt(sum w^2), then the window, the chirp and FFT_M(h) / M
+__host__ __device__ __forceinline__ int bluestein_size(int n) { return b2d_bluestein::bluestein_size(n, n); }
 
 template <int M> constexpr size_t smem_bytes() {
     return (size_t)2 * b2d_fft_smem::Plan<M>::kPad * sizeof(float2) +
@@ -80,28 +73,6 @@ template <int M> struct Smem {
         red = reinterpret_cast<float*>(tw3 + b2d_fft_smem::Plan<M>::kTw3);
     }
 };
-
-// Bluestein's DFT_n of the NB transforms at z0 (, z1): on entry slot m < n holds z[m] conj(c[m]) and [n, M/2) is zero;
-// on exit DFT_n(z)[k] = conj(c[k]) z[(M - k) mod M]  (read with bluestein_out)
-template <int M, int NB>
-__device__ __forceinline__ void bluestein_core(float2* z0, const float2* __restrict__ hspec, const float2* tw2,
-                                               const float2* tw3, int tid) {
-    constexpr int kPad = b2d_fft_smem::Plan<M>::kPad;
-    b2d_fft_smem::fft_forward<M, NB, true, true>(z0, tw2, tw3, tid);
-    for (int i = tid; i < M; i += kThreads) {
-        const float2 h = __ldg(hspec + i);
-        z0[padi(i)] = cmul(z0[padi(i)], h);
-        if (NB == 2) z0[kPad + padi(i)] = cmul(z0[kPad + padi(i)], h);
-    }
-    __syncthreads();
-    b2d_fft_smem::fft_forward<M, NB, true>(z0, tw2, tw3, tid);
-}
-
-template <int M>
-__device__ __forceinline__ float2 bluestein_out(const float2* z, const float2* __restrict__ chirp, int k) {
-    const float2 c = __ldg(chirp + k), v = z[padi((M - k) & (M - 1))];
-    return make_float2(fmaf(c.x, v.x, c.y * v.y), fmaf(c.x, v.y, -c.y * v.x));      // conj(c) v
-}
 
 // the windowed, chirped frame at x into z (w x conj(c) on [0, n)), zero on [n, M/2)
 template <int M>
@@ -259,7 +230,7 @@ __global__ void __launch_bounds__(kThreads) rss_bwd_kernel(RssParams p) {
 
 extern "C" int b2d_rss_table_floats(int n) {
     if (n < kNMin || n > kNMax) return 0;
-    return hspec_off(n) + 2 * bluestein_size(n);
+    return bluestein_table_floats(n, n);
 }
 
 extern "C" int b2d_rss_frames(int n_samples, int n) {

@@ -155,7 +155,26 @@ def _patch_units(saved):
                 setattr(mod, name, getattr(own, name))
 
 
-def patch_reference(reflow=False, diffusion=False, hifigan=False, rmvpe=False, units=False):
+_VOCODER_MODULES = ("diffusion.vocoder", "reflow.vocoder")
+
+
+def _patch_vocoder(saved):
+    """rebind Vocoder in the reference's diffusion.vocoder and reflow.vocoder (those that import); originals into
+    saved["vocoder"] by module"""
+    import importlib
+    from .nsf_vocoder import Vocoder
+    for modname in _VOCODER_MODULES:
+        try:
+            mod = importlib.import_module(modname)
+        except ImportError as e:
+            saved.setdefault("_not_patched", {})[modname] = "%s: %s" % (type(e).__name__, e)
+            continue
+        if hasattr(mod, "Vocoder"):
+            saved.setdefault("vocoder", {}).setdefault(modname, {})["Vocoder"] = mod.Vocoder
+            mod.Vocoder = Vocoder
+
+
+def patch_reference(reflow=False, diffusion=False, hifigan=False, rmvpe=False, units=False, vocoder=False):
     """Swap the synthesizer classes inside the (importable) reference package.  Returns the dict
     of original classes so a caller can restore them; its keys say what was patched.  If the enhancer stack
     (nsf_hifigan.models) cannot be imported, only the synthesizers are patched and the reason is returned under
@@ -192,12 +211,18 @@ def patch_reference(reflow=False, diffusion=False, hifigan=False, rmvpe=False, u
     to ``ddsp_svc_b200.Units_Encoder`` / ``ddsp_svc_b200.HubertSoft``, so main.py, the GUIs, the APIs and preprocess.py
     encode units on the kernels ('hubertsoft', the 'hubertbase*' and the 'contentvec*' encoders; fairseq checkpoints
     load without fairseq).  Off by default.  If encoder.hubert.model does not import, that is reported under
-    ``"_not_patched"``."""
+    ``"_not_patched"``.
+
+    ``vocoder=True`` rebinds ``Vocoder`` in diffusion.vocoder and reflow.vocoder to ``ddsp_svc_b200.Vocoder``, so
+    preprocess.py extracts its mels, the pitch-augmented ones included, and train_diff.py / main_diff.py extract and
+    vocode on the kernels.  preprocess.py and train_diff.py import ``Vocoder`` by name: patch before importing them.
+    Off by default; a module that does not import is reported under ``"_not_patched"``."""
     import ddsp.vocoder as ref_vocoder          # the reference checkout must be on sys.path
+    from . import vocoder as synths             # (the argument `vocoder` hides the module name here)
     names = ("Sins", "CombSub", "CombSubSuperFast", "CombSubFast")
     saved = {name: getattr(ref_vocoder, name) for name in names}
     for name in names:
-        setattr(ref_vocoder, name, getattr(vocoder, name))
+        setattr(ref_vocoder, name, getattr(synths, name))
     from . import frontend                      # Volume_Extractor (numpy in -> numpy out like the reference, computed on the GPU)
     saved["Volume_Extractor"] = ref_vocoder.Volume_Extractor
     ref_vocoder.Volume_Extractor = frontend.Volume_Extractor
@@ -230,6 +255,8 @@ def patch_reference(reflow=False, diffusion=False, hifigan=False, rmvpe=False, u
         _patch_rmvpe(saved)
     if units:
         _patch_units(saved)
+    if vocoder:
+        _patch_vocoder(saved)
     return saved
 
 
@@ -255,7 +282,7 @@ def unpatch_reference(saved):
                 if mod is not None and name in saved and hasattr(mod, name):
                     setattr(mod, name, saved[name])
     for modname, originals in (list(saved.get("diffusion", {}).items()) + list(saved.get("rmvpe", {}).items())
-                               + list(saved.get("units", {}).items())):
+                               + list(saved.get("units", {}).items()) + list(saved.get("vocoder", {}).items())):
         mod = sys.modules.get(modname)
         if mod is not None:
             for name, cls in originals.items():

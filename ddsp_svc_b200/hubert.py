@@ -30,7 +30,7 @@ import torch.nn.functional as F
 from torch.nn.modules.utils import consume_prefix_in_state_dict_if_present
 
 from . import ops
-from .rmvpe import resample_table, resampled_length
+from .rmvpe import Resampler
 from .unit2control import _Gemm, _split
 
 D_MODEL, N_HEADS, D_FFN, N_LAYERS, C_FEAT = 768, 12, 3072, 12, 512
@@ -440,23 +440,13 @@ class Units_Encoder:
             model = load_fairseq_hubert(encoder_ckpt)
             self.pad = 0
         self.model = model.eval().to(device)
-        self.resample_kernel = {}
+        self._resampler = Resampler(encoder_sample_rate)
+        self.resample_kernel = self._resampler.tables
         self.encoder_sample_rate = encoder_sample_rate
         self.encoder_hop_size = encoder_hop_size
-        self._lock = threading.Lock()
 
     def _resample(self, audio, sample_rate):
-        if sample_rate == self.encoder_sample_rate:
-            return audio
-        key = (str(sample_rate), audio.device)
-        with self._lock:
-            tab = self.resample_kernel.get(key)
-            if tab is None:
-                k, width, orig, new = resample_table(sample_rate, self.encoder_sample_rate)
-                tab = self.resample_kernel[key] = (k.to(audio.device), width, orig, new)
-        k, width, orig, new = tab
-        n_out = resampled_length(audio.shape[-1], sample_rate, self.encoder_sample_rate)
-        return ops.rmvpe_resample(audio, k, new, orig, width, n_out)
+        return self._resampler(audio, sample_rate)
 
     def _units(self, audio, sample_rate, flatten):
         if not (isinstance(audio, torch.Tensor) and audio.is_cuda):

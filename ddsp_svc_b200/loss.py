@@ -12,63 +12,41 @@ recomputes both spectra from the inputs.
 Not built (NotImplementedError): overlap != 0, scales outside [256, 2048], a gradient with respect to x_true.
 """
 import ctypes
-import threading
 
-import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, bluestein
 from .ops import _count, _need_cuda_f32, _stream
 
 N_MIN, N_MAX = 256, 2047
 MAX_SCALES = 64
 
-_tables = {}
-_tables_lock = threading.Lock()
-
 
 def bluestein_size(n):
     """the transform size the kernels use for n_fft = n: the smallest of 1024 / 2048 / 4096 that is >= 2n - 1"""
-    return next(M for M in (1024, 2048, 4096) if M >= 2 * n - 1)
+    return bluestein.size(n, n)
 
 
 def table_host(n):
-    """float32 table of csrc/rss_loss.cu for n_fft = n (see its layout): [0] c = sqrt(sum w^2) as torchaudio computes
-    it, the periodic Hann window (torch.hann_window), the chirp exp(+i pi (m^2 mod 2n) / n) and FFT_M(chirp filter) / M,
-    both computed in float64 from the integer m^2 mod 2n and rounded once"""
+    """float32 table of csrc/rss_loss.cu for n_fft = n (bluestein.py's layout, all n bins): [0] c = sqrt(sum w^2) as
+    torchaudio computes it, the periodic Hann window (torch.hann_window), the chirp and FFT_M(chirp filter) / M"""
     n = int(n)
     L = _lib.lib().b2d_rss_table_floats(n)
     if L <= 0:
         raise ValueError("n_fft=%d outside [%d, %d]" % (n, N_MIN, N_MAX))
-    M = bluestein_size(n)
     window = torch.hann_window(n)
-    chirp_off = 4 + ((n + 3) & ~3)
-    hspec_off = chirp_off + 2 * n
-    m = np.arange(n, dtype=np.int64)
-    chirp = np.exp(1j * np.pi * ((m * m) % (2 * n)).astype(np.float64) / n)
-    h = np.zeros(M, np.complex128)
-    h[:n] = chirp
-    h[M - n + 1:] = chirp[1:][::-1]
-    hspec = np.fft.fft(h) / M
-    t = np.zeros(L, np.float32)
-    t[0] = window.pow(2.0).sum().sqrt().item()
-    t[4:4 + n] = window.numpy()
-    t[chirp_off:chirp_off + 2 * n] = chirp.astype(np.complex64).view(np.float32)
-    t[hspec_off:hspec_off + 2 * M] = hspec.astype(np.complex64).view(np.float32)
+    t = bluestein.table_host(n, n, window.numpy(), head=[window.pow(2.0).sum().sqrt().item()])
+    assert t.size == L
     return t
+
+
+_cache = bluestein.TableCache(table_host)
+_tables = _cache.tables
 
 
 def table(n, device):
     """table_host(n) on ``device``, cached per (n, device)"""
-    key = (int(n), torch.device(device).index)
-    with _tables_lock:
-        t = _tables.get(key)
-        if t is None:
-            t = torch.from_numpy(table_host(n)).to(device)
-            # built once per device and then read from whatever stream the caller is on: make it visible to all of them
-            torch.cuda.current_stream().synchronize()
-            _tables[key] = t
-    return t
+    return _cache.get(n, device)
 
 
 def prebuild_tables(device, fft_min=N_MIN, fft_max=N_MAX + 1):

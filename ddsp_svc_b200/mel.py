@@ -8,13 +8,18 @@ Other shapes raise NotImplementedError (there is no PyTorch fallback in this pac
 grad mode is on), the result is differentiable with respect to ``y``: the backward runs ``mel_bwd_kernel`` (same file),
 which recomputes the spectra from ``y`` instead of storing them.
 
+``STFT.get_mel_keyshift(y, keyshift)`` is get_mel(y, keyshift=keyshift) for any shift whose transform length
+n' = round(2048 * 2^(keyshift / 12)) lies in [hop, 3072] (about -24 to +7.02 semitones at hop 512): one launch of
+``mel_keyshift_kernel`` (an n'-point Bluestein DFT, tables cached per (n', device)).  Forward only: preprocess.py's
+pitch augmentation and main_diff.py's formant shift differentiate nothing through it.
+
 The mel filterbank is librosa's (``librosa.filters.mel``, Slaney scale and normalisation: a third-party dependency of
 the reference, unpinned in requirements.txt and absent here); ``mel_filterbank`` restates its published algorithm.
 """
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, bluestein, ops
 from .ops import _count, _need_cuda_f32, _stream
 
 
@@ -75,6 +80,29 @@ def _bin_filters(basis):
     return np.stack([lo, hi], 1).astype(np.int32)
 
 
+KEYSHIFT_MAX_N = 3072
+
+
+def keyshift_n_fft(n_fft, keyshift):
+    """nvSTFT.py's shifted transform / window length: int(np.round(n_fft * 2 ** (keyshift / 12)))"""
+    return int(np.round(n_fft * 2 ** (keyshift / 12)))
+
+
+def keyshift_table_host(n):
+    """float32 table of mel_keyshift_kernel for n' = n (bluestein.py's layout, bins k < min(1025, n // 2 + 1)): the
+    periodic Hann window torch.hann_window(n) the reference frames with, the chirp and the filter spectrum"""
+    n = int(n)
+    L = _lib.lib().b2d_mel_keyshift_table_floats(n)
+    if L <= 0:
+        raise ValueError("n_fft=%d outside [1, %d]" % (n, KEYSHIFT_MAX_N))
+    t = bluestein.table_host(n, min(1025, n // 2 + 1), torch.hann_window(n).numpy())
+    assert t.size == L
+    return t
+
+
+_keyshift_tables = bluestein.TableCache(keyshift_table_host)
+
+
 class STFT:
     def __init__(self, sr=22050, n_mels=80, n_fft=1024, win_size=1024, hop_length=256, fmin=20, fmax=11025, clip_val=1e-5):
         self.target_sr = sr
@@ -132,6 +160,26 @@ class STFT:
                                          _stream()), "b2d_mel_spectrogram")
         _count(1)
         return out
+
+    def get_mel_keyshift(self, y, keyshift):
+        """y [B, T] CUDA fp32 -> log-mel [B, n_mels, n_frames] of get_mel(y, keyshift=keyshift) (nvSTFT.py:73-117 with
+        speed 1, center False).  A shift that rounds to n' = 2048 returns get_mel(y), bit for bit.  Forward only."""
+        if torch.is_grad_enabled() and isinstance(y, torch.Tensor) and y.requires_grad:
+            raise NotImplementedError("get_mel_keyshift has no backward (the pitch-augmented and formant-shifted mels "
+                                      "are data); call it under torch.no_grad() or pass y.detach()")
+        n, hop = keyshift_n_fft(self.n_fft, keyshift), int(self.hop_length)
+        if n != self.n_fft and not hop <= n <= KEYSHIFT_MAX_N:
+            lo = 12 * np.log2((hop - 0.5) / self.n_fft) if hop > 0 else float("-inf")
+            hi = 12 * np.log2((KEYSHIFT_MAX_N + 0.5) / self.n_fft)
+            raise NotImplementedError(
+                "the keyshift mel kernel covers transform lengths round(2048 * 2^(keyshift / 12)) in [hop, %d] = "
+                "[%d, %d], i.e. keyshift in about (%.2f, %.2f); got keyshift=%r (length %d)"
+                % (KEYSHIFT_MAX_N, hop, KEYSHIFT_MAX_N, lo, hi, keyshift, n))
+        y = self._checked(y, 0, 1, False)[0]
+        if n == self.n_fft:
+            return self._forward(y)
+        basis, lohi, _, _ = self._tables(y.device)
+        return ops.mel_keyshift(y, _keyshift_tables.get(n, y.device), basis, lohi, n, hop, self.clip_val)
 
     def get_mel_backward(self, y, grad_mel):
         """Gradient of get_mel(y) with respect to y for dL/dmel ``grad_mel`` [B, n_mels, n_frames] -> [B, n_samples].

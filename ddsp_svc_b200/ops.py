@@ -958,6 +958,28 @@ def rmvpe_mel(audio, window, basis, lohi, hop, t_pad):
     return out
 
 
+def mel_keyshift(y, table, basis, lohi, n_fft, hop, clip_val):
+    """y [B, T] -> key-shifted log-mel [B, n_mels, b2d_mel_frames(T, n_fft, n_fft, hop)] for the shifted transform length
+    n_fft, through its Bluestein ``table`` (mel.keyshift_table_host) (b2d_mel_spectrogram_keyshift)"""
+    _need_cuda_f32("y", y)
+    _need_cuda_f32("table", table)
+    _need_cuda_f32("basis", basis)
+    _need_cuda_f32("lohi", lohi, torch.int32)
+    if y.dim() != 2 or not y.is_contiguous() or basis.dim() != 2 or not basis.is_contiguous():
+        raise ValueError("y must be a contiguous [B, T] tensor and basis a contiguous [n_mels, 1025] one")
+    B, T = y.shape
+    L = _lib.lib()
+    n_frames = L.b2d_mel_frames(T, int(n_fft), int(n_fft), int(hop))
+    if n_frames <= 0:
+        raise ValueError("signal of %d samples is too short for one frame" % T)
+    out = torch.empty(B, basis.shape[0], n_frames, dtype=torch.float32, device=y.device)
+    _lib.check(L.b2d_mel_spectrogram_keyshift(y.data_ptr(), table.data_ptr(), basis.data_ptr(), lohi.data_ptr(), B, T,
+                                              int(n_fft), int(hop), int(basis.shape[0]), float(clip_val), out.data_ptr(),
+                                              _stream()), "b2d_mel_spectrogram_keyshift")
+    _count(1)
+    return out
+
+
 def rmvpe_decode(salience, n_frames, thred):
     """salience [B, t_pad, 360] -> f0 [B, n_frames] in Hz, 0 where unvoiced (b2d_rmvpe_decode)"""
     _need_cuda_f32("salience", salience)

@@ -306,6 +306,30 @@ def resampled_length(n, orig_freq, new_freq=SAMPLE_RATE):
     return -(-w * n // o)
 
 
+class Resampler:
+    """torchaudio Resample(orig_freq, new_freq, lowpass_filter_width=128) of CUDA [B, N] audio on the kernels
+    (ops.rmvpe_resample), the polyphase table of each (orig_freq, device) built once: ``resampler(audio, orig_freq)``.
+    ``tables`` maps (str(orig_freq), device) to (table, width, orig / gcd, new / gcd)."""
+
+    def __init__(self, new_freq):
+        self.new_freq = int(new_freq)
+        self.tables = {}
+        self._lock = threading.Lock()
+
+    def __call__(self, audio, orig_freq):
+        orig_freq = int(orig_freq)
+        if orig_freq == self.new_freq:
+            return audio
+        key = (str(orig_freq), audio.device)
+        with self._lock:
+            tab = self.tables.get(key)
+            if tab is None:
+                k, width, orig, new = resample_table(orig_freq, self.new_freq)
+                tab = self.tables[key] = (k.to(audio.device), width, orig, new)
+        k, width, orig, new = tab
+        return ops.rmvpe_resample(audio, k, new, orig, width, resampled_length(audio.shape[-1], orig_freq, self.new_freq))
+
+
 def mel_basis():
     """spec.py's basis: librosa.filters.mel(sr=16000, n_fft=1024, n_mels=128, fmin=30, fmax=8000, htk=True)"""
     return mel_filterbank(SAMPLE_RATE, WINDOW_LENGTH, N_MELS, MEL_FMIN, MEL_FMAX, htk=True)

@@ -530,6 +530,19 @@ int b2d_mel_spectrogram_backward(const float* audio, const float* window, const 
                                  const int* bin_filter_range, int B, int n_samples, int n_fft, int win_size, int hop,
                                  int n_mels, float clip_val, const float* grad_mel, int64_t grad_stride_b,
                                  int64_t grad_stride_mel, int64_t grad_stride_frame, float* grad_audio, void* stream);
+/* Key-shifted log-mel (STFT.get_mel with keyshift != 0, speed 1; forward only).  n_fft = n' = round(2048 *
+ * 2^(keyshift / 12)) is the transform and window length, hop <= n' <= 3072 (B2D_ERR_UNSUPPORTED otherwise): padding by
+ * (n' - hop)/2 as nvSTFT.py does for win_size n', periodic Hann(n') frames, the n'-point DFT's bins k < K = min(1025,
+ * n'/2 + 1), magnitude sqrt(re^2 + im^2 + 1e-9) * 2048 / n' (bins K..1024 zero), the unshifted mel_basis [n_mels, 1025]
+ * (n_mels <= 128) and log(max(., clip_val)) -> mel [B, n_mels, b2d_mel_frames(n_samples, n', n', hop)].
+ * table: b2d_mel_keyshift_table_floats(n') floats (device, 8-byte aligned) for this n': [4, 4 + n') the window, then
+ * the Bluestein chirp exp(+i pi (m^2 mod 2n') / n') at 4 + ((n' + 3) & ~3) (n' complex) and FFT_M(h) / M right after
+ * it (M complex), M the smallest of 1024 / 2048 / 4096 >= n' + K - 1, h the chirp on [0, K) and mirrored on
+ * (M - n', M).  Deterministic (no atomics).  Argument errors return before any CUDA call. */
+int b2d_mel_keyshift_table_floats(int n_fft);
+int b2d_mel_spectrogram_keyshift(const float* audio, const float* table, const float* mel_basis, const int* filter_lohi,
+                                 int B, int n_samples, int n_fft, int hop, int n_mels, float clip_val, float* mel,
+                                 void* stream);
 
 /* ---- random-scale spectral loss (RSSLoss, ddsp/loss.py:9-54; the loss of configs/combsub.yaml and sins.yaml) ------------
  * Per scale n = n_ffts[s] (host array, 256 <= n <= 2047, n <= n_samples): frames of n samples at hop n (no overlap,
