@@ -84,6 +84,8 @@ inline CombSubWorkspace combsub_workspace(int B, int nF, int block, int n_mag_al
 // ---------------------------------------------------------------------------------------
 #define B2D_PI_F 3.14159265358979323846f
 #define B2D_TWO_PI_F 6.28318530717958647692f
+// a static shared-memory array; tests/emu/host_emu.h gives each emulated CTA its own copy
+#define B2D_SHARED(T, name, dims) __shared__ T name dims
 
 namespace b2d {
 

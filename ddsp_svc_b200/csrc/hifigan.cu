@@ -23,7 +23,9 @@
 //
 // No atomics and no global mutable state: every output element has one writer and a fixed summation order, so results
 // are bit-identical from run to run, and concurrent calls from several host threads are independent.
+#ifndef B2D_HOST_EMU               // tests/emu/ runs these kernels' source on the CPU (host_emu.h provides the shims)
 #include "b2d_common.cuh"
+#endif
 #include "mma_sync.cuh"
 #include "tf32_split.cuh"
 
@@ -258,6 +260,7 @@ __global__ void __launch_bounds__(256) hg_post_kernel(const float* __restrict__ 
     }
 }
 
+#ifndef B2D_HOST_EMU
 template <int BM, int BN>
 int launch_conv(const HgConvParams& p, cudaStream_t st) {
     const int halo = p.dil * (p.k - 1) / 2;
@@ -271,9 +274,11 @@ int launch_conv(const HgConvParams& p, cudaStream_t st) {
     kern<<<grid, kWarps * 32, smem, st>>>(p);
     return b2d::check_launch("hifigan_conv");
 }
+#endif  // B2D_HOST_EMU
 
 }  // namespace
 
+#ifndef B2D_HOST_EMU
 namespace b2d {
 
 // BN: 32, or 16 when it does not divide N.  BM = 128 rows, or 64 when 128-row tiles would leave the grid under
@@ -304,3 +309,4 @@ int hifigan_post_launch(const float* x, const float* w, const float* bias, int B
 }
 
 }  // namespace b2d
+#endif  // B2D_HOST_EMU

@@ -25,7 +25,9 @@
 //
 // No atomics: every output element has one writer and a fixed summation order, so results are bit-identical from run
 // to run.
+#ifndef B2D_HOST_EMU               // tests/emu/ runs these kernels' source on the CPU (host_emu.h provides the shims)
 #include "b2d_common.cuh"
+#endif
 #include "tf32_split.cuh"
 
 namespace {
@@ -47,7 +49,7 @@ __device__ __forceinline__ float hb_gelu(float x) { return (x * 0.5f) * (1.0f + 
 __global__ void __launch_bounds__(256) hb_conv0_kernel(const float* __restrict__ x, int N, int pad,
                                                        const float* __restrict__ w, int L0, int La,
                                                        float* __restrict__ y, double* __restrict__ part) {
-    __shared__ float s[5 * (kConv0Tile - 1) + 10];
+    B2D_SHARED(float, s, [5 * (kConv0Tile - 1) + 10]);
     const int tile = blockIdx.x, b = blockIdx.y, t0 = tile * kConv0Tile;
     const int n_tiles = gridDim.x;
     const float* xb = x + (size_t)b * N;
@@ -325,13 +327,16 @@ __global__ void __launch_bounds__(256) hb_align_kernel(const float* __restrict__
     }
 }
 
+#ifndef B2D_HOST_EMU
 unsigned hb_grid(size_t n) {
     const size_t blocks = (n + 255) / 256, cap = (size_t)b2d::num_sms() * 16;
     return (unsigned)(blocks < cap ? (blocks ? blocks : 1) : cap);
 }
+#endif  // B2D_HOST_EMU
 
 }  // namespace
 
+#ifndef B2D_HOST_EMU
 namespace b2d {
 
 int hubert_conv0_launch(const float* x, int B, int N, int pad, const float* w, int L0, int La, float* y, double* part,
@@ -393,3 +398,4 @@ int hubert_align_launch(const float* units, int B, int T, int C, float ratio, in
 }
 
 }  // namespace b2d
+#endif  // B2D_HOST_EMU

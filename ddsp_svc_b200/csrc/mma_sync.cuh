@@ -1,6 +1,7 @@
 // cp.async staging and the mma.sync m16n8k8 TF32 tensor-core product shared by the implicit-GEMM convolutions
 // (hifigan.cu, rmvpe.cu).
 #pragma once
+#ifndef B2D_HOST_EMU               // tests/emu/host_emu.h models these three and mma_tf32 from the PTX ISA
 #include <cstdint>
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
@@ -16,3 +17,4 @@ __device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], 
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
+#endif  // B2D_HOST_EMU

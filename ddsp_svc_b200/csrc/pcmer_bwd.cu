@@ -12,7 +12,7 @@
 // No atomics and no shared memory: every output element has one owning warp and every sum runs over one row in a fixed
 // butterfly order, so results are bit-identical from run to run.  A warp past the last row still joins the shuffles (the
 // row index is clamped) and only skips its stores: every warp of a CTA runs the same shuffle sequence.
-#ifndef B2D_HOST_EMU               // tests/emu/ runs this source on the CPU (host_emu.h + the driver's shuffle shim)
+#ifndef B2D_HOST_EMU               // tests/emu/ runs this source on the CPU (host_emu.h provides the shims)
 #include "b2d_common.cuh"
 #endif
 

@@ -29,9 +29,11 @@
 //
 // No atomics and no global mutable state: every output element has one writer and a fixed summation order, so results
 // are bit-identical from run to run.
+#ifndef B2D_HOST_EMU               // tests/emu/ runs these kernels' source on the CPU (host_emu.h provides the shims)
 #include <cooperative_groups.h>
 
 #include "b2d_common.cuh"
+#endif
 #include "fft_smem.cuh"
 #include "mma_sync.cuh"
 #include "tf32_split.cuh"
@@ -219,6 +221,7 @@ __global__ void __launch_bounds__(kWarps * 32) rv_conv_kernel(RvConvParams p) {
         }
 }
 
+#ifndef B2D_HOST_EMU
 template <int BM, int BN>
 int launch_conv(RvConvParams p, cudaStream_t st) {
     p.tF = p.F < BM / 4 ? p.F : BM / 4;
@@ -239,6 +242,7 @@ int launch_conv(RvConvParams p, cudaStream_t st) {
     kern<<<grid, kWarps * 32, smem, st>>>(p);
     return b2d::check_launch("rmvpe_conv");
 }
+#endif  // B2D_HOST_EMU
 
 // ---------------------------------------------------------------------------------------------------------------------
 // rv_conv_small: one thread per output pixel, every output channel
@@ -334,8 +338,8 @@ __global__ void __cluster_dims__(kGruCta, 1, 1) __launch_bounds__(kGruThreads, 1
     rv_gru_kernel(const float* __restrict__ xg, const float* __restrict__ whh, const float* __restrict__ bhh, int B,
                   int T, float* __restrict__ out) {
     cg::cluster_group cluster = cg::this_cluster();
-    __shared__ float hbuf[2][kGruB][kGruH];
-    __shared__ float red[kGruThreads / 32][kGruB][12];
+    B2D_SHARED(float, hbuf, [2][kGruB][kGruH]);
+    B2D_SHARED(float, red, [kGruThreads / 32][kGruB][12]);
     const int rank = (int)cluster.block_rank(), dir = blockIdx.x / kGruCta;
     const int b0 = blockIdx.y * kGruB, nb = min(kGruB, B - b0);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -528,13 +532,16 @@ __global__ void __launch_bounds__(256) rv_decode_kernel(const float* __restrict_
     }
 }
 
+#ifndef B2D_HOST_EMU
 unsigned grid_for(long long n, int threads) {
     const long long g = (n + threads - 1) / threads, cap = (long long)b2d::num_sms() * 16;
     return (unsigned)(g < 1 ? 1 : (g > cap ? cap : g));
 }
+#endif  // B2D_HOST_EMU
 
 }  // namespace
 
+#ifndef B2D_HOST_EMU
 namespace b2d {
 
 // BN: 32, or 16 when it does not divide N.  BM = 128 pixels, or 64 when 128-pixel tiles would leave the grid under two
@@ -594,3 +601,4 @@ int rmvpe_decode_launch(const float* sal, int B, int t_pad, int n_frames, float 
 }
 
 }  // namespace b2d
+#endif  // B2D_HOST_EMU

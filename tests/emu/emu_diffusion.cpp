@@ -7,8 +7,6 @@
 namespace emu_df { inline dim3 grid_dim, block_dim; }
 #define gridDim (emu_df::grid_dim)
 #define blockDim (emu_df::block_dim)
-inline uint32_t __float_as_uint(float f) { uint32_t u; std::memcpy(&u, &f, 4); return u; }
-inline float __uint_as_float(uint32_t u) { float f; std::memcpy(&f, &u, 4); return f; }
 
 #include "../../ddsp_svc_b200/csrc/diffusion.cu"
 

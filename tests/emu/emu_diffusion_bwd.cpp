@@ -7,8 +7,6 @@
 namespace emu_dfb { inline dim3 grid_dim, block_dim; }
 #define gridDim (emu_dfb::grid_dim)
 #define blockDim (emu_dfb::block_dim)
-inline uint32_t __float_as_uint(float f) { uint32_t u; std::memcpy(&u, &f, 4); return u; }
-inline float __uint_as_float(uint32_t u) { float f; std::memcpy(&f, &u, 4); return f; }
 inline float __int_as_float(int i) { float f; std::memcpy(&f, &i, 4); return f; }
 
 #include "../../ddsp_svc_b200/csrc/diffusion_bwd.cu"

@@ -7,8 +7,6 @@
 namespace emu_rf { inline dim3 grid_dim, block_dim; }
 #define gridDim (emu_rf::grid_dim)
 #define blockDim (emu_rf::block_dim)
-inline uint32_t __float_as_uint(float f) { uint32_t u; std::memcpy(&u, &f, 4); return u; }
-inline float __uint_as_float(uint32_t u) { float f; std::memcpy(&f, &u, 4); return f; }
 using std::erff;
 
 #include "../../ddsp_svc_b200/csrc/reflow_bwd.cu"

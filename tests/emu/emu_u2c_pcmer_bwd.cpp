@@ -1,27 +1,6 @@
 // CPU execution of csrc/pcmer_bwd.cu's kernel sources (see host_emu.h).  Built by tests/test_emu_u2c_pcmer_backward.py.
-// host_emu.h has no warp intrinsics, so __shfl_xor_sync is provided here: every thread of the emulated CTA writes its
-// value to a slot, the CTA meets at a barrier, reads its partner's slot (lane ^ d stays inside the warp) and meets again.
-// That needs every thread of the CTA to run the same sequence of shuffles, which the kernels guarantee (a warp past the
-// last row clamps its row index and still joins them).
 #define B2D_HOST_EMU 1
 #include "host_emu.h"
-
-namespace emu_shfl { inline float f[256]; inline int i[256]; }
-inline float __shfl_xor_sync(unsigned, float v, int d) {
-    emu_shfl::f[threadIdx.x] = v;
-    emu::sync();
-    const float r = emu_shfl::f[threadIdx.x ^ d];
-    emu::sync();
-    return r;
-}
-inline int __shfl_xor_sync(unsigned, int v, int d) {
-    emu_shfl::i[threadIdx.x] = v;
-    emu::sync();
-    const int r = emu_shfl::i[threadIdx.x ^ d];
-    emu::sync();
-    return r;
-}
-inline float rsqrtf(float x) { return 1.0f / std::sqrt(x); }
 
 #include "../../ddsp_svc_b200/csrc/pcmer_bwd.cu"
 

@@ -54,6 +54,22 @@ def tsan(source, tmp_path, define=None, *args):
                           env=dict(os.environ, TSAN_OPTIONS="halt_on_error=0 exitcode=66"))
 
 
+def asan(source, tmp_path, define=None, *args):
+    """tests/emu/<source> (with -D<define>) built under AddressSanitizer and UndefinedBehaviorSanitizer and run with
+    `args`: the completed process.  Any report makes the run exit with 66."""
+    _need_gxx()
+    exe = str(tmp_path / (os.path.splitext(source)[0] + "_asan"))
+    cmd = GXX + ["-O1", "-g", "-ffp-contract=off", "-fsanitize=address,undefined", "-fno-sanitize-recover=all"]
+    cmd += ["-D" + define] if define else []
+    proc = subprocess.run(cmd + ["-o", exe, os.path.join(EMU, source)], capture_output=True, text=True)
+    if proc.returncode != 0 and "asan" in proc.stderr.lower():
+        pytest.skip("AddressSanitizer runtime not available: " + proc.stderr.strip().splitlines()[-1])
+    assert proc.returncode == 0, proc.stderr
+    return subprocess.run([exe, *args], capture_output=True, text=True, timeout=900,
+                          env=dict(os.environ, ASAN_OPTIONS="exitcode=66:detect_leaks=0",
+                                   UBSAN_OPTIONS="exitcode=66:print_stacktrace=1"))
+
+
 def assert_race_free(res):
     assert "ThreadSanitizer" not in res.stderr, res.stderr[-4000:]
     assert res.returncode == 0

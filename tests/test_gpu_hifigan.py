@@ -108,6 +108,51 @@ def test_transposed_conv_with_source(stage, B, T):
     assert rel < CONV_RMS and mx < CONV_MAX, (rel, mx)
 
 
+def _takes_128_rows(T, N, B):
+    """hifigan_conv_launch's choice: BM = 128 unless 128-row tiles leave the grid under two CTAs per SM"""
+    BN = 32 if N % 32 == 0 else 16
+    return -(-T // 128) * (N // BN) * B >= 2 * torch.cuda.get_device_properties(0).multi_processor_count
+
+
+@pytest.mark.parametrize("C,k,d", [(32, 11, 5), (16, 7, 3)])
+def test_resblock_conv_on_the_128_row_tile(C, k, d):
+    """B 2 and T long enough for <128, 32> (C 32) and <128, 16> (C 16), with a T % 128 tail and + residual"""
+    B = 2
+    T = 128 * (-(-2 * torch.cuda.get_device_properties(0).multi_processor_count // ((C // (32 if C % 32 == 0 else 16))
+                                                                                  * B))) + 37
+    assert _takes_128_rows(T, C, B)
+    w, b = _rand(C, C, k, seed=C + k, scale=1.0 / (C * k) ** 0.5), _rand(C, seed=d, scale=0.1)
+    x, res = _rand(B, T, C, seed=5), _rand(B, T, C, seed=6)
+    ref = F.conv1d(_lrelu(x, True).transpose(1, 2), w, b, padding=d * (k - 1) // 2, dilation=d).transpose(1, 2) + res
+    out = ops.hifigan_conv(x.float().to(DEV), hifigan.pack_conv(w.float().to(DEV)), b.float().to(DEV), k, d, C, True,
+                           residual=res.float().to(DEV))
+    rel, mx = _err(out, ref)
+    report.record("hifigan/resblock_bm128/C%d_k%d_d%d/%d" % (C, k, d, T), rel_rms=rel, rel_max=mx)
+    assert rel < CONV_RMS and mx < CONV_MAX, (rel, mx)
+
+
+@pytest.mark.parametrize("stage", [3, 4])
+def test_transposed_conv_on_the_128_row_tile(stage):
+    """the last two stages (N = u C_out = 64, BN 32; 32, BN 32) at B 2 and T long enough for BM = 128"""
+    Cin, Cout, u, s = STAGES[stage]
+    nk, pad = (2 * s, s // 2) if stage < 4 else (1, 0)
+    B, N = 2, u * Cout
+    T = 128 * (-(-2 * torch.cuda.get_device_properties(0).multi_processor_count // ((N // 32) * B))) + 5
+    assert _takes_128_rows(T, N, B)
+    w, b = _rand(Cin, Cout, 2 * u, seed=stage, scale=1.0 / Cin ** 0.5), _rand(Cout, seed=9, scale=0.1)
+    wn, bn = _rand(Cout, 1, nk, seed=10, scale=1.0 / nk ** 0.5), _rand(Cout, seed=11, scale=0.1)
+    x, har = _rand(B, T, Cin, seed=12), torch.tanh(_rand(B, T * u * s, 1, seed=13))
+    ref = (F.conv_transpose1d(_lrelu(x, True).transpose(1, 2), w, b, stride=u, padding=u // 2) +
+           F.conv1d(har.transpose(1, 2), wn, bn, stride=s, padding=pad)).transpose(1, 2)
+    out = ops.hifigan_conv(x.float().to(DEV), hifigan.pack_conv(hifigan.polyphase(w.float().to(DEV), u)),
+                           b.float().to(DEV), 3, 1, N, True, up=u, source=har.float().to(DEV),
+                           noise_w=wn.float().reshape(Cout, nk).to(DEV), noise_b=bn.float().to(DEV), noise_stride=s,
+                           noise_pad=pad)
+    rel, mx = _err(out, ref)
+    report.record("hifigan/ups_bm128/%d/%dx%d" % (stage, B, T), rel_rms=rel, rel_max=mx)
+    assert rel < CONV_RMS and mx < CONV_MAX, (rel, mx)
+
+
 @pytest.mark.parametrize("B,T", [(1, 1), (2, 4096), (3, 5000)])
 def test_post(B, T):
     w, b = _rand(1, 16, 7, seed=14, scale=0.1), _rand(1, seed=15, scale=0.1)
