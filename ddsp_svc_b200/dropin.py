@@ -174,7 +174,20 @@ def _patch_vocoder(saved):
             mod.Vocoder = Vocoder
 
 
-def patch_reference(reflow=False, diffusion=False, hifigan=False, rmvpe=False, units=False, vocoder=False):
+def _patch_enhancer(saved):
+    """rebind Enhancer in the reference's enhancer module; the original into saved["enhancer"]"""
+    try:
+        import enhancer as ref_enhancer
+    except ImportError as e:
+        saved.setdefault("_not_patched", {})["enhancer"] = "%s: %s" % (type(e).__name__, e)
+        return
+    from .enhancer import Enhancer
+    saved.setdefault("enhancer", {})["enhancer"] = {"Enhancer": ref_enhancer.Enhancer}
+    ref_enhancer.Enhancer = Enhancer
+
+
+def patch_reference(reflow=False, diffusion=False, hifigan=False, rmvpe=False, units=False, vocoder=False,
+                    enhancer=False):
     """Swap the synthesizer classes inside the (importable) reference package.  Returns the dict
     of original classes so a caller can restore them; its keys say what was patched.  If the enhancer stack
     (nsf_hifigan.models) cannot be imported, only the synthesizers are patched and the reason is returned under
@@ -216,7 +229,12 @@ def patch_reference(reflow=False, diffusion=False, hifigan=False, rmvpe=False, u
     ``vocoder=True`` rebinds ``Vocoder`` in diffusion.vocoder and reflow.vocoder to ``ddsp_svc_b200.Vocoder``, so
     preprocess.py extracts its mels, the pitch-augmented ones included, and train_diff.py / main_diff.py extract and
     vocode on the kernels.  preprocess.py and train_diff.py import ``Vocoder`` by name: patch before importing them.
-    Off by default; a module that does not import is reported under ``"_not_patched"``."""
+    Off by default; a module that does not import is reported under ``"_not_patched"``.
+
+    ``enhancer=True`` rebinds ``Enhancer`` in the reference's enhancer module to ``ddsp_svc_b200.enhancer.Enhancer``:
+    resampling, f0 regridding, mel and vocoder on the kernels, and no host round trip for a numeric adaptive key.
+    main.py and the GUIs import ``Enhancer`` by name: patch before importing them.  Off by default; if the module does
+    not import, that is reported under ``"_not_patched"``."""
     import ddsp.vocoder as ref_vocoder          # the reference checkout must be on sys.path
     from . import vocoder as synths             # (the argument `vocoder` hides the module name here)
     names = ("Sins", "CombSub", "CombSubSuperFast", "CombSubFast")
@@ -257,6 +275,8 @@ def patch_reference(reflow=False, diffusion=False, hifigan=False, rmvpe=False, u
         _patch_units(saved)
     if vocoder:
         _patch_vocoder(saved)
+    if enhancer:
+        _patch_enhancer(saved)
     return saved
 
 
@@ -282,7 +302,8 @@ def unpatch_reference(saved):
                 if mod is not None and name in saved and hasattr(mod, name):
                     setattr(mod, name, saved[name])
     for modname, originals in (list(saved.get("diffusion", {}).items()) + list(saved.get("rmvpe", {}).items())
-                               + list(saved.get("units", {}).items()) + list(saved.get("vocoder", {}).items())):
+                               + list(saved.get("units", {}).items()) + list(saved.get("vocoder", {}).items())
+                               + list(saved.get("enhancer", {}).items())):
         mod = sys.modules.get(modname)
         if mod is not None:
             for name, cls in originals.items():

@@ -1132,3 +1132,61 @@ def hubert_align(units, ratio, n_frames):
                                            _stream()), "b2d_hubert_align")
     _count(1)
     return out
+
+
+def _need_vector(name, t, n=None):
+    _need_cuda_f32(name, t)
+    if t.dim() != 1 or not t.is_contiguous() or (n is not None and t.numel() < n):
+        raise ValueError("%s must be a contiguous 1-D tensor%s, got %s"
+                         % (name, "" if n is None else " of at least %d samples" % n, tuple(t.shape)))
+
+
+def rt_f0_regrid(src, src_step, n_dst, dst_step, src_div=1.0, src_scale=1.0, rmvpe=False, pad=0, f0_min=0.0,
+                 post_scale=1.0):
+    """np.interp of src [n] from positions (src_step i) / src_div to positions dst_step j -> [n_dst] (b2d_rt_f0_regrid).
+    rmvpe=False: src times src_scale first (Enhancer's real_factor).  rmvpe=True: F0_Extractor's 'rmvpe'
+    post-processing with uv_interp, `pad` leading frames, the clamp to f0_min and the pitch factor post_scale."""
+    _need_vector("src", src)
+    n_src = src.numel()
+    L = _lib.lib()
+    out = torch.empty(int(n_dst), dtype=torch.float32, device=src.device)
+    nbytes = L.b2d_rt_f0_regrid_workspace_bytes(n_src, int(n_dst))
+    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=src.device)
+    _lib.check(L.b2d_rt_f0_regrid(src.data_ptr(), n_src, float(src_step), float(src_div), float(src_scale), int(n_dst),
+                                  int(pad), float(dst_step), 1 if rmvpe else 0, float(f0_min), float(post_scale),
+                                  out.data_ptr(), ws.data_ptr(), nbytes, _stream()), "b2d_rt_f0_regrid")
+    _count(1)
+    return out
+
+
+def rt_sola(x, buf, search):
+    """the SOLA shift of gui.py's callback -> int32 [1] on the device: the first s <= search maximising the normalised
+    cross-correlation of x[s:][:crossfade] with buf [crossfade] (b2d_rt_sola)"""
+    _need_vector("buf", buf)
+    _need_vector("x", x, buf.numel() + int(search))
+    shift = torch.empty(1, dtype=torch.int32, device=x.device)
+    _lib.check(_lib.lib().b2d_rt_sola(x.data_ptr(), buf.data_ptr(), buf.numel(), int(search), shift.data_ptr(),
+                                      _stream()), "b2d_rt_sola")
+    _count(1)
+    return shift
+
+
+def rt_crossfade(x, shift, search, buf, fade_in, fade_out, block, phase_vocoder=False):
+    """gui.py's crossfade at the device-side shift (int32 [1], <= search) -> (out [block], next_buf [crossfade]): the
+    linear sin^2 fade or phase_vocoder over the first crossfade samples of x[shift:] (b2d_rt_crossfade)"""
+    cf = buf.numel()
+    _need_vector("buf", buf)
+    _need_vector("fade_in", fade_in, cf)
+    _need_vector("fade_out", fade_out, cf)
+    _need_vector("x", x, int(search) + int(block) + cf)
+    _need_cuda_f32("shift", shift, torch.int32)
+    L = _lib.lib()
+    out = torch.empty(int(block), dtype=torch.float32, device=x.device)
+    next_buf = torch.empty(cf, dtype=torch.float32, device=x.device)
+    nbytes = L.b2d_rt_crossfade_workspace_bytes(cf, int(bool(phase_vocoder)))
+    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=x.device)
+    _lib.check(L.b2d_rt_crossfade(x.data_ptr(), shift.data_ptr(), buf.data_ptr(), fade_in.data_ptr(), fade_out.data_ptr(),
+                                  int(block), cf, int(bool(phase_vocoder)), out.data_ptr(), next_buf.data_ptr(),
+                                  ws.data_ptr(), nbytes, _stream()), "b2d_rt_crossfade")
+    _count(2 if phase_vocoder else 1)
+    return out, next_buf

@@ -688,6 +688,33 @@ int b2d_hubert_posconv(const float* x, int B, int T, const float* w, const float
 int b2d_hubert_attention(const float* qkv, int B, int T, float* hi, float* lo, void* stream);
 int b2d_hubert_align(const float* units, int B, int T, int C, float ratio, int n_frames, float* out, void* stream);
 
+/* ---- real-time conversion block of gui.py (realtime.cu), B = 1 -----------------------------------------------------
+ * b2d_rt_f0_regrid: np.interp between uniform grids in fp64 as numpy computes it, values held at the edges.  Source
+ *   position i is (src_step i) / src_div, target position of frame j >= pad is dst_step (j - pad); out [n_dst] fp32.
+ *   mode 0 (Enhancer.enhance, enhancer.py:65-70): src times src_scale in fp32, regridded; pad must be 0.
+ *   mode 1 (F0_Extractor 'rmvpe' with uv_interp, ddsp/vocoder.py:108-118, :138-144): unvoiced (zero) src frames filled
+ *   from their voiced neighbours and rounded to fp32; f0 and the uv flag regridded, zero where the regridded uv > 0.5;
+ *   `pad` leading zero frames; unvoiced frames filled again in fp64; values below f0_min set to f0_min; then times
+ *   post_scale in fp32.  A fill with no voiced frame leaves the values as they are.  src_scale is ignored in mode 1,
+ *   f0_min and post_scale in mode 0.  workspace: b2d_rt_f0_regrid_workspace_bytes(n_src, n_dst), 16-byte aligned.
+ * b2d_rt_sola: shift[0] = the first s in [0, search] maximising sum_k x[s + k] buf[k] / sqrt(sum_k x[s + k]^2 + 1e-8),
+ *   k < crossfade (gui.py:434-440); x holds crossfade + search samples.
+ * b2d_rt_crossfade: y[t] = x[shift[0] + t], t < block + crossfade, with y[:crossfade] the linear fade
+ *   x fade_in + buf fade_out (gui.py:451-452) or, with phase_vocoder, phase_vocoder(buf, x[shift:][:crossfade],
+ *   fade_out, fade_in) (gui.py:15-31) by a direct DFT and synthesis sum.  out [block] = y[:block], next_buf [crossfade]
+ *   = y[block:]; neither may overlap buf.  crossfade <= 32768 (B2D_ERR_UNSUPPORTED).  workspace:
+ *   b2d_rt_crossfade_workspace_bytes(crossfade, phase_vocoder) bytes (none for the linear fade).
+ * No atomics and no host synchronisation: bit-identical from run to run and capturable in a CUDA graph. */
+size_t b2d_rt_f0_regrid_workspace_bytes(int n_src, int n_dst);
+int b2d_rt_f0_regrid(const float* src, int n_src, double src_step, double src_div, float src_scale, int n_dst, int pad,
+                     double dst_step, int mode, double f0_min, float post_scale, float* out, void* workspace,
+                     size_t workspace_bytes, void* stream);
+int b2d_rt_sola(const float* x, const float* buf, int crossfade, int search, int* shift, void* stream);
+size_t b2d_rt_crossfade_workspace_bytes(int crossfade, int phase_vocoder);
+int b2d_rt_crossfade(const float* x, const int* shift, const float* buf, const float* fade_in, const float* fade_out,
+                     int block, int crossfade, int phase_vocoder, float* out, float* next_buf, void* workspace,
+                     size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
