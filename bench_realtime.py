@@ -83,7 +83,8 @@ class GuiBlock:
         self.input_wav = np.zeros(s.n_in, dtype=np.float32)
         self.sola_buffer = torch.zeros(s.cf, device=s.device)
 
-    def __call__(self, indata):
+    def front(self, indata):
+        """the ring buffer, f0, volume, the upsampled mask and the units of SvcDDSP.infer"""
         from ddsp_svc_b200 import frontend
         s, dev = self.s, self.s.device
         self.input_wav[:] = np.roll(self.input_wav, -s.block)
@@ -100,6 +101,11 @@ class GuiBlock:
         mask = F.interpolate(torch.cat((mask, mask[:, :, -1:]), 2), size=mask.shape[-1] * s.block_size + 1,
                              mode="linear", align_corners=True)[:, :, :-1].permute(0, 2, 1).squeeze(-1)
         units = s.units_encoder.encode(audio_t, s.sr, s.hop)
+        return f0, volume, mask, units
+
+    def __call__(self, indata):
+        s = self.s
+        f0, volume, mask, units = self.front(indata)
         with torch.no_grad():
             out, _, _ = s.model(units, f0, volume[..., None], spk_id=s.spk_id, spk_mix_dict=s.spk_mix_dict,
                                 noise=s.noise)
@@ -110,9 +116,14 @@ class GuiBlock:
                     key = max(0, np.ceil(12 * np.log2(float(torch.max(f0[:, s.start_frame:]) / 760))))
                 out, _ = s.enhancer.enhance(out, s.model_sr, f0, s.block_size, adaptive_key=key,
                                             silence_front=s.silence_front, rand_ini=s.gen_rand_ini, noise=s.gen_noise)
+        return self.tail(out, s.out_sr)
+
+    def tail(self, out, out_sr):
+        """audio_callback after SvcDDSP.infer: resampling, SOLA by conv1d, the crossfade or phase vocoder"""
+        s, dev = self.s, self.s.device
         audio = out.squeeze()
-        if s.out_sr != s.sr:
-            audio = s.to_device_rate(audio[None].contiguous(), s.out_sr)[0]
+        if out_sr != s.sr:
+            audio = s.to_device_rate(audio[None].contiguous(), out_sr)[0]
         temp = audio[-s.block - s.cf - s.search - s.delay:-s.delay]
         conv_input = temp[None, None, :s.cf + s.search]
         nom = F.conv1d(conv_input, self.sola_buffer[None, None, :])

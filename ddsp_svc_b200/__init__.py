@@ -13,11 +13,12 @@ from .loss import RSSLoss  # noqa: F401
 from .diffusion import GaussianDiffusion, WaveNet  # noqa: F401
 from .dropin import build_model, load_model, patch_reference, unpatch_reference  # noqa: F401
 from .pipeline import HostPipeline  # noqa: F401
-from .realtime import RealtimeVC  # noqa: F401
+from .realtime import RealtimeReflowVC, RealtimeVC  # noqa: F401
 from .reflow import NaiveV2Diff, RectifiedFlow  # noqa: F401
+from .reflow_vocoder import Unit2Wav, load_model_vocoder  # noqa: F401
 from .rmvpe import E2E0, RMVPE  # noqa: F401
 from .sinegen import SineGen, SourceModuleHnNSF  # noqa: F401
 from .vocoder import CombSub, CombSubFast, CombSubSuperFast, FixedControls, Sins  # noqa: F401
 
-__all__ = ["Sins", "CombSub", "CombSubSuperFast", "CombSubFast", "SineGen", "SourceModuleHnNSF", "FixedControls", "HostPipeline", "RealtimeVC", "NaiveV2Diff", "RectifiedFlow", "WaveNet", "GaussianDiffusion", "Generator", "E2E0", "RMVPE", "HubertSoft", "Units_Encoder", "load_fairseq_hubert", "Vocoder", "Enhancer", "Volume_Extractor", "RSSLoss", "frontend", "loss", "mel", "ops", "synthetic", "sharding",
-           "patch_reference", "unpatch_reference", "load_model", "build_model"]
+__all__ = ["Sins", "CombSub", "CombSubSuperFast", "CombSubFast", "SineGen", "SourceModuleHnNSF", "FixedControls", "HostPipeline", "RealtimeVC", "RealtimeReflowVC", "NaiveV2Diff", "RectifiedFlow", "Unit2Wav", "WaveNet", "GaussianDiffusion", "Generator", "E2E0", "RMVPE", "HubertSoft", "Units_Encoder", "load_fairseq_hubert", "Vocoder", "Enhancer", "Volume_Extractor", "RSSLoss", "frontend", "loss", "mel", "ops", "synthetic", "sharding",
+           "patch_reference", "unpatch_reference", "load_model", "build_model", "load_model_vocoder"]

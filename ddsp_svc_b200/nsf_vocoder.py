@@ -10,8 +10,10 @@ and main_reflow.py build from ``args.vocoder.type`` / ``args.vocoder.ckpt``.
   the kernels (rmvpe.Resampler, torchaudio's lowpass_filter_width=128 table), then ``mel.STFT.get_mel`` for keyshift 0
   (differentiable with respect to audio: the DDSP loss keeps its CUDA backward) or ``get_mel_keyshift`` otherwise
   (forward only).  Resampling has no backward: under grad with an audio that requires grad it raises.
-- ``infer(mel [B, n_frames, n_mels], f0 [B, >= n_frames, 1]) -> audio``: the package's NSF-HiFiGAN ``Generator``,
-  built on first use from config.json and ``ckpt['generator']`` as nsf_hifigan.models.load_model builds it.
+- ``infer(mel [B, n_frames, n_mels], f0 [B, >= n_frames, 1], rand_ini=None, noise=None) -> audio``: the package's
+  NSF-HiFiGAN ``Generator``, built on first use from config.json and ``ckpt['generator']`` as
+  nsf_hifigan.models.load_model builds it.  ``rand_ini`` [1, 1, 9] / ``noise`` [B, n_frames upp, 9] (not in the
+  reference) take SineGen's draws, for seeded runs and CUDA graphs; without them it draws as the reference does.
 """
 import json
 import os
@@ -79,7 +81,7 @@ class Vocoder:
             m = self.stft.get_mel_keyshift(audio_res, keyshift)
         return m.transpose(1, 2)                            # B, n_frames, bins
 
-    def infer(self, mel, f0):
+    def infer(self, mel, f0, rand_ini=None, noise=None):
         f0 = f0[:, :mel.size(1), 0]                         # B, n_frames
         if self.model is None:
             print('| Load HifiGAN: ', self.model_path)
@@ -88,4 +90,5 @@ class Vocoder:
             c = mel.transpose(1, 2)
             if self.vocoder_type == "nsf-hifigan-log10":
                 c = LOG10_SCALE * c
-            return self.model(c, f0)
+            draws = {k: v for k, v in (("rand_ini", rand_ini), ("noise", noise)) if v is not None}
+            return self.model(c, f0, **draws)

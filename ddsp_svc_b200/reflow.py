@@ -241,10 +241,16 @@ class RectifiedFlow(nn.Module):
         self.spec_min = spec_min
         self.spec_max = spec_max
 
-    def forward(self, condition, gt_spec=None, infer=True, infer_step=10, method='euler', t_start=0.0, use_tqdm=True):
+    def forward(self, condition, gt_spec=None, infer=True, infer_step=10, method='euler', t_start=0.0, use_tqdm=True,
+                noise=None):
         """condition [B, T, M] (the DDSP mel), gt_spec [B, T, M] or None -> the sampled mel [B, T, M] (reflow.py:59-105).
         The initial noise is ONE torch.randn((B, 1, M, T)) on condition's device, as in the reference, so seeded runs
-        compare.  ``use_tqdm`` is accepted and ignored.
+        compare; ``noise`` [B, 1, M, T] (not in the reference) takes that draw instead, for seeded runs and CUDA graphs.
+        ``use_tqdm`` is accepted and ignored.
+
+        The step schedule's rows (embedding, MLP and every layer's step projection) are computed on the first call and
+        kept for the calls with the same infer_step, method, t_start, gt_spec presence, device and weights, so later
+        calls copy nothing to the device and never synchronise (capturable in a CUDA graph).
 
         ``infer=False`` with ``NaiveV2Diff.reflow_backward`` on: the reference's reflow loss (reflow.py:20-35, :63-68,
         loss_type 'l2_lognorm') with its draws: t = t_start + (1 - t_start) torch.rand(B) clipped to [1e-7, 1 - 1e-7],
@@ -271,50 +277,69 @@ class RectifiedFlow(nn.Module):
             _need_cuda_f32("gt_spec", gt_spec)
             if gt_spec.shape != (B, T, M):
                 raise ValueError("RectifiedFlow: gt_spec must be [B, T, %d] like condition" % M)
-        noise = torch.randn(shape, device=dev)
-        return self._sample(condition, noise, gt_spec, infer_step, method, t_start)
+        if noise is None:
+            noise = torch.randn(shape, device=dev)
+        return self._sample(condition, noise, gt_spec, infer_step, method, t_start, keep_schedule=True)
 
-    def _sample(self, condition, noise, gt_spec, infer_step, method, t_start):
-        """forward after the noise draw: noise [B, 1, M, T] given"""
+    def _sample(self, condition, noise, gt_spec, infer_step, method, t_start, keep_schedule=False):
+        """forward after the noise draw: noise [B, 1, M, T] given; ``keep_schedule``: reuse (and keep) the cached step
+        rows, as forward does, instead of computing them for this call alone"""
         fn, (B, T, _), M, dev = self.velocity_fn, condition.shape, self.out_dims, condition.device
         _need_cuda_f32("noise", noise)
         if noise.shape != (B, 1, M, T):
             raise ValueError("RectifiedFlow: noise must be [B, 1, %d, T]" % M)
         if gt_spec is None:
-            # the reference writes torch.full((b,), 0): an int64 t whose first `t += dt` raises; t here is fp32 from 0
-            t, gt, ts = torch.zeros(1), None, 0.0
+            gt, ts = None, 0.0
             dt = 1.0 / infer_step
         else:
-            t, gt, ts = torch.full((1,), float(t_start)), gt_spec.contiguous(), float(t_start)
+            gt, ts = gt_spec.contiguous(), float(t_start)
             dt = (1.0 - ts) / infer_step
         if method not in ("euler", "rk4"):
             raise NotImplementedError(method)
-        # the step schedule with the reference's fp32 arithmetic (t += dt, 1000 (t + 0.5 dt), ...); every utterance shares it
-        sched = []
-        for _ in range(infer_step):
-            sched += [1000 * t] if method == "euler" else [1000 * t, 1000 * (t + 0.5 * dt), 1000 * (t + 0.5 * dt), 1000 * (t + dt)]
-            t += dt
         noise = noise.contiguous()
         L, N = _lib.lib(), B * T
         with torch.no_grad(), _Gemm(fn.gemm_precision) as g:
             P = fn._pack()
             crows = fn._cond_rows(g, P, condition.contiguous())
-            srows = fn._step_rows(g, P, torch.cat(sched).to(dev)).contiguous() if sched else None   # [E, n_layers dim]
+            srows = self._schedule_rows(g, P, infer_step, method, ts, dt, gt is None, dev, keep_schedule)
+            n_eval = 0 if srows is None else srows.shape[0]
             x = torch.empty(N, M, dtype=torch.float32, device=dev)
-            acc = torch.empty_like(x) if method == "rk4" and sched else None
+            acc = torch.empty_like(x) if method == "rk4" and n_eval else None
             xs = fn._operand(g, N, M, dev)
             hi, lo = fn._ptrs(xs)
             rng = float(self.spec_max - self.spec_min)
             _k(L.b2d_rf_start(noise.data_ptr(), 0 if gt is None else gt.data_ptr(), ts, 1.0 - ts, float(self.spec_min), rng,
                               B, T, M, x.data_ptr(), hi, lo, _stream()), "b2d_rf_start")
             stages = (-1,) if method == "euler" else (0, 1, 2, 3)
-            for e in range(len(sched)):
+            for e in range(n_eval):
                 G = fn._velocity(g, P, xs, srows[e], 0, crows, B, T)
                 _k(L.b2d_rf_ode_update(G.data_ptr(), P["out_b"].data_ptr(), x.data_ptr(), 0 if acc is None else acc.data_ptr(),
                                        stages[e % len(stages)], dt, N, M, hi, lo, _stream()), "b2d_rf_ode_update")
             out = torch.empty(B, T, M, dtype=torch.float32, device=dev)
             _k(L.b2d_rf_finish(x.data_ptr(), float(self.spec_min), rng, N * M, out.data_ptr(), _stream()), "b2d_rf_finish")
         return out
+
+    def _schedule_rows(self, g, P, infer_step, method, ts, dt, no_gt, dev, keep):
+        """the step rows [E, n_layers dim] of the whole schedule (None when it is empty).  With ``keep`` they are cached
+        on everything they depend on: infer_step, method, t_start, gt_spec's presence, the device and the packed weights
+        (_pack's key)"""
+        fn = self.velocity_fn
+        key = (infer_step, method, ts, no_gt, dev, fn.__dict__["_packed"][0])
+        c = self.__dict__.get("_sched_rows")
+        if keep and c is not None and c[0] == key:
+            return c[1]
+        # the reference writes torch.full((b,), 0) without gt_spec: an int64 t whose first `t += dt` raises; t here is
+        # fp32 from 0.  The schedule keeps the reference's fp32 arithmetic (t += dt, 1000 (t + 0.5 dt), ...); every
+        # utterance shares it
+        t = torch.zeros(1) if no_gt else torch.full((1,), ts)
+        sched = []
+        for _ in range(infer_step):
+            sched += [1000 * t] if method == "euler" else [1000 * t, 1000 * (t + 0.5 * dt), 1000 * (t + 0.5 * dt), 1000 * (t + dt)]
+            t += dt
+        rows = fn._step_rows(g, P, torch.cat(sched).to(dev)).contiguous() if sched else None
+        if keep:
+            self.__dict__["_sched_rows"] = (key, rows)
+        return rows
 
     # ---- training ----
     def _training_loss(self, condition, gt_spec, t_start):
