@@ -33,15 +33,12 @@ STAGES = ("rmvpe", "units", "ddsp", "mel", "sampler", "vocoder", "tail")
 SAMPLERS = {"euler20": dict(sampling_method="euler", infer_step=20), "rk4_5": dict(sampling_method="rk4", infer_step=5)}
 
 
-def write_synthetic_reflow(d, n_chans=512, n_layers=6, encoder="contentvec768l12", n_spk=2, model_type="RectifiedFlow"):
-    """seeded checkpoints of a reflow session in directory d -> (model path, rmvpe path).  The velocity network's
-    parameters are all non-zero (tests/reflow_oracle.seeded_weights; the default init zeroes its output projection);
-    ``encoder``: 'contentvec768l12' (reflow.yaml) or 'hubertsoft'"""
+def write_front(d, encoder="contentvec768l12"):
+    """seeded checkpoints of what every diffusion / reflow session loads besides its model, in directory d: the units
+    encoder, RMVPE and NSF-HiFiGAN (voc/model.ckpt) -> the config's data and vocoder sections"""
     import ddsp_svc_b200 as pkg
     from ddsp_svc_b200 import dropin
     from ddsp_svc_b200.hifigan import Generator
-    from tests import reflow_oracle
-    torch.manual_seed(0)
     os.makedirs(os.path.join(d, "voc"), exist_ok=True)
     if encoder == "hubertsoft":
         enc_path, n_unit = os.path.join(d, "hubert.pt"), 256
@@ -55,11 +52,24 @@ def write_synthetic_reflow(d, n_chans=512, n_layers=6, encoder="contentvec768l12
         json.dump(HIFIGAN, f)
     gen = Generator(dropin.DotDict(HIFIGAN))
     torch.save({"generator": gen.state_dict()}, os.path.join(d, "voc", "model.ckpt"))
-    cfg = {"data": {"sampling_rate": 44100, "block_size": 512, "encoder": encoder, "encoder_ckpt": enc_path,
-                    "encoder_sample_rate": 16000, "encoder_hop_size": 320, "encoder_out_channels": n_unit},
+    return ({"sampling_rate": 44100, "block_size": 512, "encoder": encoder, "encoder_ckpt": enc_path,
+             "encoder_sample_rate": 16000, "encoder_hop_size": 320, "encoder_out_channels": n_unit},
+            {"type": "nsf-hifigan", "ckpt": os.path.join(d, "voc", "model.ckpt")})
+
+
+def write_synthetic_reflow(d, n_chans=512, n_layers=6, encoder="contentvec768l12", n_spk=2, model_type="RectifiedFlow"):
+    """seeded checkpoints of a reflow session in directory d -> (model path, rmvpe path).  The velocity network's
+    parameters are all non-zero (tests/reflow_oracle.seeded_weights; the default init zeroes its output projection);
+    ``encoder``: 'contentvec768l12' (reflow.yaml) or 'hubertsoft'"""
+    import ddsp_svc_b200 as pkg
+    from tests import reflow_oracle
+    torch.manual_seed(0)
+    data, voc = write_front(d, encoder)
+    n_unit = data["encoder_out_channels"]
+    cfg = {"data": data,
            "model": {"type": model_type, "win_length": 2048, "n_layers": n_layers, "n_chans": n_chans,
                      "use_pitch_aug": True, "n_spk": n_spk},
-           "vocoder": {"type": "nsf-hifigan", "ckpt": os.path.join(d, "voc", "model.ckpt")}}
+           "vocoder": voc}
     with open(os.path.join(d, "config.yaml"), "w") as f:
         yaml.safe_dump(cfg, f)
     model = pkg.Unit2Wav(44100, 512, 2048, n_unit, n_spk, True, HIFIGAN["num_mels"], n_layers, n_chans)

@@ -4,7 +4,8 @@
 // GEMMs issued by the host side (ddsp_svc_b200/unit2control.py); between them the activations [B, T, C] (token-major,
 // C contiguous) pass through these kernels exactly once each:
 //
-//   u2c_embed           x += f0_embed(log(1 + f0/700)) + phase_embed(phase/pi) + volume_embed(volume) + spk (+ aug)  (:93-102)
+//   u2c_embed           x += f0_embed(log(1 + f0/700)) + phase_embed(phase/pi) + volume_embed(volume) + spk (+ aug)  (:93-102);
+//                       without a phase (Unit2Mel, diffusion/vocoder.py:206-215) the phase term is left out
 //   u2c_groupnorm_lrelu GroupNorm(4, 256) over (64 channels x T) per utterance + LeakyReLU(0.01)                      (:50-52)
 //   u2c_layernorm       LayerNorm(C) per token                                                (pcmer.py:143,209; :104)
 //   u2c_glu_dwconv_silu GLU -> depthwise Conv1d(k = 31, same padding) -> SiLU                  (pcmer.py:211-215)
@@ -18,7 +19,8 @@ namespace {
 
 constexpr int kC = 256;     // model width of Unit2Control (fixed by the reference: every embed / norm is 256 wide)
 
-// x [N, 256] += w_f0 * log(1 + f0/700) + b_f0 + w_ph * (phase/pi) + b_ph + w_vol * vol + b_vol + spk[b] (+ w_aug * aug/5)
+// x [N, 256] += w_f0 * log(1 + f0/700) + b_f0 + w_ph * (phase/pi) + b_ph + w_vol * vol + b_vol + spk[b] (+ w_aug * aug/5);
+// phase null: x + (w_f0 * log(1 + f0/700) + b_f0) + (w_vol * vol + b_vol) + spk[b] (+ ...), Unit2Mel's association
 __global__ void __launch_bounds__(256) u2c_embed_kernel(float* __restrict__ x, const float* __restrict__ f0,
                                                         const float* __restrict__ phase, const float* __restrict__ volume,
                                                         const float* __restrict__ emb /* [7][256]: wf bf wp bp wv bv wa */,
@@ -30,9 +32,13 @@ __global__ void __launch_bounds__(256) u2c_embed_kernel(float* __restrict__ x, c
     for (int n = blockIdx.x; n < n_tokens; n += gridDim.x) {
         const int b = n / T;
         const float lf = logf(1.0f + __ldg(f0 + n) / 700.0f);
-        const float ph = __ldg(phase + n) / B2D_PI_F;
         float v = x[(size_t)n * kC + c];
-        v = v + (wf * lf + bf) + (wp * ph + bp) + (wv * __ldg(volume + n) + bv);        // the reference's association
+        if (phase) {
+            const float ph = __ldg(phase + n) / B2D_PI_F;
+            v = v + (wf * lf + bf) + (wp * ph + bp) + (wv * __ldg(volume + n) + bv);    // the reference's association
+        } else {
+            v = v + (wf * lf + bf) + (wv * __ldg(volume + n) + bv);
+        }
         if (spk) v += spk[(size_t)(spk_rows == 1 ? 0 : b) * kC + c];
         if (aug) v += wa * (__ldg(aug + b) / 5.0f);
         x[(size_t)n * kC + c] = v;
@@ -201,7 +207,7 @@ extern "C" int b2d_split_tf32(const float* x, float* hi, float* lo, size_t n, vo
 
 extern "C" int b2d_u2c_embed(float* x, const float* f0, const float* phase, const float* volume, const float* embed_table,
                              const float* spk, int spk_rows, const float* aug_shift, int B, int T, void* stream) {
-    if (!x || !f0 || !phase || !volume || !embed_table) return b2d::fail(B2D_ERR_NULL, "u2c_embed: null pointer");
+    if (!x || !f0 || !volume || !embed_table) return b2d::fail(B2D_ERR_NULL, "u2c_embed: null pointer");   // phase may be null
     if (B <= 0 || T <= 0 || (spk && spk_rows != 1 && spk_rows != B)) return b2d::fail(B2D_ERR_SHAPE, "u2c_embed: bad shape");
     const int n = B * T;
     u2c_embed_kernel<<<min(n, b2d::num_sms() * 8), 256, 0, (cudaStream_t)stream>>>(x, f0, phase, volume, embed_table, spk, spk_rows, aug_shift, n, T);

@@ -447,13 +447,18 @@ class GaussianDiffusion(nn.Module):
         return (x + 1) / 2 * (self.spec_max - self.spec_min) + self.spec_min
 
     def forward(self, condition, gt_spec=None, infer=True, infer_speedup=10, method='dpm-solver', k_step=None,
-                use_tqdm=True):
+                use_tqdm=True, noise=None, step_noise=None):
         """condition [B, T, M_cond] -> the sampled mel [B, T, M] (diffusion.py:216-378).  The start: gt_spec or k_step
         None -> ONE torch.randn((B, 1, M, T)) from t = self.k_step; otherwise q_sample(norm(gt_spec), k_step - 1) with
         its noise drawn as randn_like of the transposed [B, 1, M, T] view, from t = k_step.  Then ``method``:
         'dpm-solver', 'unipc' (t // infer_speedup steps, at least 2), 'pndm', 'ddim'; None or infer_speedup 1: DDPM,
         one torch.randn((B, 1, M, T)) per step.  The draws happen on condition's device in the reference's order, so
         seeded runs compare.  ``use_tqdm`` is accepted and ignored.
+
+        Not in the reference: ``noise`` [B, 1, M, T] (any strides) takes the start's draw and ``step_noise`` (an iterable
+        of [B, 1, M, T] tensors, one per step) DDPM's, for seeded runs and CUDA graphs; absent, each is drawn as above.
+        The step rows and the coefficient table are kept on the device between calls (_schedule), so after one warm
+        call with the same settings a forward copies nothing to the device and never synchronises.
 
         ``infer=False`` with the denoiser's switch on (``WaveNet.diffusion_backward``, ``NaiveV2Diff.reflow_backward``):
         the reference's training loss (diffusion.py:194-238, loss_type 'l2') with its draws: t = torch.randint(0, t_max,
@@ -474,38 +479,42 @@ class GaussianDiffusion(nn.Module):
         B, T, Mc = condition.shape
         if M != fn.mel_channels or Mc != fn.condition_dim:
             raise ValueError("GaussianDiffusion: out_dims / condition width do not match the denoiser")
+        if noise is not None:
+            _need_cuda_f32("noise", noise)
+            if tuple(noise.shape) != (B, 1, M, T):
+                raise ValueError("GaussianDiffusion: noise must be [B, 1, %d, T] like condition" % M)
         if gt_spec is None or k_step is None:
             t, gt = self.k_step, None
-            noise = torch.randn((B, 1, M, T), device=dev)
+            if noise is None:
+                noise = torch.randn((B, 1, M, T), device=dev)
         else:
             _need_cuda_f32("gt_spec", gt_spec)
             if gt_spec.shape != (B, T, M):
                 raise ValueError("GaussianDiffusion: gt_spec must be [B, T, %d] like condition" % M)
             t, gt = int(k_step), gt_spec.contiguous()
-            # randn_like(x_start) of the transposed view keeps its strides: the draw fills [B, T, M] in order
-            noise = torch.empty_strided((B, 1, M, T), (T * M, T * M, 1, M), device=dev).normal_()
-        return self._sample(condition, noise, gt, t, infer_speedup, method)
+            if noise is None:
+                # randn_like(x_start) of the transposed view keeps its strides: the draw fills [B, T, M] in order
+                noise = torch.empty_strided((B, 1, M, T), (T * M, T * M, 1, M), device=dev).normal_()
+        return self._sample(condition, noise, gt, t, infer_speedup, method, step_noise, keep_schedule=True)
 
-    def _sample(self, condition, noise, gt_spec, t, infer_speedup, method, step_noise=None):
+    def _sample(self, condition, noise, gt_spec, t, infer_speedup, method, step_noise=None, keep_schedule=False):
         """forward after the start's draw: noise [B, 1, M, T] (any strides), gt_spec [B, T, M] or None, t the first
         step (k_step, or self.k_step without gt_spec).  DDPM draws its per-step noise here, one torch.randn((B, 1, M, T))
-        per step, or takes them from ``step_noise`` (an iterable of [B, 1, M, T] tensors) when given."""
+        per step, or takes them from ``step_noise`` (an iterable of [B, 1, M, T] tensors) when given.
+        ``keep_schedule``: reuse (and keep) the cached step rows and coefficients (_schedule)."""
         fn, M, dev = self.denoise_fn, self.out_dims, condition.device
         B, T, _ = condition.shape
         if t < 1:
             raise ValueError("GaussianDiffusion: the first step (k_step) must be a positive int, got %r" % (t,))
         buf = self._host()
         if method is None or infer_speedup <= 1:
-            plan, slots = _discrete_plan(buf, t, 1, "ddpm")
+            method, infer_speedup = "ddpm", 1
         elif method in ("dpm-solver", "unipc"):
             steps = t // infer_speedup
             if steps < 2:
                 raise ValueError("GaussianDiffusion: %s needs at least 2 steps (order 2), got k_step // infer_speedup = %d"
                                  % (method, steps))
-            plan, slots = _multistep_plan(buf["betas"][:t], steps, method)
-        elif method in ("pndm", "ddim"):
-            plan, slots = _discrete_plan(buf, t, infer_speedup, method)
-        else:
+        elif method not in ("pndm", "ddim"):
             raise NotImplementedError(method)
         L, N = _lib.lib(), B * T
         spec_min = float(buf["spec_min"][0])
@@ -518,8 +527,8 @@ class GaussianDiffusion(nn.Module):
         with torch.no_grad(), _Gemm(fn.gemm_precision) as g:
             P = fn._pack()
             crows = fn._cond_rows(g, P, condition.contiguous())
-            srows = fn._step_rows(g, P, torch.tensor([ev.step for ev in plan], dtype=torch.float32).to(dev)).contiguous()
-            coefs = torch.tensor([ev.coef for ev in plan], dtype=torch.float32).to(dev)
+            plan, slots, srows, coefs = self._schedule(g, P, buf, t, infer_speedup, method, gt_spec is None, dev,
+                                                       keep_schedule)
             x = torch.empty(N, M, dtype=torch.float32, device=dev)
             hist = [torch.empty(N, M, dtype=torch.float32, device=dev) for _ in range(slots)]
             xs = fn._operand(g, N, M, dev)
@@ -540,6 +549,29 @@ class GaussianDiffusion(nn.Module):
             out = torch.empty(B, T, M, dtype=torch.float32, device=dev)
             _k(L.b2d_rf_finish(x.data_ptr(), spec_min, spec_range, N * M, out.data_ptr(), _stream()), "b2d_rf_finish")
         return out
+
+    def _schedule(self, g, P, buf, t, speedup, method, no_gt, dev, keep):
+        """-> (plan, history slots, step rows [E, n_layers C], coefficients [E, 8]) of one sampler call ('ddpm' with
+        speedup 1 for DDPM).  With ``keep`` the device tensors are cached on everything they depend on: t, the speedup,
+        the method, gt_spec's presence, the device, the denoiser's packed weights (_pack's key) and the schedule
+        buffers"""
+        key = (t, speedup, method, no_gt, dev, self.denoise_fn.__dict__["_packed"][0],
+               tuple((b.data_ptr(), b._version) for b in (getattr(self, n) for n in _BUFFERS)))
+        c = self.__dict__.get("_sched")
+        if keep and c is not None and c[0] == key:
+            return c[1]
+        if method == "ddpm":
+            plan, slots = _discrete_plan(buf, t, 1, "ddpm")
+        elif method in ("dpm-solver", "unipc"):
+            plan, slots = _multistep_plan(buf["betas"][:t], t // speedup, method)
+        else:
+            plan, slots = _discrete_plan(buf, t, speedup, method)
+        srows = self.denoise_fn._step_rows(g, P, torch.tensor([ev.step for ev in plan], dtype=torch.float32).to(dev))
+        coefs = torch.tensor([ev.coef for ev in plan], dtype=torch.float32).to(dev)
+        sched = (plan, slots, srows.contiguous(), coefs)
+        if keep:
+            self.__dict__["_sched"] = (key, sched)
+        return sched
 
     # ---- training ----
     def _training_loss(self, condition, gt_spec, k_step):

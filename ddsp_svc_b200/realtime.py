@@ -1,4 +1,4 @@
-"""The real-time conversion blocks of gui.py and gui_reflow.py on the device, replayed as CUDA graphs.
+"""The real-time conversion blocks of gui.py, gui_reflow.py and gui_diff.py on the device, replayed as CUDA graphs.
 
 ``RealtimeVC(model_path, samplerate, block_time, crossfade_time, extra_time, f0_min, f0_max, threhold, spk_id,
 pitch_adjust, use_spk_mix, spk_mix_dict, use_enhancer, enhancer_adaptive_key, use_phase_vocoder, graph=True)`` takes
@@ -26,14 +26,26 @@ rt_crossfade -> pinned copy, ONE graph: no value in it is data-dependent.  Its d
 initial noise, SineGen's rand_ini and noise) are static buffers filled by torch's CUDA generator, and the sampler's step
 rows are cached by RectifiedFlow after the warm-up, so a replay copies nothing to the device and never synchronises.
 
-Both sessions share ``_Session``: the ring buffer, the upload and the owned stream, capture with a warm-up and a state
+``RealtimeDiffVC(model_path, diff_model_path, ..., k_step, diff_acc, diff_method, diff_silence, ...)`` is gui_diff.py's
+block (audio_callback, gui_diff.py:437-503, with SvcDDSP.update_model / infer, :48-154) on the diffusion cascade
+(diffusion_vocoder): ring buffer -> RMVPE -> rt_f0_regrid -> volume -> mask -> units -> the DDSP model -> DiffGtMel.infer
+(the mel of the DDSP output, the shallow-diffusion sampler from k_step, the crop at its start_frame or the diff_silence
+input crop, NSF-HiFiGAN) -> mask multiply -> resampling -> rt_sola -> rt_crossfade -> pinned copy, ONE graph.  Its draws
+(the DDSP noise, the sampler's start, DDPM's per-step noise, SineGen's rand_ini and noise) are static buffers filled by
+torch's CUDA generator, and GaussianDiffusion keeps its step rows and coefficients after the warm-up.
+
+The sessions share ``_Session``: the ring buffer, the upload and the owned stream, capture with a warm-up and a state
 restore, the f0 / volume / mask / units front half, the resampling -> SOLA -> crossfade -> pinned-copy tail and
-SineGen's draws.  ``reflow_frames`` is the reflow block's frame bookkeeping as a pure function.
+SineGen's draws.  ``reflow_frames`` and ``diff_frames`` are the reflow and diffusion blocks' frame bookkeeping as pure
+functions.
 """
+import gc
+
 import numpy as np
 import torch
 
 from . import frontend, ops
+from .diffusion_vocoder import DiffGtMel, Unit2WavFast, read_config
 from .dropin import load_model
 from .enhancer import Enhancer, adaptive_rate, auto_key
 from .hubert import Units_Encoder
@@ -98,8 +110,51 @@ def reflow_frames(samplerate, block_time, crossfade_time, extra_time, model_sr, 
     return f
 
 
+def _mel_frames(n, vocoder_hop, win_size):
+    """the frames nvSTFT.get_mel makes of n samples (its reflect-or-constant padding, center=False)"""
+    pad_left = (win_size - vocoder_hop) // 2
+    pad_right = max((win_size - vocoder_hop + 1) // 2, win_size - n - pad_left)
+    return (n + pad_left + pad_right - win_size) // vocoder_hop + 1
+
+
+def diff_frames(samplerate, block_time, crossfade_time, extra_time, model_sr, block_size, vocoder_sr, vocoder_hop,
+                win_size=2048, diff_silence=False):
+    """The frame bookkeeping of one gui_diff.py block -> dict:
+
+    - gui_frames' lengths and silence_front; ``hop`` and ``n_frames`` (F0_Extractor's and the volume's frames);
+    - ``start_frame`` / ``trim``: F0_Extractor's leading frames and the samples RMVPE skips;
+    - ``diff_start``: DiffGtMel.infer's start_frame, int(silence_front * vocoder rate / vocoder hop);
+    - ``cond_frames``: the frames the diffusion model sees (n_frames, or n_frames - diff_start with diff_silence), which
+      are also its mel frames; ``voc_frames``: the frames vocoded (from diff_start on);
+    - ``out_len``: the output's samples at the model rate after the left pad (n_frames block_size), ``out_dev`` its
+      length at the device rate and ``tail``: the (start, stop) of the samples SOLA reads.
+    Raises ValueError where the reference's block cannot run: a non-integer hop, a vocoder rate or hop other than the
+    model's (``output *= mask`` would not broadcast), or a mel whose frame count differs from the condition's."""
+    f = gui_frames(samplerate, block_time, crossfade_time, extra_time)
+    sr = f["sr"]
+    hop = model_hop(sr, model_sr, block_size, "RealtimeDiffVC")
+    if vocoder_sr != model_sr or vocoder_hop != block_size:
+        raise ValueError("the vocoder runs at %d Hz with hop %d, the model at %d Hz with block_size %d: gui_diff.py's "
+                         "output *= mask needs both equal" % (vocoder_sr, vocoder_hop, model_sr, block_size))
+    n_frames = f["n_in"] // hop + 1
+    start_frame = int(f["silence_front"] * sr / hop)
+    diff_start = int(f["silence_front"] * vocoder_sr / vocoder_hop)
+    cond_frames = n_frames - diff_start if diff_silence else n_frames
+    mel_frames = _mel_frames(cond_frames * block_size, vocoder_hop, win_size)
+    if mel_frames != cond_frames:
+        raise ValueError("the mel of %d DDSP frames has %d frames: the diffusion model's condition has %d"
+                         % (cond_frames, mel_frames, cond_frames))
+    out_len = n_frames * vocoder_hop
+    out_dev = out_len if model_sr == sr else resampled_length(out_len, model_sr, sr)
+    tail = (out_dev - f["block"] - f["cf"] - f["search"] - f["delay"], out_dev - f["delay"])
+    f.update(hop=hop, n_frames=n_frames, start_frame=start_frame, trim=int(np.round(start_frame * hop / sr * sr)),
+             diff_start=diff_start, cond_frames=cond_frames, mel_frames=mel_frames, voc_frames=n_frames - diff_start,
+             out_len=out_len, out_dev=out_dev, tail=tail)
+    return f
+
+
 class _Session:
-    """What the gui.py and gui_reflow.py sessions share (see the module's docstring)"""
+    """What the real-time sessions share (see the module's docstring)"""
 
     def _init_block(self, samplerate, block_time, crossfade_time, extra_time, device, who):
         self.device = torch.device("cuda" if device is None else device)
@@ -173,7 +228,12 @@ class _Session:
 
     def _capture(self, fn, state):
         """fn captured on the session's stream after one eager warm-up run (tables, packed weights, allocator); the
-        warm-up's writes to the session state tensors are undone, so the first replay starts where it should"""
+        warm-up's writes to the session state tensors are undone, so the first replay starts where it should.
+
+        Python's cycle collector does not run during the capture: it could free an unreachable CUDAGraph (another
+        session's, dropped while in a reference cycle), and destroying a graph while a stream captures is an operation
+        CUDA forbids, which corrupts this capture.  Garbage is collected just before instead (torch.cuda.graph no
+        longer does that by default)."""
         self.stream.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(self.stream):
             saved = [t.clone() for t in state]
@@ -181,9 +241,16 @@ class _Session:
             for t, v in zip(state, saved):
                 t.copy_(v)
         self.stream.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g, stream=self.stream):
-            static = fn()
+        collecting = gc.isenabled()
+        gc.collect()
+        gc.disable()
+        try:
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, stream=self.stream):
+                static = fn()
+        finally:
+            if collecting:
+                gc.enable()
         return g, static
 
     def upload(self, indata):
@@ -366,6 +433,142 @@ class RealtimeReflowVC(_Session):
                              silence_front=self.silence_front, use_tqdm=False, ddsp_noise=self.noise,
                              reflow_noise=self.reflow_noise, rand_ini=self.gen_rand_ini, sine_noise=self.gen_noise)
         out = frontend.mask_apply_(out.reshape(1, -1).contiguous(), mask, self.block_size, self.mask_offset)
+        self._tail(out, self.model_sr)
+
+    def run(self):
+        """enqueue the block's graph (or its eager code) on the session's stream"""
+        if not self.graph:
+            with torch.cuda.stream(self.stream):
+                self._stage()
+            return
+        if self.graph_block is None:
+            self.graph_block, _ = self._capture(self._stage, [self.ring, self.sola_buffer])
+        with torch.cuda.stream(self.stream):
+            self.graph_block.replay()
+
+    def process(self, indata):
+        """audio_callback's math: indata [frames, channels] -> outdata [frames, 2] (float32)"""
+        self.upload(indata)
+        self.run()
+        return self._output()
+
+
+DIFF_METHODS = ("ddim", "pndm", "dpm-solver", "unipc")
+
+
+class RealtimeDiffVC(_Session):
+    """gui_diff.py's block on the diffusion models (see the module's docstring).  ``model_path`` is the DDSP checkpoint
+    (None or '' for none), ``diff_model_path`` the diffusion model's.  A 'Diffusion' model (Unit2Mel) starts its sampler
+    from the DDSP output's mel at k_step; without a DDSP checkpoint it samples from noise from GaussianDiffusion.k_step
+    (1000), as the reference does.  diff_acc 1 samples with DDPM.
+
+    Deviations from the reference: for 'DiffusionNew' / 'DiffusionFast', Unit2Wav computes its own DDSP mel and ignores
+    the external DDSP output, so the session checks the DDSP checkpoint's config against the diffusion model's but does
+    not run it; and, as in the other sessions, a speaker mix applies only with use_spk_mix."""
+
+    def __init__(self, model_path, diff_model_path, samplerate=44100, block_time=0.5, crossfade_time=0.04,
+                 extra_time=2.0, f0_min=50, f0_max=1100, threhold=-45, spk_id=1, pitch_adjust=0.0, use_spk_mix=False,
+                 spk_mix_dict=None, use_phase_vocoder=False, k_step=100, diff_acc=10, diff_method="ddim",
+                 diff_silence=False, graph=True, pitch_extractor_type="rmvpe", rmvpe_ckpt="pretrain/rmvpe/model.pt",
+                 device=None):
+        if pitch_extractor_type != "rmvpe":
+            raise ValueError("RealtimeDiffVC extracts f0 with 'rmvpe' only: %r has no kernels" % (pitch_extractor_type,))
+        if diff_method not in DIFF_METHODS:
+            raise ValueError("diff_method must be one of %s, got %r" % (", ".join(DIFF_METHODS), diff_method))
+        if int(k_step) != k_step or k_step < 0:
+            raise ValueError("k_step must be an integer >= 0, got %r" % (k_step,))
+        if int(diff_acc) != diff_acc or (k_step > 0 and not 1 <= diff_acc <= k_step // 2):
+            raise ValueError("diff_acc must be an integer in [1, k_step // 2] = [1, %d] (1: DDPM), got %r"
+                             % (int(k_step) // 2, diff_acc))
+        self._init_block(samplerate, block_time, crossfade_time, extra_time, device, "RealtimeDiffVC")
+        self.f0_max = float(f0_max)
+        self.k_step, self.diff_acc, self.diff_method = int(k_step), int(diff_acc), diff_method
+        self.diff_silence, self.use_pv, self.graph = bool(diff_silence), bool(use_phase_vocoder), bool(graph)
+
+        # SvcDDSP.update_model: the DDSP checkpoint's config is checked against the diffusion model's (check_args)
+        args = read_config(diff_model_path)
+        kind = args.model.type
+        k_step_max = int(args.model.k_step_max) if kind == "DiffusionNew" else 1000
+        if self.k_step > k_step_max:
+            raise ValueError("k_step %d exceeds the model's k_step_max %d" % (self.k_step, k_step_max))
+        if kind == "Diffusion" and self.k_step == 0:
+            raise ValueError("a 'Diffusion' model needs k_step >= 1: its shallow start noises to step k_step - 1")
+        self.diff = DiffGtMel(device=self.device)
+        ddsp_args = read_config(model_path) if model_path else None
+        if ddsp_args is not None:
+            self.diff.check_args(ddsp_args, args)
+        self.diff.flush_model(diff_model_path, ddsp_config=ddsp_args)
+        self.model, self.vocoder, self.args = self.diff.model, self.diff.vocoder, self.diff.args
+        self.ddsp_model = None
+        if kind == "Diffusion" and model_path:
+            self.ddsp_model, self.ddsp_args = load_model(model_path, device=self.device)
+        data = self.args.data
+        self.frames = diff_frames(self.sr, block_time, crossfade_time, extra_time, int(data.sampling_rate),
+                                  int(data.block_size), self.vocoder.vocoder_sample_rate, self.vocoder.vocoder_hop_size,
+                                  self.vocoder.h.win_size, self.diff_silence)
+        self._init_front(data, f0_min, threhold, pitch_adjust, spk_id, use_spk_mix, spk_mix_dict, rmvpe_ckpt,
+                         "RealtimeDiffVC")
+
+        dev, fr, M = self.device, self.frames, self.vocoder.dimension
+        T = fr["cond_frames"]
+        self.ext_noise = None                 # the external DDSP model's noise: randn for CombSubSuperFast, else uniform
+        if self.ddsp_model is not None:
+            self.ext_noise = torch.zeros(1, self.n_frames * self.block_size, device=dev)
+            self.ext_normal = self.ddsp_args.model.type == "CombSubSuperFast"
+        self.ddsp_noise = None                # Unit2Wav's CombSubFast (uniform) / Unit2WavFast's CombSubSuperFast (randn)
+        if kind != "Diffusion":
+            self.ddsp_noise = torch.zeros(1, T * self.block_size, device=dev)
+        # the sampler's start: with a gt_spec, randn_like of the transposed [B, 1, M, T] view; without, torch.randn
+        has_gt = kind != "Diffusion" or self.ddsp_model is not None
+        runs = kind == "Diffusion" or self.k_step > 0
+        self.diff_noise = self.step_noise = None
+        if runs:
+            self.diff_noise = (torch.empty_strided((1, 1, M, T), (T * M, T * M, 1, M), device=dev) if has_gt else
+                               torch.empty(1, 1, M, T, device=dev)).zero_()
+            if self.diff_acc == 1:
+                n_steps = self.k_step if has_gt else self.model.decoder.k_step
+                self.step_noise = torch.zeros(n_steps, 1, 1, M, T, device=dev)
+        self.gen_rand_ini = torch.zeros(1, 1, SINEGEN_DIM, device=dev)
+        self.gen_noise = torch.zeros(1, fr["voc_frames"] * self.vocoder.vocoder_hop_size, SINEGEN_DIM, device=dev)
+        self.graph_block = None
+
+    def _draw_noise(self):
+        """the block's draws: the DDSP noise, the sampler's start, DDPM's per-step noise, SineGen's rand_ini and noise"""
+        if self.ext_noise is not None:
+            if self.ext_normal:
+                self.ext_noise.normal_()
+            else:
+                self.ext_noise.uniform_(-1, 1)
+        if self.ddsp_noise is not None:
+            if isinstance(self.model, Unit2WavFast):
+                self.ddsp_noise.normal_()
+            else:
+                self.ddsp_noise.uniform_(-1, 1)
+        if self.diff_noise is not None:
+            self.diff_noise.normal_()
+        if self.step_noise is not None:
+            self.step_noise.normal_()
+        self._draw_sinegen(self.gen_rand_ini, self.gen_noise)
+
+    def draws(self):
+        """the draws DiffGtMel.infer takes, from the static buffers"""
+        d = dict(noise=self.diff_noise, step_noise=self.step_noise, rand_ini=self.gen_rand_ini, sine_noise=self.gen_noise)
+        if self.ddsp_noise is not None:
+            d["ddsp_noise"] = self.ddsp_noise
+        return d
+
+    def _stage(self):
+        f0, volume, mask, units = self._front()
+        self._draw_noise()
+        with torch.no_grad():
+            out = None
+            if self.ddsp_model is not None:
+                out, _, _ = self.ddsp_model(units, f0, volume[..., None], spk_id=self.spk_id,
+                                            spk_mix_dict=self.spk_mix_dict, noise=self.ext_noise)
+            out = self.diff.infer(out, f0, units, volume[..., None], acc=self.diff_acc, spk_id=self.spk_id,
+                                  k_step=self.k_step, method=self.diff_method, silence_front=self.silence_front,
+                                  use_silence=self.diff_silence, spk_mix_dict=self.spk_mix_dict, **self.draws())
+        out = frontend.mask_apply_(out.reshape(1, -1).contiguous(), mask, self.block_size)
         self._tail(out, self.model_sr)
 
     def run(self):

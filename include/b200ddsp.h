@@ -325,7 +325,9 @@ int b2d_cross_fade(const float* a, int64_t len_a, const float* b, int64_t len_b,
  * [B, T, C] fp32; the model width is 256 as in the reference.
  * u2c_embed (:93-102): x [B*T, 256] += f0_embed(log(1 + f0/700)) + phase_embed(phase/pi) + volume_embed(volume) + spk
  *   (+ aug_embed(aug_shift/5)); embed_table [7, 256] = f0 w, f0 b, phase w, phase b, volume w, volume b, aug w;
- *   spk [spk_rows, 256] (spk_rows 1 or B) or NULL; aug_shift [B] or NULL.
+ *   spk [spk_rows, 256] (spk_rows 1 or B) or NULL; aug_shift [B] or NULL.  phase NULL leaves the phase term out (rows
+ *   2-3 of embed_table are then not read): x + f0 term + volume term (+ spk) (+ aug), the condition of the diffusion
+ *   model Unit2Mel (diffusion/vocoder.py:206-215), in its association.
  * u2c_groupnorm_lrelu (:50-52): GroupNorm(groups, C = 256) with statistics over (C/groups channels x T) of each utterance,
  *   then LeakyReLU(slope), in place; stats_ws: B * groups * 2 doubles of scratch.
  * u2c_layernorm: LayerNorm over the last dimension C (multiple of 32, <= 1024) of n_tokens rows.
