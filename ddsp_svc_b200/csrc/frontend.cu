@@ -5,10 +5,16 @@
 //   * silence mask                    main.py:210-214           threshold, 4-frame edge padding, 9-frame max (dilation)
 //   * mask upsample x multiply        main.py:215,260           `seg_output *= upsample(mask, block)` (ddsp/core.py:66-70)
 //   * segment cross-fade              main.py:142-149           linear fade over the overlap of two rendered segments
+//   * Slicer's frame RMS              slicer.py (main.py:124)   librosa.feature.rms(center=True, constant padding), fp64
+//   * segment placement               main.py:266-273           one segment into the whole-file result, faded in place
 //
 // All are HBM-bound, one pass, coalesced 128-bit accesses where alignment allows; algorithmic bytes: volume 4 B per input
-// sample read, mask-apply 8 B per sample (read + write in place), cross-fade 12 B per overlapped sample.
+// sample read, mask-apply 8 B per sample (read + write in place), cross-fade 12 B per overlapped sample, slicer RMS
+// 4 B per sample per overlapping frame (frame_length / hop of them), placement 8 B per segment sample (+4 B faded).
+// No atomics: every output has one writer and a fixed summation order, so results are bit-identical run to run.
+#ifndef B2D_HOST_EMU               // tests/emu/ runs these kernels' source on the CPU (host_emu.h provides the shims)
 #include "b2d_common.cuh"
+#endif
 
 namespace {
 
@@ -94,25 +100,70 @@ __global__ void __launch_bounds__(256) mask_apply_kernel(float* __restrict__ sig
     }
 }
 
+// sample r < fade of main.py:147's fade, (1 - k_r) a + k_r b in fp64 rounded to fp32, k = numpy.linspace(0, 1, fade):
+// k_r = r * step with step = 1 / (fade - 1) (the caller's fade_step), the end point pinned to exactly 1, [0] for fade 1
+__device__ __forceinline__ double fade_step(long long fade) { return fade > 1 ? 1.0 / (double)(fade - 1) : 0.0; }
+__device__ __forceinline__ float fade_sample(float a, float b, long long r, long long fade, double step) {
+    const double k = (fade == 1) ? 0.0 : (r == fade - 1 ? 1.0 : (double)r * step);   // linspace pins the end point
+    return (float)((1.0 - k) * (double)a + k * (double)b);
+}
+
 // out = [ a[:idx] | (1-k) a[idx:] + k b[:fade] | b[fade:] ],  fade = len_a - idx,  k = linspace(0, 1, fade)   (main.py:142-149)
 __global__ void __launch_bounds__(256) cross_fade_kernel(const float* __restrict__ a, long long len_a, const float* __restrict__ b,
                                                          long long len_b, long long idx, float* __restrict__ out) {
     const long long fade = len_a - idx, total = idx + len_b;
-    const double step = fade > 1 ? 1.0 / (double)(fade - 1) : 0.0;            // numpy.linspace(0, 1, fade): k_i = i / (fade - 1)
+    const double step = fade_step(fade);
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         float v;
         if (i < idx) v = a[i];
         else if (i < len_a) {
             const long long r = i - idx;
-            const double k = (fade == 1) ? 0.0 : (r == fade - 1 ? 1.0 : (double)r * step);   // linspace pins the end point
-            v = (float)((1.0 - k) * (double)a[i] + k * (double)b[r]);
+            v = fade_sample(a[i], b[r], r, fade, step);
         } else v = b[i - idx];
         out[i] = v;
     }
 }
 
+// main.py's assembly step for one segment, in place on the whole-file result (zero where nothing was written yet):
+// result[idx + r] = fade_sample(result[idx + r], seg[r], r, fade_len) for r < fade_len, = seg[r] after, r < seg_len.
+// The samples from idx + seg_len on are left alone: main.py's cross_fade drops nothing there, since fade_len <= seg_len.
+__global__ void __launch_bounds__(256) segment_place_kernel(float* __restrict__ result, const float* __restrict__ seg,
+                                                            long long seg_len, long long idx, long long fade_len) {
+    const double step = fade_step(fade_len);
+    for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < seg_len; r += (long long)gridDim.x * blockDim.x)
+        result[idx + r] = r < fade_len ? fade_sample(result[idx + r], seg[r], r, fade_len, step) : seg[r];
+}
+
+// warp-wide fp64 sum, butterfly order (every lane ends with the same bits)
+__device__ __forceinline__ double warp_sum(double v) {
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
+    return v;
+}
+
+// librosa.feature.rms(y, frame_length, hop_length) as the reference's Slicer calls it (center=True, constant padding):
+// frame f covers y[f hop - frame_length / 2 + j], j < frame_length, zero outside the signal, and
+// rms[f] = sqrt(sum_j y^2 / frame_length), squares exact and summed in fp64, rounded to fp32 once.  One warp per frame;
+// each lane sums its strided samples in order, then the warp's butterfly: a fixed order, so the result is deterministic.
+__global__ void __launch_bounds__(256) slicer_rms_kernel(const float* __restrict__ y, long long n, int frame_length, int hop,
+                                                         long long n_frames, float* __restrict__ rms) {
+    const long long f = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (f >= n_frames) return;
+    const long long start = f * hop - frame_length / 2;
+    const long long j0 = start < 0 ? -start : 0, j1 = min((long long)frame_length, n - start);
+    double acc = 0.0;
+    for (long long j = j0 + lane; j < j1; j += 32) {
+        const double v = (double)y[start + j];
+        acc += v * v;
+    }
+    acc = warp_sum(acc);
+    if (lane == 0) rms[f] = (float)sqrt(acc / (double)frame_length);
+}
+
 }  // namespace
 
+#ifndef B2D_HOST_EMU
 extern "C" int b2d_volume_extract(const float* audio, int B, int n_samples, int hop, float* volume, void* stream) {
     if (!audio || !volume) return b2d::fail(B2D_ERR_NULL, "volume_extract: null pointer");
     if (B <= 0 || n_samples < 2 || hop <= 0 || hop / 2 >= n_samples)
@@ -162,3 +213,33 @@ extern "C" int b2d_cross_fade(const float* a, int64_t len_a, const float* b, int
     cross_fade_kernel<<<(unsigned)gx, 256, 0, (cudaStream_t)stream>>>(a, len_a, b, len_b, idx, out);
     return b2d::check_launch("cross_fade");
 }
+
+extern "C" int b2d_slicer_rms(const float* audio, int64_t n_samples, int frame_length, int hop, float* rms, void* stream) {
+    if (!audio || !rms) return b2d::fail(B2D_ERR_NULL, "slicer_rms: null pointer");
+    if (n_samples <= 0 || frame_length <= 0 || hop <= 0)
+        return b2d::fail(B2D_ERR_SHAPE, "slicer_rms: bad shape n=%lld frame_length=%d hop=%d", (long long)n_samples,
+                         frame_length, hop);
+    const long long padded = (long long)n_samples + 2 * (frame_length / 2);
+    if (padded < frame_length)
+        return b2d::fail(B2D_ERR_SHAPE, "slicer_rms: %lld samples padded by %d each side are shorter than one frame of %d",
+                         (long long)n_samples, frame_length / 2, frame_length);
+    const long long n_frames = 1 + (padded - frame_length) / hop;
+    const long long blocks = (n_frames + 7) / 8;
+    if (blocks > 0x7fffffffLL) return b2d::fail(B2D_ERR_UNSUPPORTED, "slicer_rms: %lld frames", n_frames);
+    slicer_rms_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(audio, n_samples, frame_length, hop, n_frames, rms);
+    return b2d::check_launch("slicer_rms");
+}
+
+extern "C" int b2d_segment_place(float* result, int64_t result_len, const float* seg, int64_t seg_len, int64_t idx,
+                                 int64_t fade_len, void* stream) {
+    if (!result || !seg) return b2d::fail(B2D_ERR_NULL, "segment_place: null pointer");
+    if (seg_len <= 0 || idx < 0 || fade_len < 0 || fade_len > seg_len || idx + seg_len > result_len)
+        return b2d::fail(B2D_ERR_SHAPE, "segment_place: need idx >= 0, 0 <= fade_len <= seg_len and idx + seg_len <= "
+                         "result_len (got idx %lld, fade_len %lld, seg_len %lld, result_len %lld)", (long long)idx,
+                         (long long)fade_len, (long long)seg_len, (long long)result_len);
+    long long gx = (seg_len + 255) / 256;
+    if (gx > b2d::num_sms() * 16) gx = b2d::num_sms() * 16;
+    segment_place_kernel<<<(unsigned)gx, 256, 0, (cudaStream_t)stream>>>(result, seg, seg_len, idx, fade_len);
+    return b2d::check_launch("segment_place");
+}
+#endif  // B2D_HOST_EMU

@@ -2,6 +2,8 @@
 drivers do in numpy around `model(...)` -- Volume_Extractor (ddsp/vocoder.py:147-157), the silence mask (main.py:210-215),
 `seg_output *= mask` (main.py:260) and the segment cross-fade (main.py:142-149) -- as streaming kernels of
 libb200ddsp.so, so a rendered segment never has to leave the device between the synthesizer and the enhancer.
+``slicer_rms`` and ``segment_place_`` are the two device halves of main.py's whole-file loop (offline.py): the Slicer's
+frame RMS and the placement of one converted segment into the result.
 
 ``Volume_Extractor`` keeps the reference's constructor and ``extract`` contract (1-D numpy in -> 1-D numpy out) and
 additionally accepts CUDA tensors ([T] or [B, T]) and then returns a CUDA tensor.
@@ -71,6 +73,41 @@ def cross_fade(a, b, idx):
                "b2d_cross_fade")
     _count(1)
     return out
+
+
+def slicer_rms_frames(n_samples, frame_length, hop):
+    """the frames librosa.feature.rms(center=True) makes of n_samples: 1 + (n + 2 (frame_length // 2) - frame_length) // hop"""
+    return 1 + (int(n_samples) + 2 * (int(frame_length) // 2) - int(frame_length)) // int(hop)
+
+
+def slicer_rms(audio, frame_length, hop):
+    """audio [N] CUDA fp32 -> rms [slicer_rms_frames(N, frame_length, hop)]: librosa.feature.rms(y=audio,
+    frame_length=frame_length, hop_length=hop) as the reference's Slicer calls it (center=True, zero padding), in fp64
+    rounded to fp32 (b2d_slicer_rms)."""
+    _need_cuda_f32("audio", audio)
+    if audio.dim() != 1:
+        raise ValueError("audio must be 1-D [n_samples]")
+    audio = audio.contiguous()
+    out = torch.empty(slicer_rms_frames(audio.shape[0], frame_length, hop), dtype=torch.float32, device=audio.device)
+    _lib.check(_lib.lib().b2d_slicer_rms(audio.data_ptr(), audio.shape[0], int(frame_length), int(hop), out.data_ptr(),
+                                         _stream()), "b2d_slicer_rms")
+    _count(1)
+    return out
+
+
+def segment_place_(result, seg, idx, fade_len):
+    """In place: result[idx : idx + len(seg)] = seg, its first fade_len samples cross-faded against what result holds
+    there with numpy.linspace(0, 1, fade_len) in fp64 (main.py:142-149 and :266-273; b2d_segment_place).  Returns
+    ``result``."""
+    _need_cuda_f32("result", result)
+    _need_cuda_f32("seg", seg)
+    if result.dim() != 1 or seg.dim() != 1 or not result.is_contiguous():
+        raise ValueError("segment_place_ takes a contiguous 1-D result and a 1-D segment")
+    seg = seg.contiguous()
+    _lib.check(_lib.lib().b2d_segment_place(result.data_ptr(), result.shape[0], seg.data_ptr(), seg.shape[0], int(idx),
+                                            int(fade_len), _stream()), "b2d_segment_place")
+    _count(1)
+    return result
 
 
 class Volume_Extractor:

@@ -77,6 +77,13 @@ def model_hop(samplerate, model_sr, block_size, who):
     return int(hop)
 
 
+def units_encoder(data, device):
+    """the checkpoint config's data section -> its Units_Encoder, built as main.py and the GUIs build it (the
+    cnhubertsoft_gate from the config, 10 without one)"""
+    return Units_Encoder(data.encoder, data.encoder_ckpt, data.encoder_sample_rate, data.encoder_hop_size, device=device,
+                         cnhubertsoft_gate=getattr(data, "cnhubertsoft_gate", None) or 10)
+
+
 def reflow_frames(samplerate, block_time, crossfade_time, extra_time, model_sr, block_size, vocoder_hop,
                   win_size=2048):
     """The frame bookkeeping of one gui_reflow.py block -> dict:
@@ -174,9 +181,7 @@ class _Session:
         self.threhold = float(threhold)
         self.model_sr, self.block_size = int(data.sampling_rate), int(data.block_size)
         self.hop = model_hop(self.sr, self.model_sr, self.block_size, who)
-        self.units_encoder = Units_Encoder(data.encoder, data.encoder_ckpt, data.encoder_sample_rate,
-                                           data.encoder_hop_size, device=dev,
-                                           cnhubertsoft_gate=getattr(data, "cnhubertsoft_gate", None) or 10)
+        self.units_encoder = units_encoder(data, dev)
         self.rmvpe = RMVPE(rmvpe_ckpt, hop_length=160)
         self.to_device_rate = Resampler(self.sr)
         self.n_frames = self.n_in // self.hop + 1

@@ -320,6 +320,19 @@ int b2d_mask_apply(float* signal, const float* mask_frames, int B, int n_mask_fr
  * k = linspace(0, 1, len_a - idx) evaluated in fp64.  Requires 0 <= idx < len_a and len_a - idx <= len_b. */
 int b2d_cross_fade(const float* a, int64_t len_a, const float* b, int64_t len_b, int64_t idx, float* out, void* stream);
 
+/* The reference Slicer's frame RMS (slicer.py, called by main.py's split): librosa.feature.rms(y, frame_length, hop)
+ * with center=True and constant (zero) padding of frame_length / 2 each side -> rms [1 + (n_samples + 2 (frame_length / 2)
+ * - frame_length) / hop], rms[f] = sqrt(sum_{j < frame_length} y[f hop - frame_length / 2 + j]^2 / frame_length), summed
+ * in fp64 and rounded to fp32 once.  Deterministic (no atomics). */
+int b2d_slicer_rms(const float* audio, int64_t n_samples, int frame_length, int hop, float* rms, void* stream);
+
+/* main.py's assembly of one converted segment (main.py:266-273) in place on the whole-file result:
+ * result[idx + r] = (1 - k_r) result[idx + r] + k_r seg[r] for r < fade_len (k = linspace(0, 1, fade_len), fp64, as
+ * b2d_cross_fade), result[idx + r] = seg[r] for fade_len <= r < seg_len.  Requires idx >= 0,
+ * 0 <= fade_len <= seg_len and idx + seg_len <= result_len. */
+int b2d_segment_place(float* result, int64_t result_len, const float* seg, int64_t seg_len, int64_t idx,
+                      int64_t fade_len, void* stream);
+
 /* ---- fused frame-rate kernels of the control network (Unit2Control inference, ddsp/unit2control.py:84-109 with
  * ddsp/pcmer.py / diffusion/model_conformer_naive.py): everything that is not a plain GEMM.  Activations are token-major
  * [B, T, C] fp32; the model width is 256 as in the reference.
