@@ -218,6 +218,17 @@ class Unit2WavFast(nn.Module):
                         step_noise, rand_ini, sine_noise)
 
 
+#: the data fields a DDSP checkpoint must share with the diffusion model to feed its shallow diffusion, in
+#: main_diff.py's check_args order
+DATA_FIELDS = ("sampling_rate", "block_size", "encoder")
+
+
+def data_mismatches(ddsp_args, diff_args):
+    """the DATA_FIELDS in which the two configs differ, in that order (empty when the DDSP model can feed the diffusion
+    model): the comparison of main_diff.py's / batch_infer.py's check_args and infer_gt_mel.py's"""
+    return [f for f in DATA_FIELDS if getattr(ddsp_args.data, f) != getattr(diff_args.data, f)]
+
+
 class DiffGtMel:
     """diffusion/infer_gt_mel.py on the package's cascade.  Beyond the reference, ``__call__`` and ``infer`` take the
     draws (``ddsp_noise`` for Unit2Wav / Unit2WavFast's synthesizer, ``noise``, ``step_noise``, ``rand_ini``,
@@ -240,12 +251,10 @@ class DiffGtMel:
                 self.project_path = project_path
 
     def check_args(self, args1, args2):
-        if args1.data.block_size != args2.data.block_size:
-            raise ValueError("the DDSP and diffusion models' block_size differ")
-        if args1.data.sampling_rate != args2.data.sampling_rate:
-            raise ValueError("the DDSP and diffusion models' sampling_rate differ")
-        if args1.data.encoder != args2.data.encoder:
-            raise ValueError("the DDSP and diffusion models' encoder differ")
+        bad = data_mismatches(args1, args2)
+        for field in ("block_size", "sampling_rate", "encoder"):        # infer_gt_mel.py's order
+            if field in bad:
+                raise ValueError("the DDSP and diffusion models' %s differ" % field)
         return True
 
     def __call__(self, audio, f0, hubert, volume, acc=1, spk_id=1, k_step=0, method='pndm', spk_mix_dict=None,

@@ -12,8 +12,10 @@ and main_reflow.py build from ``args.vocoder.type`` / ``args.vocoder.ckpt``.
   (forward only).  Resampling has no backward: under grad with an audio that requires grad it raises.
 - ``infer(mel [B, n_frames, n_mels], f0 [B, >= n_frames, 1], rand_ini=None, noise=None) -> audio``: the package's
   NSF-HiFiGAN ``Generator``, built on first use from config.json and ``ckpt['generator']`` as
-  nsf_hifigan.models.load_model builds it.  ``rand_ini`` [1, 1, 9] / ``noise`` [B, n_frames upp, 9] (not in the
-  reference) take SineGen's draws, for seeded runs and CUDA graphs; without them it draws as the reference does.
+  nsf_hifigan.models.load_model builds it, with torch's CPU generator restored after the build (SineGen's noise seed
+  comes from it, so the first call draws what later calls draw under the same seed).  ``rand_ini`` [1, 1, 9] /
+  ``noise`` [B, n_frames upp, 9] (not in the reference) take SineGen's draws, for seeded runs and CUDA graphs; without
+  them it draws as the reference does.
 """
 import json
 import os
@@ -85,7 +87,10 @@ class Vocoder:
         f0 = f0[:, :mel.size(1), 0]                         # B, n_frames
         if self.model is None:
             print('| Load HifiGAN: ', self.model_path)
-            self.model, self.h = load_generator(self.model_path, self.device)
+            # the modules' default init draws from torch's CPU generator, which also seeds SineGen's noise below: a
+            # forked generator keeps the first call's draws those of every later call under the same seed
+            with torch.random.fork_rng(devices=[]):
+                self.model, self.h = load_generator(self.model_path, self.device)
         with torch.no_grad():
             c = mel.transpose(1, 2)
             if self.vocoder_type == "nsf-hifigan-log10":

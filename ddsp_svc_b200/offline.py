@@ -1,10 +1,14 @@
-"""The whole-file conversion of main.py and main_reflow.py on the device: the Slicer's cut, every segment's model call
-and the cross-faded assembly, queued on one stream without a host round trip per segment.
+"""The whole-file conversion of main.py, main_reflow.py, main_diff.py and batch_infer.py on the device: the Slicer's
+cut, every segment's model call and the cross-faded assembly, queued on one stream without a host round trip per
+segment.
 
 ``OfflineVC(model_path, device=None, enhance=True, rmvpe_ckpt=...)`` is main.py (its lines after the argument parsing,
 with the DDSP model of ``load_model`` and the ``Enhancer``); ``OfflineReflowVC(model_path, device=None, rmvpe_ckpt=...)``
-is main_reflow.py (``load_model_vocoder``'s Unit2Wav and its vocoder).  Both take mono CUDA fp32 audio [N] and return
-CUDA fp32 audio [N_out] with its sample rate; file I/O and the f0 cache stay with the caller.
+is main_reflow.py (``load_model_vocoder``'s Unit2Wav and its vocoder); ``OfflineDiffVC(diff_model_path,
+ddsp_model_path=None, device=None, rmvpe_ckpt=...)`` is main_diff.py (``convert``) and batch_infer.py
+(``convert_whole``) on diffusion_vocoder's Unit2Mel / Unit2Wav / Unit2WavFast, with an optional external DDSP model
+for the shallow diffusion (``diff_settings`` picks the mode as each driver does).  All take mono CUDA fp32 audio [N]
+and return CUDA fp32 audio [N_out] with its sample rate; file I/O and the f0 cache stay with the caller.
 
 - ``split(audio, sample_rate)`` -> [(start_frame, end_frame)]: main.py's ``split()`` (db_thresh -40, min_len 5000 ms).
   The Slicer's frame RMS is ``frontend.slicer_rms`` on the device, copied back once; its silence state machine and
@@ -12,20 +16,27 @@ CUDA fp32 audio [N_out] with its sample rate; file I/O and the f0 cache stay wit
 - ``convert(audio, sample_rate, ..., segments=None)``: f0 for the whole file (RMVPE, then ``ops.rt_f0_regrid``:
   F0_Extractor's 'rmvpe' post-processing with uv_interp and the key's pitch factor), volume and mask for the whole
   file, then per segment, in main.py's order: units of a view of the segment, f0 / volume sliced to its unit frames,
-  the model, the mask at the segment's frame offset and the enhancer (main.py) or the vocoder (main_reflow.py).
+  the model, the mask at the segment's frame offset and the enhancer (main.py) or the vocoder (main_reflow.py,
+  main_diff.py, after the shallow diffusion's mel of the external DDSP model or of the input).
   ``frontend.segment_place_`` writes each output into the zero-filled result with main.py's fade; ``assembly_plan``
   is main.py's integer bookkeeping (``silent_length`` / ``current_length``), which needs only the output lengths.
   With ``segments`` given and a numeric ``enhancer_adaptive_key``, the call queues all its work without a host
-  synchronisation; ``'auto'`` reads one scalar per segment, as the reference's Enhancer does.
+  synchronisation (so do OfflineDiffVC's ``convert`` and ``convert_whole`` once a call at the same settings has built
+  the sampler's cached step rows); ``'auto'`` reads one scalar per segment, as the reference's Enhancer does.
 - ``render(...)`` is ``convert`` without the assembly: the segments' outputs, for callers that place them themselves.
+- ``OfflineDiffVC.convert_whole(...)`` is batch_infer.py's infer(): no split, one model call over the whole input and
+  the mask over the whole output.
 
 Only 'rmvpe' f0 and integer hops (block_size * sample_rate / sampling_rate) are supported: the volume kernel needs an
 integer hop, as in the real-time sessions.
 """
+import collections
+import warnings
+
 import numpy as np
 import torch
 
-from . import frontend, ops
+from . import diffusion_vocoder, frontend, ops
 from .dropin import load_model
 from .enhancer import Enhancer
 from .realtime import model_hop, units_encoder
@@ -321,3 +332,143 @@ class OfflineReflowVC(_Offline):
         return super().convert(audio, sample_rate, key=key, spk_id=spk_id, spk_mix_dict=spk_mix_dict, f0_min=f0_min,
                                f0_max=f0_max, threhold=threhold, formant_shift_key=formant_shift_key,
                                infer_step=infer_step, method=method, t_start=t_start, segments=segments)
+
+
+DiffSettings = collections.namedtuple("DiffSettings", "mode k_step infer_speedup method diff_spk_id")
+
+
+def diff_settings(args, ddsp_args, k_step=None, speedup="auto", method="auto", diff_spk_id="auto", whole=False):
+    """main_diff.py's choices (``whole`` False) or batch_infer.py's (True) for a diffusion model's config ``args`` and a
+    DDSP checkpoint's config ``ddsp_args`` (None without one) -> DiffSettings(mode, k_step, infer_speedup, method,
+    diff_spk_id).
+
+    ``mode`` is where the shallow diffusion's mel comes from: 'ddsp' (the external DDSP model's output), 'input_mel'
+    (the input's own mel, a 'Diffusion' model with a k_step and no usable DDSP model) or 'none' (no gt_spec: the
+    built-in DDSP model of 'DiffusionNew' / 'DiffusionFast', or sampling from noise).  A DDSP checkpoint is usable when
+    its sampling_rate, block_size and encoder match (``diffusion_vocoder.data_mismatches``).  The two drivers differ:
+    - a 'Diffusion' model with a k_step and an unusable DDSP checkpoint samples from noise in main_diff.py but from the
+      input's mel in batch_infer.py;
+    - batch_infer.py loads the DDSP checkpoint of a 'DiffusionFast' model only with a k_step.
+    k_step is clamped to model.k_step_max (its default when None) for 'DiffusionNew' and 'DiffusionFast' only; a
+    'Diffusion' model keeps the given k_step or None.  'auto' speedup / method read infer.speedup / infer.method and
+    raise ValueError without them; ``diff_spk_id`` is None for 'auto' (the DDSP model's speaker) or the given id."""
+    def infer(key):
+        section = args.infer
+        if section is None or section.get(key) is None:
+            raise ValueError("%s='auto' needs infer.%s in the model's config" % (key, key))
+        return section.get(key)
+
+    infer_speedup = infer("speedup") if speedup == "auto" else int(speedup)
+    method = infer("method") if method == "auto" else method
+    usable = ddsp_args is not None and not diffusion_vocoder.data_mismatches(ddsp_args, args)
+    kind = args.model.type
+    if kind in ("DiffusionNew", "DiffusionFast"):
+        loaded = not whole or kind == "DiffusionNew" or k_step is not None
+        k_step = args.model.k_step_max if k_step is None else min(int(k_step), args.model.k_step_max)
+        mode = "ddsp" if usable and loaded else "none"
+    elif kind == "Diffusion":
+        if k_step is None:
+            mode = "none"
+        else:
+            k_step = int(k_step)
+            mode = "ddsp" if usable else "input_mel" if ddsp_args is None or whole else "none"
+    else:
+        raise ValueError(f" [x] Unknown Model: {kind}")
+    return DiffSettings(mode, k_step, infer_speedup, method, None if diff_spk_id == "auto" else int(diff_spk_id))
+
+
+class OfflineDiffVC(_Offline):
+    """main_diff.py's conversion (``convert``) and batch_infer.py's (``convert_whole``) on ``load_model_vocoder``'s
+    diffusion model and its vocoder, with the shallow diffusion fed by an optional external DDSP model of
+    ``load_model``.  A DDSP checkpoint whose sampling_rate, block_size or encoder differ from the diffusion model's is
+    dropped with a warning naming the field, as main_diff.py drops it with a message."""
+
+    def __init__(self, diff_model_path, ddsp_model_path=None, device=None, rmvpe_ckpt="pretrain/rmvpe/model.pt",
+                 pitch_extractor="rmvpe"):
+        self._init_device(device, pitch_extractor, "OfflineDiffVC")
+        self.model, self.vocoder, self.args = diffusion_vocoder.load_model_vocoder(diff_model_path, device=self.device)
+        self.ddsp_model, self.ddsp_args = None, None
+        if ddsp_model_path is not None:
+            self.ddsp_model, self.ddsp_args = load_model(ddsp_model_path, device=self.device)
+            bad = diffusion_vocoder.data_mismatches(self.ddsp_args, self.args)
+            if bad:
+                warnings.warn("the DDSP model's data.%s differs from the diffusion model's: it cannot feed the shallow "
+                              "diffusion and is not used" % bad[0], stacklevel=2)
+                self.ddsp_model = None
+        self._init_front(self.args.data, rmvpe_ckpt)
+
+    def settings(self, k_step=None, speedup="auto", method="auto", diff_spk_id="auto", whole=False):
+        """diff_settings for this model and DDSP checkpoint"""
+        return diff_settings(self.args, self.ddsp_args, k_step, speedup, method, diff_spk_id, whole)
+
+    def _input_mel(self, audio, sample_rate):
+        """the input's mel with its last frame repeated (main_diff.py:338-339) -> [1, n_frames, M]"""
+        mel = self.vocoder.extract(audio[None], sample_rate)
+        return torch.cat((mel, mel[:, -1:, :]), 1)
+
+    def _synthesize(self, s, units, f0, volume, spk, diff_spk, spk_mix_dict, aug, formant_shift_key, input_mel):
+        """one segment of main_diff.py's loop or batch_infer.py's infer() call, before the mask: the shallow
+        diffusion's mel of s.mode, the model, the vocoder -> audio [1, 1, n block_size]"""
+        if s.mode == "ddsp":
+            ddsp_f0 = 2 ** (-float(formant_shift_key) / 12) * f0
+            out, _, _ = self.ddsp_model(units, ddsp_f0, volume, spk_id=spk, spk_mix_dict=spk_mix_dict)
+            # n_units frames already; batch_infer.py's [:, :n_units] is a no-op on it
+            gt_spec = self.vocoder.extract(out, self.model_sr, keyshift=float(formant_shift_key))
+        elif s.mode == "input_mel":
+            gt_spec = input_mel
+        else:
+            gt_spec = None
+        mel = self.model(units, f0, volume, spk_id=diff_spk, spk_mix_dict=spk_mix_dict, aug_shift=aug,
+                         vocoder=self.vocoder, gt_spec=gt_spec, infer=True, infer_speedup=s.infer_speedup,
+                         method=s.method, k_step=s.k_step, use_tqdm=False)
+        return self.vocoder.infer(mel, f0)
+
+    def _speakers(self, s, spk_id, formant_shift_key):
+        spk = self._spk_id(spk_id)
+        diff_spk = spk if s.diff_spk_id is None else self._spk_id(s.diff_spk_id)
+        aug = torch.full((1, 1), float(formant_shift_key), dtype=torch.float32, device=self.device)
+        return spk, diff_spk, aug
+
+    def render(self, audio, sample_rate, key=0, spk_id=1, spk_mix_dict=None, f0_min=50, f0_max=1100, threhold=-60,
+               formant_shift_key=0, diff_spk_id="auto", speedup="auto", method="auto", k_step=None, segments=None):
+        """convert() without the assembly -> ([(start_frame, output [T])], the model's sample rate)"""
+        _need_audio(audio)
+        sample_rate = int(sample_rate)
+        s = self.settings(k_step, speedup, method, diff_spk_id, whole=False)
+        rendered = []
+        with torch.cuda.device(self.device), torch.no_grad():
+            spk, diff_spk, aug = self._speakers(s, spk_id, formant_shift_key)
+            input_mel = self._input_mel(audio, sample_rate) if s.mode == "input_mel" else None
+            for start, units, f0, volume, mask in self._segments(audio, sample_rate, key, f0_min, threhold, segments):
+                seg_mel = input_mel[:, start:start + units.size(1)] if input_mel is not None else None
+                out = self._synthesize(s, units, f0, volume, spk, diff_spk, spk_mix_dict, aug, formant_shift_key,
+                                       seg_mel)
+                rendered.append((start, self._mask(out, mask, start).reshape(-1)))
+        return rendered, self.model_sr
+
+    def convert(self, audio, sample_rate, key=0, spk_id=1, spk_mix_dict=None, f0_min=50, f0_max=1100, threhold=-60,
+                formant_shift_key=0, diff_spk_id="auto", speedup="auto", method="auto", k_step=None, segments=None):
+        """main_diff.py's whole-file conversion, sliced and cross-faded -> (output [N_out] CUDA fp32, the model's
+        sample rate)"""
+        return super().convert(audio, sample_rate, key=key, spk_id=spk_id, spk_mix_dict=spk_mix_dict, f0_min=f0_min,
+                               f0_max=f0_max, threhold=threhold, formant_shift_key=formant_shift_key,
+                               diff_spk_id=diff_spk_id, speedup=speedup, method=method, k_step=k_step,
+                               segments=segments)
+
+    def convert_whole(self, audio, sample_rate, key=0, spk_id=1, spk_mix_dict=None, f0_min=50, f0_max=1100,
+                      threhold=-60, formant_shift_key=0, diff_spk_id="auto", speedup="auto", method="auto",
+                      k_step=None):
+        """batch_infer.py's infer(): the whole input in one model call, unsliced -> (output [n_frames block_size]
+        CUDA fp32, the model's sample rate)"""
+        _need_audio(audio)
+        sample_rate = int(sample_rate)
+        s = self.settings(k_step, speedup, method, diff_spk_id, whole=True)
+        with torch.cuda.device(self.device), torch.no_grad():
+            hop = self.hop(sample_rate)
+            f0, volume, mask = self._front(audio, sample_rate, key, f0_min, threhold)
+            units = self.units_encoder.encode(audio[None], sample_rate, hop)
+            input_mel = self._input_mel(audio, sample_rate)[:, :units.size(1)] if s.mode == "input_mel" else None
+            spk, diff_spk, aug = self._speakers(s, spk_id, formant_shift_key)
+            out = self._synthesize(s, units, f0, volume[..., None], spk, diff_spk, spk_mix_dict, aug,
+                                   formant_shift_key, input_mel)
+            return self._mask(out, mask, 0).reshape(-1), self.model_sr
