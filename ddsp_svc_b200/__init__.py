@@ -15,12 +15,12 @@ from .diffusion_vocoder import DiffGtMel, Unit2Mel, Unit2WavFast  # noqa: F401
 from .dropin import build_model, load_model, patch_reference, unpatch_reference  # noqa: F401
 from .offline import OfflineDiffVC, OfflineReflowVC, OfflineVC  # noqa: F401
 from .pipeline import HostPipeline  # noqa: F401
-from .realtime import RealtimeDiffVC, RealtimeReflowVC, RealtimeVC  # noqa: F401
+from .realtime import BatchedRealtimeVC, RealtimeDiffVC, RealtimeReflowVC, RealtimeVC  # noqa: F401
 from .reflow import NaiveV2Diff, RectifiedFlow  # noqa: F401
 from .reflow_vocoder import Unit2Wav, load_model_vocoder  # noqa: F401
 from .rmvpe import E2E0, RMVPE  # noqa: F401
 from .sinegen import SineGen, SourceModuleHnNSF  # noqa: F401
 from .vocoder import CombSub, CombSubFast, CombSubSuperFast, FixedControls, Sins  # noqa: F401
 
-__all__ = ["Sins", "CombSub", "CombSubSuperFast", "CombSubFast", "SineGen", "SourceModuleHnNSF", "FixedControls", "HostPipeline", "RealtimeVC", "RealtimeReflowVC", "RealtimeDiffVC", "OfflineVC", "OfflineReflowVC", "OfflineDiffVC", "NaiveV2Diff", "RectifiedFlow", "Unit2Wav", "Unit2Mel", "Unit2WavFast", "DiffGtMel", "WaveNet", "GaussianDiffusion", "Generator", "E2E0", "RMVPE", "HubertSoft", "Units_Encoder", "load_fairseq_hubert", "Vocoder", "Enhancer", "Volume_Extractor", "RSSLoss", "frontend", "loss", "mel", "ops", "synthetic", "sharding",
+__all__ = ["Sins", "CombSub", "CombSubSuperFast", "CombSubFast", "SineGen", "SourceModuleHnNSF", "FixedControls", "HostPipeline", "RealtimeVC", "BatchedRealtimeVC", "RealtimeReflowVC", "RealtimeDiffVC", "OfflineVC", "OfflineReflowVC", "OfflineDiffVC", "NaiveV2Diff", "RectifiedFlow", "Unit2Wav", "Unit2Mel", "Unit2WavFast", "DiffGtMel", "WaveNet", "GaussianDiffusion", "Generator", "E2E0", "RMVPE", "HubertSoft", "Units_Encoder", "load_fairseq_hubert", "Vocoder", "Enhancer", "Volume_Extractor", "RSSLoss", "frontend", "loss", "mel", "ops", "synthetic", "sharding",
            "patch_reference", "unpatch_reference", "load_model", "build_model", "load_model_vocoder"]

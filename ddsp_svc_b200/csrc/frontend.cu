@@ -48,10 +48,13 @@ __global__ void __launch_bounds__(256) volume_extract_kernel(const float* __rest
 }
 
 // mask[n] = max_{|d| <= 4} (volume[clamp(n + d)] > thr)      (main.py:211-213: edge-pad by 4, 9-frame running max)
-__global__ void volume_mask_kernel(const float* __restrict__ volume, int n_frames, float thr, float* __restrict__ mask) {
+// thr_rows: row b's threshold thr_rows[b] (b2d_volume_mask_rows); null: thr for every row
+__global__ void volume_mask_kernel(const float* __restrict__ volume, int n_frames, float thr,
+                                   const float* __restrict__ thr_rows, float* __restrict__ mask) {
     const int b = blockIdx.y;
     const int n = blockIdx.x * blockDim.x + threadIdx.x;
     if (n >= n_frames) return;
+    if (thr_rows) thr = thr_rows[b];
     const float* v = volume + (size_t)b * n_frames;
     float m = 0.f;
 #pragma unroll
@@ -179,8 +182,18 @@ extern "C" int b2d_volume_mask(const float* volume, int B, int n_frames, float t
     if (!volume || !mask) return b2d::fail(B2D_ERR_NULL, "volume_mask: null pointer");
     if (B <= 0 || n_frames <= 0 || B > 65535) return b2d::fail(B2D_ERR_SHAPE, "volume_mask: bad shape B=%d nF=%d", B, n_frames);
     dim3 grid((n_frames + 255) / 256, B);
-    volume_mask_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(volume, n_frames, threshold, mask);
+    volume_mask_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(volume, n_frames, threshold, nullptr, mask);
     return b2d::check_launch("volume_mask");
+}
+
+extern "C" int b2d_volume_mask_rows(const float* volume, int B, int n_frames, const float* thresholds, float* mask,
+                                    void* stream) {
+    if (!volume || !thresholds || !mask) return b2d::fail(B2D_ERR_NULL, "volume_mask_rows: null pointer");
+    if (B <= 0 || n_frames <= 0 || B > 65535)
+        return b2d::fail(B2D_ERR_SHAPE, "volume_mask_rows: bad shape B=%d nF=%d", B, n_frames);
+    dim3 grid((n_frames + 255) / 256, B);
+    volume_mask_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(volume, n_frames, 0.f, thresholds, mask);
+    return b2d::check_launch("volume_mask_rows");
 }
 
 extern "C" int b2d_mask_apply(float* signal, const float* mask_frames, int B, int n_mask_frames, int frame_offset,

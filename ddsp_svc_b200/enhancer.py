@@ -2,8 +2,8 @@
 on the DDSP output, on the kernels end to end.
 
 ``Enhancer(enhancer_type, enhancer_ckpt, device=None)`` loads the package's ``Generator`` from the checkpoint and its
-config.json.  ``enhance(audio [1, T], sample_rate, f0 [1, n_frames, 1], hop_size, adaptive_key=0, silence_front=0)
--> (audio [1, 1, T'], enhancer_sample_rate)`` keeps the reference's contract:
+config.json.  ``enhance(audio [B, T], sample_rate, f0 [B, n_frames, 1], hop_size, adaptive_key=0, silence_front=0)
+-> (audio [B, 1, T'], enhancer_sample_rate)`` keeps the reference's contract:
 
 - audio is resampled to the adaptive rate and back with torchaudio's lowpass_filter_width=128 table
   (rmvpe.Resampler), on the kernels;
@@ -14,7 +14,9 @@ config.json.  ``enhance(audio [1, T], sample_rate, f0 [1, n_frames, 1], hop_size
 
 Two additions serve graph capture (realtime.RealtimeVC): ``prepare(sample_rate, keys)`` builds the resampling tables
 of those adaptive keys ahead of time, and ``enhance(..., rand_ini=, noise=)`` takes the generator's draws from the
-caller ([1, 1, 9] and [1, >= n_mel_frames hop, 9]) instead of the in-kernel generator, whose seed is a host integer.
+caller ([1, 1, 9] and [B, >= n_mel_frames hop, 9]) instead of the in-kernel generator, whose seed is a host integer.
+A third serves independent sessions in one batch (realtime.BatchedRealtimeVC): audio [B, T] and f0 [B, n_frames, 1]
+at a numeric key, every row enhanced on its own; 'auto' would pick one key per row, so it takes B = 1.
 """
 import numpy as np
 import torch
@@ -73,10 +75,14 @@ class Enhancer:
                 self._resampler(self.enhancer_sample_rate)(x, rate)
 
     def enhance(self, audio, sample_rate, f0, hop_size, adaptive_key=0, silence_front=0, rand_ini=None, noise=None):
-        if not (isinstance(audio, torch.Tensor) and audio.is_cuda and audio.dim() == 2 and audio.shape[0] == 1):
-            raise ValueError("audio must be a [1, T] CUDA tensor")
-        if not (isinstance(f0, torch.Tensor) and f0.is_cuda and f0.dim() == 3 and f0.shape[0] == 1):
-            raise ValueError("f0 must be a [1, n_frames, 1] CUDA tensor")
+        if not (isinstance(audio, torch.Tensor) and audio.is_cuda and audio.dim() == 2):
+            raise ValueError("audio must be a [B, T] CUDA tensor")
+        B = audio.shape[0]
+        if not (isinstance(f0, torch.Tensor) and f0.is_cuda and f0.dim() == 3 and f0.shape[0] == B):
+            raise ValueError("f0 must be a [B, n_frames, 1] CUDA tensor with audio's B = %d rows" % B)
+        if adaptive_key == 'auto' and B != 1:
+            raise ValueError("adaptive_key 'auto' picks a key, and so a sample rate, from one utterance's f0: enhance "
+                             "%d rows at a numeric key, or one row at a time" % B)
         start_frame = int(silence_front * sample_rate / hop_size)
         real_silence_front = start_frame * hop_size / sample_rate
         audio = audio[:, int(np.round(real_silence_front * sample_rate)):]
@@ -90,16 +96,16 @@ class Enhancer:
         if hop_size == self.enhancer_hop_size and sample_rate == self.enhancer_sample_rate and sample_rate == rate:
             f0_res = f0.squeeze(-1)
         else:
-            f0_res = ops.rt_f0_regrid(f0[0, :, 0].float().contiguous(), hop_size / sample_rate, n_frames,
-                                      self.enhancer_hop_size / self.enhancer_sample_rate, src_div=real_factor,
-                                      src_scale=real_factor).unsqueeze(0)
+            f0_res = ops.rt_f0_regrid_batch(f0[:, :, 0].float().contiguous(), hop_size / sample_rate, n_frames,
+                                            self.enhancer_hop_size / self.enhancer_sample_rate, src_div=real_factor,
+                                            src_scale=real_factor)
         with torch.no_grad():
             mel = self.stft.get_mel(audio_res)
             if noise is not None:
                 noise = noise[:, :mel.size(-1) * self.enhancer_hop_size]
             enhanced = self.model(mel, f0_res[:, :mel.size(-1)], rand_ini=rand_ini, noise=noise)
         if rate != self.enhancer_sample_rate:
-            enhanced = self._resample(enhanced.reshape(1, -1), rate, self.enhancer_sample_rate).unsqueeze(0)
+            enhanced = self._resample(enhanced.reshape(B, -1), rate, self.enhancer_sample_rate).unsqueeze(1)
         if start_frame > 0:
             enhanced = F.pad(enhanced, (int(np.round(self.enhancer_sample_rate * real_silence_front)), 0))
         return enhanced, self.enhancer_sample_rate

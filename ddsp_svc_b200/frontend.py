@@ -36,8 +36,31 @@ def volume_mask(volume, threshold_db=-60.0):
     volume = volume.contiguous()
     B, nF = volume.shape
     out = torch.empty_like(volume)
-    thr = float(np.float32(10 ** (float(threshold_db) / 20)))
+    thr = mask_threshold(threshold_db)
     _lib.check(_lib.lib().b2d_volume_mask(volume.data_ptr(), B, nF, thr, out.data_ptr(), _stream()), "b2d_volume_mask")
+    _count(1)
+    return out
+
+
+def mask_threshold(threshold_db):
+    """the linear threshold volume_mask compares with: float32(10 ** (dB / 20))"""
+    return float(np.float32(10 ** (float(threshold_db) / 20)))
+
+
+def volume_mask_rows(volume, thresholds):
+    """volume_mask with row b's linear threshold read from thresholds [B] (CUDA fp32, mask_threshold of each row's dB)
+    when the kernel runs (b2d_volume_mask_rows)."""
+    _need_cuda_f32("volume", volume)
+    _need_cuda_f32("thresholds", thresholds)
+    if volume.dim() != 2:
+        raise ValueError("volume must be [B, n_frames]")
+    volume = volume.contiguous()
+    B, nF = volume.shape
+    if thresholds.dim() != 1 or thresholds.numel() != B or not thresholds.is_contiguous():
+        raise ValueError("thresholds must be a contiguous [%d] tensor, got %s" % (B, tuple(thresholds.shape)))
+    out = torch.empty_like(volume)
+    _lib.check(_lib.lib().b2d_volume_mask_rows(volume.data_ptr(), B, nF, thresholds.data_ptr(), out.data_ptr(),
+                                               _stream()), "b2d_volume_mask_rows")
     _count(1)
     return out
 

@@ -1190,3 +1190,73 @@ def rt_crossfade(x, shift, search, buf, fade_in, fade_out, block, phase_vocoder=
                                   ws.data_ptr(), nbytes, _stream()), "b2d_rt_crossfade")
     _count(2 if phase_vocoder else 1)
     return out, next_buf
+
+
+def _need_rows(name, t, rows=None, n=None):
+    _need_cuda_f32(name, t)
+    if t.dim() != 2 or t.stride(1) != 1 or (rows is not None and t.shape[0] != rows) or (n is not None and t.shape[1] < n):
+        raise ValueError("%s must be [%s, %s] with unit stride along the samples, got %s"
+                         % (name, "rows" if rows is None else rows, "n" if n is None else ">= %d" % n, tuple(t.shape)))
+
+
+def rt_f0_regrid_batch(src, src_step, n_dst, dst_step, src_div=1.0, src_scale=1.0, rmvpe=False, pad=0, f0_min=0.0,
+                       post_scale=None):
+    """rt_f0_regrid of every row of src [N, n] -> [N, n_dst] in one launch (b2d_rt_f0_regrid_batch); with rmvpe=True,
+    row i's pitch factor is post_scale[i] (a CUDA fp32 [N] tensor, read when the kernel runs)."""
+    _contig("src", src)
+    if src.dim() != 2:
+        raise ValueError("src must be [N, n_src], got %s" % (tuple(src.shape),))
+    rows, n_src = src.shape
+    if rmvpe:
+        _need_vector("post_scale", post_scale, rows)
+    L = _lib.lib()
+    out = torch.empty(rows, int(n_dst), dtype=torch.float32, device=src.device)
+    nbytes = rows * L.b2d_rt_f0_regrid_workspace_bytes(n_src, int(n_dst))
+    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=src.device)
+    _lib.check(L.b2d_rt_f0_regrid_batch(src.data_ptr(), rows, n_src, float(src_step), float(src_div), float(src_scale),
+                                        int(n_dst), int(pad), float(dst_step), 1 if rmvpe else 0, float(f0_min),
+                                        post_scale.data_ptr() if rmvpe else None, out.data_ptr(), ws.data_ptr(), nbytes,
+                                        _stream()), "b2d_rt_f0_regrid_batch")
+    _count(1)
+    return out
+
+
+def rt_sola_batch(x, buf, search):
+    """rt_sola of every row: x [N, >= crossfade + search] (any row stride), buf [N, crossfade] -> int32 [N] on the device
+    (b2d_rt_sola_batch)"""
+    _contig("buf", buf)
+    if buf.dim() != 2:
+        raise ValueError("buf must be [N, crossfade], got %s" % (tuple(buf.shape),))
+    rows, cf = buf.shape
+    _need_rows("x", x, rows, cf + int(search))
+    shift = torch.empty(rows, dtype=torch.int32, device=x.device)
+    _lib.check(_lib.lib().b2d_rt_sola_batch(x.data_ptr(), x.stride(0), buf.data_ptr(), rows, cf, int(search),
+                                            shift.data_ptr(), _stream()), "b2d_rt_sola_batch")
+    _count(1)
+    return shift
+
+
+def rt_crossfade_batch(x, shift, search, buf, fade_in, fade_out, block, phase_vocoder=False):
+    """rt_crossfade of every row at its shift (int32 [N]): x [N, >= search + block + crossfade] (any row stride), buf
+    [N, crossfade] -> (out [N, block], next_buf [N, crossfade]) (b2d_rt_crossfade_batch)"""
+    _contig("buf", buf)
+    if buf.dim() != 2:
+        raise ValueError("buf must be [N, crossfade], got %s" % (tuple(buf.shape),))
+    rows, cf = buf.shape
+    _need_vector("fade_in", fade_in, cf)
+    _need_vector("fade_out", fade_out, cf)
+    _need_rows("x", x, rows, int(search) + int(block) + cf)
+    _need_cuda_f32("shift", shift, torch.int32)
+    if shift.dim() != 1 or shift.numel() != rows or not shift.is_contiguous():
+        raise ValueError("shift must be a contiguous [%d] int32 tensor, got %s" % (rows, tuple(shift.shape)))
+    L = _lib.lib()
+    out = torch.empty(rows, int(block), dtype=torch.float32, device=x.device)
+    next_buf = torch.empty(rows, cf, dtype=torch.float32, device=x.device)
+    nbytes = rows * L.b2d_rt_crossfade_workspace_bytes(cf, int(bool(phase_vocoder)))
+    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=x.device)
+    _lib.check(L.b2d_rt_crossfade_batch(x.data_ptr(), x.stride(0), shift.data_ptr(), buf.data_ptr(), rows,
+                                        fade_in.data_ptr(), fade_out.data_ptr(), int(block), cf,
+                                        int(bool(phase_vocoder)), out.data_ptr(), next_buf.data_ptr(), ws.data_ptr(),
+                                        nbytes, _stream()), "b2d_rt_crossfade_batch")
+    _count(2 if phase_vocoder else 1)
+    return out, next_buf

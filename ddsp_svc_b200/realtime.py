@@ -34,6 +34,9 @@ input crop, NSF-HiFiGAN) -> mask multiply -> resampling -> rt_sola -> rt_crossfa
 (the DDSP noise, the sampler's start, DDPM's per-step noise, SineGen's rand_ini and noise) are static buffers filled by
 torch's CUDA generator, and GaussianDiffusion keeps its step rows and coefficients after the warm-up.
 
+``BatchedRealtimeVC(model_path, sessions, ...)`` is gui.py's block for N independent sessions on one model, one RMVPE
+and one units encoder: rows of one batch, the same two graphs replayed for all of them (see its docstring).
+
 The sessions share ``_Session``: the ring buffer, the upload and the owned stream, capture with a warm-up and a state
 restore, the f0 / volume / mask / units front half, the resampling -> SOLA -> crossfade -> pinned-copy tail and
 SineGen's draws.  ``reflow_frames`` and ``diff_frames`` are the reflow and diffusion blocks' frame bookkeeping as pure
@@ -51,6 +54,7 @@ from .enhancer import Enhancer, adaptive_rate, auto_key
 from .hubert import Units_Encoder
 from .reflow_vocoder import load_model_vocoder
 from .rmvpe import RMVPE, Resampler, resampled_length
+from .unit2control import spk_mix_embedding
 
 # the largest f0 RMVPE decodes (cents 20 * 359 + 1997.38 above 10 Hz): bounds the keys 'auto' can pick
 RMVPE_F0_MAX = 10 * 2 ** ((20 * 359 + 1997.3794084376191) / 1200)
@@ -175,10 +179,18 @@ class _Session:
         """the f0 / volume / mask / units half (models, frames, ring and staging buffers) and the SOLA state; ``data``:
         the checkpoint config's data section"""
         dev = self.device
-        self.f0_min = float(f0_min)
         self.pitch_adjust = float(pitch_adjust)
         self.pitch_factor = 2 ** (self.pitch_adjust / 12)
         self.threhold = float(threhold)
+        self._init_models(data, f0_min, rmvpe_ckpt, who)
+        self.spk_id = torch.LongTensor(np.array([[spk_id]])).to(dev)
+        self.spk_mix_dict = spk_mix_dict if use_spk_mix else None
+        self._init_state(())
+
+    def _init_models(self, data, f0_min, rmvpe_ckpt, who):
+        """the front half's models and frame bookkeeping, the crossfade windows and the session's stream"""
+        dev = self.device
+        self.f0_min = float(f0_min)
         self.model_sr, self.block_size = int(data.sampling_rate), int(data.block_size)
         self.hop = model_hop(self.sr, self.model_sr, self.block_size, who)
         self.units_encoder = units_encoder(data, dev)
@@ -187,16 +199,18 @@ class _Session:
         self.n_frames = self.n_in // self.hop + 1
         self.start_frame = int(self.silence_front * self.sr / self.hop)
         self.trim = int(np.round(self.start_frame * self.hop / self.sr * self.sr))
-        self.spk_id = torch.LongTensor(np.array([[spk_id]])).to(dev)
-        self.spk_mix_dict = spk_mix_dict if use_spk_mix else None
-        self.ring = torch.zeros(self.n_in, device=dev)
-        self.new_block = torch.zeros(self.block, device=dev)
-        self.sola_buffer = torch.zeros(self.cf, device=dev)
         self.fade_in = torch.sin(np.pi * torch.arange(0, 1, 1 / self.cf, device=dev) / 2) ** 2
         self.fade_out = 1 - self.fade_in
-        self.in_host = torch.zeros(self.block, dtype=torch.float32).pin_memory()
-        self.out_host = torch.zeros(self.block, dtype=torch.float32).pin_memory()
         self.stream = torch.cuda.Stream(device=dev)
+
+    def _init_state(self, rows):
+        """the ring buffer, the staging buffers and the SOLA buffer, with leading dimensions ``rows``"""
+        dev = self.device
+        self.ring = torch.zeros(*rows, self.n_in, device=dev)
+        self.new_block = torch.zeros(*rows, self.block, device=dev)
+        self.sola_buffer = torch.zeros(*rows, self.cf, device=dev)
+        self.in_host = torch.zeros(*rows, self.block, dtype=torch.float32).pin_memory()
+        self.out_host = torch.zeros(*rows, self.block, dtype=torch.float32).pin_memory()
 
     @staticmethod
     def _draw_sinegen(rand_ini, noise):
@@ -382,6 +396,215 @@ class RealtimeVC(_Session):
         self.run_a()
         self.run_b(self.pick_key())
         return self._output()
+
+
+# a session's settings in BatchedRealtimeVC and their defaults (RealtimeVC's)
+SESSION_DEFAULTS = dict(spk_id=1, pitch_adjust=0.0, threhold=-45, use_spk_mix=False, spk_mix_dict=None)
+
+
+def session_settings(settings, base=None):
+    """one session's settings dict over ``base`` (default SESSION_DEFAULTS) -> the complete dict; unknown keys raise"""
+    unknown = set(settings) - set(SESSION_DEFAULTS)
+    if unknown:
+        raise ValueError("unknown session settings %s; a session sets %s"
+                         % (sorted(unknown), ", ".join(sorted(SESSION_DEFAULTS))))
+    out = dict(SESSION_DEFAULTS if base is None else base)
+    out.update(settings)
+    if out["use_spk_mix"] and not out["spk_mix_dict"]:
+        raise ValueError("use_spk_mix needs a non-empty spk_mix_dict")
+    return out
+
+
+def session_rows(sessions):
+    """complete session settings -> the per-row values the block's kernels read, at the precision of the
+    single-session kernels' scalar arguments: pitch factor 2^(pitch_adjust / 12) and linear threshold
+    10^(threhold / 20) as float32 [N], speaker ids int64 [N], and each row's mix dict (None without use_spk_mix)"""
+    return dict(pitch_factor=np.array([2 ** (float(c["pitch_adjust"]) / 12) for c in sessions], np.float32),
+                threshold=np.array([frontend.mask_threshold(c["threhold"]) for c in sessions], np.float32),
+                spk_id=np.array([int(c["spk_id"]) for c in sessions], np.int64),
+                spk_mix=[c["spk_mix_dict"] if c["use_spk_mix"] else None for c in sessions])
+
+
+class BatchedRealtimeVC(_Session):
+    """gui.py's block for N independent sessions on one model, one RMVPE and one units encoder, replayed as two CUDA
+    graphs for all of them.  ``sessions``: N dicts of the per-session settings (spk_id, pitch_adjust, threhold,
+    use_spk_mix, spk_mix_dict; absent ones take RealtimeVC's defaults).  Everything else fixes shapes or graphs and is
+    shared: the model, the rates and lengths, the enhancer and its numeric key, the phase vocoder.
+
+    - graph A: ring [N, n_in] -> RMVPE.infer_batch -> rt_f0_regrid_batch (row i's pitch factor from a device array) ->
+      volume -> volume_mask_rows (row i's threshold from a device array) -> Units_Encoder.encode_batch -> synthesizer
+      with one speaker embedding row per session (spk_embed[spk_id - 1], or the session's mix) -> mask multiply;
+    - graph B: enhancer on [N, T] -> resampling -> rt_sola_batch -> rt_crossfade_batch -> one pinned copy [N, block].
+
+    ``process(indata [N, frames(, channels)]) -> [N, frames, 2]``: one host-to-device copy, the two replays and one
+    synchronise.  ``update(i, **settings)`` changes session i's settings between blocks and ``reset(i)`` clears its
+    ring and SOLA rows; both write device arrays on the session's stream and never recapture.  Row i's output depends
+    only on row i's input, settings and draws."""
+
+    def __init__(self, model_path, sessions, samplerate=44100, block_time=0.3, crossfade_time=0.04, extra_time=2.0,
+                 f0_min=50, f0_max=1100, use_enhancer=True, enhancer_adaptive_key=0, use_phase_vocoder=False,
+                 graph=True, rmvpe_ckpt="pretrain/rmvpe/model.pt", device=None):
+        if enhancer_adaptive_key == "auto":
+            raise ValueError("BatchedRealtimeVC needs a numeric enhancer_adaptive_key: 'auto' picks a key, and so an "
+                             "enhancer sample rate, from each block's f0, and each session would need its own rate")
+        key = float(enhancer_adaptive_key)
+        self.settings = [session_settings(c) for c in sessions]
+        self.n = len(self.settings)
+        if self.n == 0:
+            raise ValueError("BatchedRealtimeVC needs at least one session")
+        self._init_block(samplerate, block_time, crossfade_time, extra_time, device, "BatchedRealtimeVC")
+        self.f0_max = float(f0_max)
+        self.use_enhancer, self.key = bool(use_enhancer), key
+        self.use_pv, self.graph = bool(use_phase_vocoder), bool(graph)
+
+        self.model, self.args = load_model(model_path, device=self.device)
+        self._init_models(self.args.data, f0_min, rmvpe_ckpt, "BatchedRealtimeVC")
+        self._init_state((self.n,))
+        self.enhancer = Enhancer(self.args.enhancer.type, self.args.enhancer.ckpt, self.device) if use_enhancer else None
+        self.out_sr = self.enhancer.enhancer_sample_rate if use_enhancer else self.model_sr
+
+        dev, N = self.device, self.n
+        rows = session_rows(self.settings)
+        self.pitch_factor = torch.from_numpy(rows["pitch_factor"]).to(dev)
+        self.threshold = torch.from_numpy(rows["threshold"]).to(dev)
+        self.spk_id = torch.from_numpy(rows["spk_id"]).reshape(N, 1).to(dev)
+        u2c = self.model.unit2ctrl
+        self.spk_weight = u2c.spk_embed.weight if u2c.n_spk is not None and u2c.n_spk > 1 else None
+        self.spk_embed = None
+        self.stream.wait_stream(torch.cuda.current_stream(dev))       # _write_speaker writes on the session's stream
+        if self.spk_weight is not None:
+            self.spk_embed = torch.zeros(N, self.spk_weight.shape[1], device=dev)
+            for i in range(N):
+                self._write_speaker(i)
+        self.noise = torch.zeros(N, self.n_frames * self.block_size, device=dev)
+        self.noise_normal = self.args.model.type == "CombSubSuperFast"
+        if use_enhancer:
+            ehop = self.enhancer.enhancer_hop_size
+            rate = adaptive_rate(self.enhancer.enhancer_sample_rate, key)[0]
+            n_mel = int(self.noise.shape[1] * rate / self.model_sr) // ehop + 4
+            self.gen_rand_ini = torch.zeros(1, 1, SINEGEN_DIM, device=dev)
+            self.gen_noise = torch.zeros(N, n_mel * ehop, SINEGEN_DIM, device=dev)
+            self.enhancer.prepare(self.model_sr, [key])
+        self.graph_a = self.graph_b = None
+        self.stream.synchronize()
+
+    _draw_noise = RealtimeVC._draw_noise
+    _draw_enhancer_noise = RealtimeVC._draw_enhancer_noise
+
+    # ---- per-session settings ---------------------------------------------------------------------------------------
+    def _write_speaker(self, i):
+        """session i's speaker embedding row from its settings, on the session's stream"""
+        c = self.settings[i]
+        with torch.no_grad(), torch.cuda.stream(self.stream):
+            self.spk_id[i].fill_(int(c["spk_id"]))
+            if self.spk_embed is None:
+                return
+            if c["use_spk_mix"]:
+                row = spk_mix_embedding(self.spk_weight, c["spk_mix_dict"])
+            else:
+                row = self.spk_weight.index_select(0, self.spk_id[i] - 1)[0]
+            self.spk_embed[i].copy_(row)
+
+    def _check_row(self, i):
+        if not (isinstance(i, (int, np.integer)) and 0 <= i < self.n):
+            raise IndexError("session index %r outside [0, %d)" % (i, self.n))
+
+    def update(self, i, **settings):
+        """change session i's spk_id, pitch_adjust, threhold, use_spk_mix or spk_mix_dict from the next block on"""
+        self._check_row(i)
+        c = session_settings(settings, self.settings[i])
+        self.settings[i] = c
+        row = session_rows([c])
+        with torch.cuda.stream(self.stream):
+            self.pitch_factor[i].fill_(float(row["pitch_factor"][0]))
+            self.threshold[i].fill_(float(row["threshold"][0]))
+        self._write_speaker(i)
+
+    def reset(self, i):
+        """zero session i's ring row and SOLA row: the slot starts over as a new voice"""
+        self._check_row(i)
+        with torch.cuda.stream(self.stream):
+            self.ring[i].zero_()
+            self.sola_buffer[i].zero_()
+
+    # ---- the two halves of the block --------------------------------------------------------------------------------
+    def _stage_a(self):
+        """ring buffer -> (masked synthesizer output [N, T], f0 [N, n_frames, 1])"""
+        self.ring.copy_(torch.cat([self.ring[:, self.block:], self.new_block], 1))
+        audio = self.ring
+        f0_10ms = self.rmvpe.infer_batch(audio[:, self.trim:], self.sr)
+        f0 = ops.rt_f0_regrid_batch(f0_10ms.contiguous(), 0.01, self.n_frames, self.hop / self.sr, rmvpe=True,
+                                    pad=self.start_frame, f0_min=self.f0_min, post_scale=self.pitch_factor)[:, :, None]
+        volume = frontend.volume_extract(audio, self.hop)
+        mask = frontend.volume_mask_rows(volume, self.threshold)
+        units = self.units_encoder.encode_batch(audio, self.sr, self.hop)
+        self._draw_noise()
+        with torch.no_grad():
+            out, _, _ = self.model(units, f0, volume[..., None], spk_id=self.spk_id, spk_mix_dict=self.spk_embed,
+                                   noise=self.noise)
+        out = frontend.mask_apply_(out.contiguous(), mask, self.block_size)
+        return out, f0
+
+    def _stage_b(self, out, f0):
+        """synthesizer output -> the N blocks in the pinned output buffer; the SOLA buffers advanced"""
+        if self.use_enhancer:
+            self._draw_enhancer_noise()
+            out, _ = self.enhancer.enhance(out, self.model_sr, f0, self.block_size, adaptive_key=self.key,
+                                           silence_front=self.silence_front, rand_ini=self.gen_rand_ini,
+                                           noise=self.gen_noise)
+        audio = out.reshape(self.n, -1)
+        if self.out_sr != self.sr:
+            audio = self.to_device_rate(audio.contiguous(), self.out_sr)
+        end = audio.shape[1] - self.delay
+        temp = audio[:, end - self.block - self.cf - self.search:end]
+        self.shift = ops.rt_sola_batch(temp, self.sola_buffer, self.search)
+        block_out, nxt = ops.rt_crossfade_batch(temp, self.shift, self.search, self.sola_buffer, self.fade_in,
+                                                self.fade_out, self.block, self.use_pv)
+        self.sola_buffer.copy_(nxt)
+        self.out_host.copy_(block_out, non_blocking=True)
+
+    # ---- one callback -----------------------------------------------------------------------------------------------
+    def upload(self, indata):
+        """the N new blocks (each mono as librosa.to_mono averages channels) into the device staging buffer"""
+        x = np.asarray(indata, dtype=np.float32)
+        if x.ndim == 3:
+            x = x.mean(axis=2, dtype=np.float32) if x.shape[2] > 1 else x[:, :, 0]
+        if x.ndim != 2 or x.shape != (self.n, self.block):
+            raise ValueError("indata must be [%d sessions, %d frames(, channels)], got %s"
+                             % (self.n, self.block, np.shape(indata)))
+        self.in_host.numpy()[:] = x
+        with torch.cuda.stream(self.stream):
+            self.new_block.copy_(self.in_host, non_blocking=True)
+
+    def run_a(self):
+        """enqueue graph A (or its eager code) on the session's stream"""
+        if not self.graph:
+            with torch.cuda.stream(self.stream):
+                self._a = self._stage_a()
+        else:
+            if self.graph_a is None:
+                self.graph_a, self._a = self._capture(self._stage_a, [self.ring])
+            with torch.cuda.stream(self.stream):
+                self.graph_a.replay()
+
+    def run_b(self):
+        """enqueue graph B (or its eager code) on the session's stream"""
+        if not self.graph:
+            with torch.cuda.stream(self.stream):
+                self._stage_b(*self._a)
+            return
+        if self.graph_b is None:
+            self.graph_b, _ = self._capture(lambda: self._stage_b(*self._a), [self.sola_buffer])
+        with torch.cuda.stream(self.stream):
+            self.graph_b.replay()
+
+    def process(self, indata):
+        """one callback for every session: indata [N, frames] or [N, frames, channels] -> outdata [N, frames, 2]"""
+        self.upload(indata)
+        self.run_a()
+        self.run_b()
+        self.stream.synchronize()
+        return np.repeat(self.out_host.numpy()[:, :, None], 2, axis=2)
 
 
 class RealtimeReflowVC(_Session):

@@ -21,6 +21,10 @@ an active dropout) plus the saved activations, and whose backward walks the laye
 csrc/unit2control_bwd.cu and csrc/pcmer_bwd.cu and library GEMMs.  The inputs are data: units, f0, phase, volume or
 aug_shift that require grad, and spk_mix_dict under grad, raise NotImplementedError.  With ``pcmer_backward`` off (the
 default) the PCmer decoder's outputs are detached in every mode.
+
+Speakers: ``spk_id`` [B, 1] (or one id for the batch), ``spk_mix_dict`` a {speaker id: weight} mix for the batch, or,
+for inference, a contiguous [B, 256] CUDA tensor of per-utterance embedding rows (spk_embed rows and
+``spk_mix_embedding`` mixes: what realtime.BatchedRealtimeVC serves many sessions with).
 """
 import math
 
@@ -32,6 +36,12 @@ from torch.nn.utils import weight_norm
 
 from . import _lib
 from .ops import _count, _need_cuda_f32, _stream
+
+
+def spk_mix_embedding(weight, spk_mix_dict):
+    """the speaker embedding of a {speaker id (from 1): weight} mix: the rows of ``weight`` (spk_embed.weight) summed
+    with their weights in fp32, in the dict's order"""
+    return sum(float(v) * weight[int(k) - 1] for k, v in spk_mix_dict.items())
 
 
 def split_to_dict(tensor, tensor_splits):
@@ -590,8 +600,15 @@ class Unit2Control(nn.Module):
         if save is not None:
             save["layers"], save["attn"] = [], []
         if self.n_spk is not None and self.n_spk > 1:
-            if spk_mix_dict is not None:
-                spk = sum(float(v) * self.spk_embed.weight[int(k) - 1] for k, v in spk_mix_dict.items()).reshape(1, 256).contiguous()
+            if torch.is_tensor(spk_mix_dict):                       # one embedding row per utterance
+                spk = spk_mix_dict
+                _need_cuda_f32("spk_mix_dict", spk)
+                if spk.dim() != 2 or spk.shape != (B, 256) or not spk.is_contiguous():
+                    raise ValueError("a tensor spk_mix_dict must be contiguous [B, 256] embedding rows, got %s"
+                                     % (tuple(spk.shape),))
+                spk_rows = B
+            elif spk_mix_dict is not None:
+                spk = spk_mix_embedding(self.spk_embed.weight, spk_mix_dict).reshape(1, 256).contiguous()
             else:
                 spk = self.spk_embed(spk_id.reshape(-1) - 1).reshape(-1, 256).contiguous()
                 spk_rows = spk.shape[0]

@@ -311,6 +311,12 @@ int b2d_volume_extract(const float* audio, int B, int n_samples, int hop, float*
 /* Silence mask at frame rate (main.py:211-213): mask[n] = max over frames n-4..n+4 (clamped) of (volume > threshold). */
 int b2d_volume_mask(const float* volume, int B, int n_frames, float threshold, float* mask_frames, void* stream);
 
+/* b2d_volume_mask with row b's threshold read from thresholds[b] (device, [B] fp32): one mask per independent session
+ * (realtime.BatchedRealtimeVC), a threshold changed without recapturing a graph.  Row b equals b2d_volume_mask of that
+ * row at threshold thresholds[b], bit for bit. */
+int b2d_volume_mask_rows(const float* volume, int B, int n_frames, const float* thresholds, float* mask_frames,
+                         void* stream);
+
 /* `seg_output *= upsample(mask, block)[frame_offset*block : (frame_offset+n_frames)*block]` in place (main.py:215,260;
  * upsample = ddsp/core.py:66-70: linear, last frame held).  signal [B, n_frames*block], mask_frames [B, n_mask_frames]. */
 int b2d_mask_apply(float* signal, const float* mask_frames, int B, int n_mask_frames, int frame_offset, int n_frames,
@@ -729,6 +735,26 @@ size_t b2d_rt_crossfade_workspace_bytes(int crossfade, int phase_vocoder);
 int b2d_rt_crossfade(const float* x, const int* shift, const float* buf, const float* fade_in, const float* fade_out,
                      int block, int crossfade, int phase_vocoder, float* out, float* next_buf, void* workspace,
                      size_t workspace_bytes, void* stream);
+
+/* ---- the same block for `rows` independent sessions in one launch per kernel (realtime.BatchedRealtimeVC) ----------
+ * Row r of every output depends only on row r of the inputs and equals the single-session entry point's result on that
+ * row bit for bit (the same kernels, one CTA or grid row per session).  rows >= 1.
+ * b2d_rt_f0_regrid_batch: b2d_rt_f0_regrid of src [rows, n_src] -> out [rows, n_dst]; in mode 1 row r's post_scale is
+ *   post_scale[r] (device, [rows] fp32, so a pitch change needs no recapture; required), ignored in mode 0.  workspace:
+ *   rows * b2d_rt_f0_regrid_workspace_bytes(n_src, n_dst), 16-byte aligned.
+ * b2d_rt_sola_batch: shift[r] = b2d_rt_sola of x + r x_stride (crossfade + search samples) against buf [rows, crossfade].
+ * b2d_rt_crossfade_batch: b2d_rt_crossfade of row r: x + r x_stride at shift[r], buf, out and next_buf rows r of
+ *   [rows, crossfade], [rows, block] and [rows, crossfade].  rows <= 65535 (B2D_ERR_UNSUPPORTED).  workspace:
+ *   rows * b2d_rt_crossfade_workspace_bytes(crossfade, phase_vocoder) bytes.
+ * No atomics and no host synchronisation, as above. */
+int b2d_rt_f0_regrid_batch(const float* src, int rows, int n_src, double src_step, double src_div, float src_scale,
+                           int n_dst, int pad, double dst_step, int mode, double f0_min, const float* post_scale,
+                           float* out, void* workspace, size_t workspace_bytes, void* stream);
+int b2d_rt_sola_batch(const float* x, int64_t x_stride, const float* buf, int rows, int crossfade, int search,
+                      int* shift, void* stream);
+int b2d_rt_crossfade_batch(const float* x, int64_t x_stride, const int* shift, const float* buf, int rows,
+                           const float* fade_in, const float* fade_out, int block, int crossfade, int phase_vocoder,
+                           float* out, float* next_buf, void* workspace, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }
