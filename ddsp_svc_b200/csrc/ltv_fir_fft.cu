@@ -15,9 +15,10 @@
 //     round-off of a loud channel (harmonic) never leaks into a quiet one (filtered noise);
 //   * all forward transforms of a pair (2 inputs + 1 impulse-response pair per job) run as one batch through the
 //     in-place passes below (three block barriers per batch), then all inverse transforms as a second batch;
-//   * every 1021-sample output segment is overlap-added into a 4-hop ring per job at its delay-compensated position;
-//     a hop is complete once the segment of the FOLLOWING input hop has been added and is then written exactly once
-//     (y1, y2 and mix = y1 + y2 (+ addend)) with 128-bit stores -- deterministic, no atomics.
+//   * the two output segments of a pair (P + L - 1 samples each, at their delay-compensated positions) are summed in
+//     registers over the pair's output window; its first 2P samples are then complete and written exactly once
+//     (y1, y2 and mix = y1 + y2 (+ addend)) with 128-bit stores, the L - 1 samples the next pair also reaches are
+//     carried to it -- deterministic, no atomics, no shared-memory ring.
 // 4 FFT-1024 per hop and job pair replace 2 x 2 x L x P = 1.04 M FMAs of the direct form (L = 510): ~4x fewer
 // instructions.  A CTA owns G hops (G even) of one utterance and processes the G+2 input hops that reach them (they
 // form whole pairs); white-noise input (x2 == nullptr) is the same Philox stream as in the direct-form kernels.
@@ -35,7 +36,7 @@ using namespace b2d_fft_smem;
 namespace {
 
 constexpr int kHop = 512;
-constexpr int kRing = 4 * kHop;          // power of two: slot = (t - t_lo) & (kRing - 1)
+static_assert(kHop == 4 * kThreads, "a thread loads and writes 4 samples of every hop");
 
 struct FftFirJob {
     const float* x;    // [B, T] or nullptr -> in-kernel uniform noise
@@ -206,9 +207,11 @@ __device__ __forceinline__ void ct_forward(float2* F, const float2* tw1, const f
     ct_pass3<N, NB, PK>(F, tid);
     __syncthreads();
 }
-template <int N, int NB, bool PK>
-__device__ __forceinline__ void ct_transposed(float2* F, const float2* tw1, const float2* tw2, int tid) {
+// (`after_pass3` runs between the first pass and its barrier)
+template <int N, int NB, bool PK, class AfterPass3>
+__device__ __forceinline__ void ct_transposed(float2* F, const float2* tw1, const float2* tw2, int tid, AfterPass3 after_pass3) {
     ct_pass3<N, NB, PK>(F, tid);
+    after_pass3();
     __syncthreads();
     ct_pass2<N, NB, false, PK>(F, tw2, tid);
     __syncthreads();
@@ -220,8 +223,13 @@ __device__ __forceinline__ void ct_transposed(float2* F, const float2* tw1, cons
 // so the HH buffers and a quarter of the transforms disappear: 2 NJ buffers -> 54.4 KB for N = 1024, NJ = 2 -> 4 CTAs per SM
 template <int N, int NJ, int NBANK = 0, bool SPEC = false> constexpr size_t fir_fft_smem() {
     return (size_t)(SPEC ? 2 : 3) * NJ * Plan<N>::kPad * sizeof(float2) + (size_t)(Ct<N>::kTw1 + Ct<N>::kTw2) * sizeof(float2) +
-           (size_t)NJ * kRing * sizeof(float) + (NBANK ? (size_t)5 * kBankRow * sizeof(float) : 0);
-}   // N = 1024: NJ = 2 -> 73152 B (3 CTAs per SM), NJ = 1 -> 38848 B;  N = 2048: NJ = 1 -> 69568 B, NJ = 2 -> 129984 B
+           (NBANK ? (size_t)5 * kBankRow * sizeof(float) : 0);
+}   // N = 1024: NJ = 2 -> 56768 B (4 CTAs per SM), NJ = 1 -> 30656 B;  N = 2048: NJ = 1 -> 61376 B, NJ = 2 -> 113600 B
+// __launch_bounds__ minimum: the two-job 1024-point kernels (taps or spectra) fit 4 CTAs per SM in shared memory
+// (4 x (56768 + 1024 reserved) B <= 228 KB) and hold <= 128 registers without spilling; the bank variant needs more.
+template <int N, int NJ, int NBANK> constexpr int fir_fft_min_ctas() {
+    return (N == 2048 && NJ == 2) ? 1 : (N == 1024 && NJ == 2 && NBANK == 0) ? 4 : 3;
+}
 
 // spectra of two real sequences a, c from Z = FFT(a + j c):  A[k] = (Z[k] + conj Z[N-k]) / 2,  C[k] = (Z[k] - conj Z[N-k]) / 2j
 __device__ __forceinline__ void split2(float2 zk, float2 zm, float2& A, float2& C) {
@@ -233,7 +241,7 @@ __device__ __forceinline__ void split2(float2 zk, float2 zm, float2& A, float2& 
 // NBANK: 0 = inputs from memory / Philox; 4 or 8 = job 0 is the sinusoid bank with that many bases of 16 harmonics
 // SPEC: job[j].ir holds the packed 1024-point spectra of the impulse responses instead of the taps
 template <int N, int NJ, bool PK, int NBANK = 0, bool SPEC = false>
-__global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ? 4 : 3)) ltv_fir_fft_kernel(FftFirParams p) {
+__global__ void __launch_bounds__(kThreads, fir_fft_min_ctas<N, NJ, NBANK>()) ltv_fir_fft_kernel(FftFirParams p) {
     constexpr int kN = N, kPad = Plan<N>::kPad;
     constexpr int kBins = N / 2 / kThreads;          // bins per thread (own_pos: DC .. N/2-1); Nyquist on thread 0
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -243,8 +251,7 @@ __global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ?
     float2* F = reinterpret_cast<float2*>(smem_raw);
     float2* tw1 = F + (SPEC ? 2 : 3) * NJ * kPad;
     float2* tw2 = tw1 + Ct<N>::kTw1;
-    float* ring = reinterpret_cast<float*>(tw2 + Ct<N>::kTw2);   // [NJ][kRing]
-    float* bank_act = ring + NJ * kRing;                         // BANK: [3][128] activated amplitudes of frames g, g+1, g+2
+    float* bank_act = reinterpret_cast<float*>(tw2 + Ct<N>::kTw2);   // BANK: [3][128] activated amplitudes of frames g, g+1, g+2
     float* bank_dlt = bank_act + 3 * kBankRow;                   //       [2][128] their differences
 
     const int tid = threadIdx.x;
@@ -255,7 +262,6 @@ __global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ?
     const unsigned long long utt = (unsigned long long)(p.utt_off + b);
 
     ct_twiddles<N>(tw1, tw2, tid);
-    for (int i = tid; i < NJ * kRing; i += kThreads) ring[i] = 0.f;
     auto at = [](int k) { return padi(binpos<N>(k)); };
     const auto own_bin = [&](int u) { return bin_at<N>(own_pos(tid, u)); };
 
@@ -276,6 +282,8 @@ __global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ?
     };
     // Global loads of a hop pair (input samples read from memory, impulse-response taps), issued ONE ITERATION AHEAD into
     // registers: they are in flight during the previous pair's transforms instead of stalling the head of the iteration.
+    // They land in shared memory as soon as the previous pair has freed it (stage), so the registers are not held
+    // through that pair's inverse transforms and overlap-add.
     constexpr int kTau = kN / 2 / kThreads;
     struct Prefetch { float4 xa[NJ], xb[NJ]; float ha[NJ][kTau], hb[NJ][kTau]; };
     auto fetch = [&](int g, Prefetch& q) {
@@ -303,10 +311,32 @@ __global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ?
             }
         }
     };
-    auto put_ir_pair = [&](int j, const Prefetch& q) {
-        float2* buf = F + (2 * NJ + j) * kPad;
+    // Taps go to the HH buffers.  Input samples go unchanged to the upper half of XB(j), which the transforms do not read
+    // (zero upper halves) and load_x does not write; each thread reads back only its own samples.
+    auto xstage = [&](int j, int hop) { return F + (NJ + j) * kPad + padi(kN / 2 + hop * (kHop / 2) + (tid << 1)); };
+    auto stage = [&](const Prefetch& q) {
 #pragma unroll
-        for (int u = 0; u < kTau; ++u) buf[padi(tid + u * kThreads)] = make_float2(q.ha[j][u], q.hb[j][u]);
+        for (int j = 0; j < NJ; ++j) {
+            if (!SPEC) {
+                float2* buf = F + (2 * NJ + j) * kPad;
+#pragma unroll
+                for (int u = 0; u < kTau; ++u) buf[padi(tid + u * kThreads)] = make_float2(q.ha[j][u], q.hb[j][u]);
+            }
+            if (p.job[j].x && !(NBANK && j == 0)) {
+                xstage(j, 0)[0] = make_float2(q.xa[j].x, q.xa[j].y);
+                xstage(j, 0)[1] = make_float2(q.xa[j].z, q.xa[j].w);
+                xstage(j, 1)[0] = make_float2(q.xb[j].x, q.xb[j].y);
+                xstage(j, 1)[1] = make_float2(q.xb[j].z, q.xb[j].w);
+            }
+        }
+    };
+    auto staged_x = [&](int j, int hop) {
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (p.job[j].x) {
+            const float2 lo = xstage(j, hop)[0], hi = xstage(j, hop)[1];
+            v = make_float4(lo.x, lo.y, hi.x, hi.y);
+        }
+        return v;
     };
     // x_j[gP + i] (1 + j i/P) for i < P, zeros above; `present` false -> all zeros (hop outside the chunk's reach);
     // `pre` = the hop's samples when the job reads its input from memory (prefetched), else Philox noise is drawn here
@@ -357,9 +387,8 @@ __global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ?
     };
 #endif
 
-    // spectrum of frame g per job at the bins own_bin(u); thread 0 additionally holds DC (u = 0) and Nyquist (real)
+    // spectrum of frame g per job at the bins own_bin(u); thread 0 holds the real DC and Nyquist values as (DC, Nyquist) at u = 0
     float2 Hp[NJ][kBins];
-    float HpN[NJ];
     // Input hops are always transformed in the SAME pairs (2m-1, 2m), whatever the chunking: G is even, so the first hop
     // that reaches this chunk (h0 - 1, odd) starts a pair and the last one (h1, even) ends one -- no extra work, and
     // since the partner of a pair only enters through the round-off of the shared transforms, every output sample is
@@ -379,12 +408,10 @@ __global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ?
 #pragma unroll
             for (int u = 0; u < kBins; ++u) {
                 const int k = own_bin(u);
-                const float2 h = __ldg(row + k);
-                Hp[j][u] = k == 0 ? make_float2(h.x, 0.f) : h;
-                if (k == 0) HpN[j] = h.y;
+                Hp[j][u] = __ldg(row + k);                              // row[0] = (DC, Nyquist) as well
             }
         }
-        __syncthreads();                                                // twiddles and the cleared rings
+        __syncthreads();                                                // twiddles
     } else {
 #pragma unroll
         for (int j = 0; j < NJ; ++j) load_ir_pair(j, gs - 1, gs, true);    // exactly the (h_{g+1}, h_{g+2}) pair of hops gs-2, gs-1
@@ -397,27 +424,39 @@ __global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ?
             for (int u = 0; u < kBins; ++u) {
                 const int k = own_bin(u);
                 float2 unused;
-                if (k == 0) Hp[j][u] = make_float2(H[at(0)].y, 0.f);
+                if (k == 0) Hp[j][u] = make_float2(H[at(0)].y, H[at(kN / 2)].y);
                 else split2(H[padi(own_pos(tid, u))], H[at(kN - k)], unused, Hp[j][u]);
             }
-            HpN[j] = H[at(kN / 2)].y;                                 // only thread 0 uses it
         }
         __syncthreads();
     }
 
-    // write hop h (complete) from the rings: y_j, mix; clear its ring slots
-    auto emit = [&](int h) {
-        const int slot = (((h - h0) * kHop) & (kRing - 1)) + (tid << 2);
-        const size_t o = (size_t)b * T + (size_t)h * kHop + (tid << 2);
-        float4 m = make_float4(0.f, 0.f, 0.f, 0.f);
+    // Output window of the pair that starts at input hop g: samples t = gP - A + w, w < 2P + N/2, where thread tid owns
+    // w = P c + 4 tid + e (e < 4).  A, the larger half tap count rounded up to 4, puts every job's segments at or after
+    // the window's start and keeps the 128-bit stores aligned.  Samples w < 2P are final after the pair: the next pair's
+    // segments start at (g+2)P - L/2 >= (g+2)P - A.  The rest, at most L - 1 samples per job, is the head of the next
+    // window, where the same thread owns it, so it is carried in registers.
+    constexpr int kCarry = N / 2 / kHop;              // hop-long chunks of a window carried into the next one
+    int A = p.job[0].L >> 1;
+    if (NJ == 2) A = max(A, p.job[1].L >> 1);
+    A = (A + 3) & ~3;
+    float carry[NJ][kCarry][4];
+#pragma unroll
+    for (int j = 0; j < NJ; ++j)
+#pragma unroll
+        for (int c = 0; c < kCarry; ++c)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) carry[j][c][e] = 0.f;
+
+    // write the 4 samples from t (a multiple of 4) of y_j and mix, if they belong to this CTA's hops
+    auto emit = [&](int t, const float4 (&v)[NJ]) {
+        if (t < t_lo || t >= t_hi) return;
+        const size_t o = (size_t)b * T + t;
+        float4 m = v[0];
 #pragma unroll
         for (int j = 0; j < NJ; ++j) {
-            float4* r = reinterpret_cast<float4*>(ring + j * kRing + slot);
-            const float4 v = *r;
-            *r = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (p.job[j].y) b2d::st_global_v4(p.job[j].y + o, v);
-            if (j == 0) m = v;
-            else { m.x += v.x; m.y += v.y; m.z += v.z; m.w += v.w; }
+            if (p.job[j].y) b2d::st_global_v4(p.job[j].y + o, v[j]);
+            if (j > 0) { m.x += v[j].x; m.y += v[j].y; m.z += v[j].z; m.w += v[j].w; }
         }
         if (p.mix) {
             if (p.addend) {
@@ -430,6 +469,7 @@ __global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ?
 
     Prefetch pf;
     fetch(gs, pf);
+    stage(pf);
 #pragma unroll 1
     for (int g = gs; g <= ge; g += 2) {
         const bool has_a = g >= 0, has_b = g + 1 <= nF - 1;      // properties of the utterance only, not of the chunking
@@ -462,10 +502,10 @@ __global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ?
             } else
 #endif
             {
-                load_x(j, g, has_a, pf.xa[j], F + j * kPad);
-                load_x(j, g + 1, has_b, pf.xb[j], F + (NJ + j) * kPad);
+                const float4 xa = staged_x(j, 0), xb = staged_x(j, 1);
+                load_x(j, g, has_a, xa, F + j * kPad);
+                load_x(j, g + 1, has_b, xb, F + (NJ + j) * kPad);
             }
-            if (!SPEC) put_ir_pair(j, pf);
         }
         __syncthreads();
         ct_forward<N, (SPEC ? 2 : 3) * NJ, PK, true>(F, tw1, tw2, tid);   // all have zero upper halves: pruned first pass
@@ -507,51 +547,66 @@ __global__ void __launch_bounds__(kThreads, (N == 2048 && NJ == 2) ? 1 : (SPEC ?
                 // (H_{g+1}, H_{g+2}) at DC and at Nyquist
                 const float2 z0 = SPEC ? make_float2(HaR[0].x, HbR[0].x) : HH[at(0)];
                 const float2 zN = SPEC ? make_float2(HaR[0].y, HbR[0].y) : HH[at(kN / 2)];
-                const float hp0 = Hp[j][0].x, hpN = HpN[j];
+                const float hp0 = Hp[j][0].x, hpN = Hp[j][0].y;
                 const float ya0 = fmaf(a0.y, z0.x - hp0, a0.x * hp0), yb0 = fmaf(b0.y, z0.y - z0.x, b0.x * z0.x);
                 const float yaN = fmaf(aN.y, zN.x - hpN, aN.x * hpN), ybN = fmaf(bN.y, zN.y - zN.x, bN.x * zN.x);
                 XA[at(0)] = make_float2(yb0, ya0);
                 XA[at(kN / 2)] = make_float2(ybN, yaN);
-                Hp[j][0] = make_float2(z0.y, 0.f);
-                HpN[j] = zN.y;
+                Hp[j][0] = make_float2(z0.y, zN.y);
             }
         }
         __syncthreads();
-        // the next pair's loads fly during the inverse transforms and the overlap-add (issued here, not earlier: the
-        // registers they land in would otherwise be held through the forward batch and the pointwise step)
+        // the next pair's loads fly during the first inverse pass (issued here, not earlier: the registers they land
+        // in would otherwise be held through the forward batch and the pointwise step)
         if (g + 2 <= ge) fetch(g + 2, pf);
 
-        // ---- inverse of the pairs (batch over jobs): hop g = stored .y / N, hop g+1 = stored .x / N ----
-        ct_transposed<N, NJ, PK>(F, tw1, tw2, tid);
+        // ---- inverse of the pairs (batch over jobs): hop g = stored .y / N, hop g+1 = stored .x / N.  The next pair's
+        //      loads are staged after the first pass: XB and HH are free since the pointwise step. ----
+        ct_transposed<N, NJ, PK>(F, tw1, tw2, tid, [&] { if (g + 2 <= ge) stage(pf); });
 
-        // ---- overlap-add at the delay-compensated positions t = gP - L/2 + n (hop g) and + P (hop g+1), kept to this
-        //      CTA's hops.  Slots hit twice (n and n - P) belong to the same thread: no race. ----
+        // ---- overlap-add over the pair's output window: job j's segments of hops g and g+1 start at w = d and d + P
+        //      (d = A - L/2); carried head + hop g+1 + hop g, the order in which a running sum would meet them.  The
+        //      final part is written, the tail carried. ----
 #pragma unroll
-        for (int j = 0; j < NJ; ++j) {
-            const float2* Y = F + j * kPad;
-            float* rj = ring + j * kRing;
-            const int base = g * kHop - (p.job[j].L >> 1) - t_lo;
-            // length of the linear convolution; the rest of the transform holds only round-off and must not spill into
-            // later hops (nor wrap around the ring)
-            const int nvalid = kHop + p.job[j].L - 1;
+        for (int c = 0; c < 2 + kCarry; ++c) {
+            float4 v[NJ];
 #pragma unroll
-            for (int u = 0; u < kN / kThreads; ++u) {
-                const int n = tid + u * kThreads;
-                const float2 v = Y[padi(n)];
-                const int ra = base + n, rb = ra + kHop;
-                const bool live = n < nvalid;
-                if (live && has_a && ra >= 0 && ra < t_hi - t_lo) rj[ra & (kRing - 1)] += v.y * (1.0f / kN);
-                if (live && has_b && rb >= 0 && rb < t_hi - t_lo) rj[rb & (kRing - 1)] += v.x * (1.0f / kN);
+            for (int j = 0; j < NJ; ++j) {
+                const float2* Y = F + j * kPad;
+                // length of the linear convolution; the rest of the transform holds only round-off and must not reach
+                // later samples
+                const int nvalid = kHop + p.job[j].L - 1;
+                const int n0 = kHop * c + (tid << 2) - (A - (p.job[j].L >> 1));
+                float s[4];
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int na = n0 + e, nb = na - kHop;
+                    float acc = c < kCarry ? carry[j][c < kCarry ? c : 0][e] : 0.f;
+                    // hop g+1 reaches w >= P, hop g only w < P + N/2 (L <= N/2, A <= N/4)
+                    if (c >= 1 && has_b && nb >= 0 && nb < nvalid) acc += Y[padi(nb)].x * (1.0f / kN);
+                    if (c <= kCarry && has_a && na >= 0 && na < nvalid) acc += Y[padi(na)].y * (1.0f / kN);
+                    s[e] = acc;
+                }
+                v[j] = make_float4(s[0], s[1], s[2], s[3]);
+                if (c >= 2) {
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) carry[j][c >= 2 ? c - 2 : 0][e] = s[e];
+                }
             }
+            if (c < 2) emit(g * kHop - A + kHop * c + (tid << 2), v);
         }
+        // the next iteration's loads overwrite the Y buffers read above
         __syncthreads();
-        // complete now: every hop below the last input hop just added
-        if (g - 1 >= h0 && g - 1 < h1) emit(g - 1);
-        if (has_b && g >= h0 && g < h1) emit(g);
-        // no barrier needed here: emit touches only the rings, the next iteration's loads only F (whose last reads
-        // were ordered by the barrier above), and the rings are next written after the FFT passes' barriers
     }
-    if (ge < h1) emit(ge);                        // last hop of the utterance: no following input hop
+    // the carried tail of the last window: output only where no later input hop reaches (the end of the utterance)
+    const int g_end = gs + 2 * ((ge - gs) / 2 + 1);
+#pragma unroll
+    for (int c = 0; c < kCarry; ++c) {
+        float4 v[NJ];
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) v[j] = make_float4(carry[j][c][0], carry[j][c][1], carry[j][c][2], carry[j][c][3]);
+        emit(g_end * kHop - A + kHop * c + (tid << 2), v);
+    }
 }
 
 // ---- impulse responses -> packed N-point spectra, once per frame (the SPEC variant of the FIR kernel reads them) ----
@@ -625,8 +680,9 @@ bool ltv_fir_fft_supported(int P, int taps1, int taps2, int njobs) {
 }
 
 // Hops per CTA, G (even).  A CTA walks its G + 2 input hops serially, so a launch takes about
-// (waves of CTAs at the kernel's occupancy) x (G + 2) hop times: G = 32 on B = 32 x 10 s gives 864 CTAs for 396 resident
-// slots, 2.18 waves, and the third wave runs 18 % full.  Pick the G that minimises that product (the largest on a tie:
+// (waves of CTAs at the kernel's occupancy) x (G + 2) hop times.  On B = 32 x 10 s (nF = 861) at 4 CTAs per SM (528
+// slots on 132 SMs) that is G = 54: 512 CTAs in one wave, 56 hop times (at 3 CTAs per SM: G = 36, 768 CTAs in two
+// waves of 396, 76 hop times).  Pick the G that minimises that product (the largest on a tie:
 // least recomputation); it also shrinks G for small launches -- one utterance of a real-time caller, one chunk of the
 // host pipeline -- until they spread over the GPU.  The output does not depend on G (hops are always paired the same way).
 // `occ` caches the occupancy per device: the query costs host time that a small (real-time) launch would notice.
