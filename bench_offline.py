@@ -1,6 +1,6 @@
 """Whole-file conversion time of main.py's loop: 60 s of 44.1 kHz synthetic speech with pauses, converted by a
 CombSubSuperFast model with the NSF-HiFiGAN enhancer (key 0, adaptive key 0; synthetic seeded checkpoints of
-bench_realtime.write_synthetic, written to a temporary directory).
+conversion_fixtures.write_synthetic, written to a temporary directory).
 
 Two arms on the same modules and the same split, alternated, each timed from the call to the end of a device
 synchronise; medians over --steps calls after --warmup calls of each:
@@ -34,7 +34,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=1)
     a = ap.parse_args()
     assert torch.cuda.is_available(), "bench_offline.py needs a CUDA device"
-    from bench_realtime import write_synthetic
+    from conversion_fixtures import write_synthetic
     from ddsp_svc_b200.offline import OfflineVC
     from tests import offline_oracle as oo
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,

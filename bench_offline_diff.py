@@ -1,8 +1,8 @@
 """Whole-file conversion time of main_diff.py's loop and batch_infer.py's infer(): 60 s of 44.1 kHz synthetic speech
 with pauses, converted by a 'DiffusionNew' model at configs/diffusion-new.yaml's sizes (CombSubFast and WaveNet(128, 20,
 512, 256), its built-in DDSP model; ContentVec units at layer 12, RMVPE, NSF-HiFiGAN) with DPM-Solver at speedup 10 and
-k_step 100 (key 0, formant key 0; synthetic seeded checkpoints of bench_realtime_diff.write_synthetic_diff, written to a
-temporary directory).
+k_step 100 (key 0, formant key 0; synthetic seeded checkpoints of conversion_fixtures.write_synthetic_diff,
+written to a temporary directory).
 
 Four arms on the same modules, alternated, each timed from the call to the end of a device synchronise; medians over
 --steps calls after --warmup calls of each:
@@ -37,7 +37,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=1)
     a = ap.parse_args()
     assert torch.cuda.is_available(), "bench_offline_diff.py needs a CUDA device"
-    from bench_realtime_diff import write_synthetic_diff
+    from conversion_fixtures import write_synthetic_diff
     from ddsp_svc_b200.offline import OfflineDiffVC
     from tests import offline_diff_oracle as odo
     from tests import offline_oracle as oo

@@ -1,6 +1,6 @@
 """Block time of gui.py's real-time callback for N independent sessions on one card, N in --sessions (default 1, 4,
 16, 64), at the GUI defaults (44.1 kHz, block 0.3 s, crossfade 0.04 s, extra 2.0 s, enhancer on, key 0) with a synthetic
-seeded Sins checkpoint (bench_realtime.write_synthetic, in a temporary directory).
+seeded Sins checkpoint (conversion_fixtures.write_synthetic, in a temporary directory).
 
 Three arms, alternated block by block, each timed with CUDA events from before the first upload to after the last output
 copy (the device's span of one block for all N sessions):
@@ -61,7 +61,7 @@ def main():
     ap.add_argument("--model", default="Sins")
     a = ap.parse_args()
     assert torch.cuda.is_available(), "bench_realtime_batch.py needs a CUDA device"
-    from bench_realtime import write_synthetic
+    from conversion_fixtures import write_synthetic
     from ddsp_svc_b200.realtime import BatchedRealtimeVC, RealtimeVC
     gpu = card()
     rng = np.random.default_rng(0)

@@ -25,16 +25,13 @@ import time
 
 import numpy as np
 import torch
-import yaml
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-from bench_realtime import MODELS, GuiBlock  # noqa: E402
-from bench_realtime_reflow import HIFIGAN, write_front  # noqa: E402
+# DDSP_MODELS is not used here: it stays importable from this script, with the writer whose ``ddsp`` keys it holds
+from conversion_fixtures import DDSP_MODELS, GuiDiffBlock, write_synthetic_diff  # noqa: E402,F401
 
-DDSP_MODELS = dict(MODELS, CombSub={"type": "CombSub", "n_mag_allpass": 256, "n_mag_harmonic": 512,
-                                    "n_mag_noise": 256, "n_spk": 2})
 SETTINGS = {
     "ddim": dict(model="DiffusionNew", diff_method="ddim"),
     "dpm": dict(model="DiffusionNew", diff_method="dpm-solver"),
@@ -42,58 +39,6 @@ SETTINGS = {
     "unit2mel_combsub_ddim": dict(model="Diffusion", ddsp="CombSub", diff_method="ddim"),
 }
 STAGES = ("front", "ddsp", "diffusion", "vocoder", "tail")
-
-
-def write_synthetic_diff(d, model_type="DiffusionNew", n_chans=512, n_layers=20, encoder="contentvec768l12", n_spk=2,
-                         ddsp=None, k_step_max=100):
-    """seeded checkpoints of a diffusion session in directory d -> (DDSP model path or None, diffusion model path, rmvpe
-    path).  model_type: 'Diffusion', 'DiffusionNew' or 'DiffusionFast'; the denoiser's parameters are all non-zero
-    (tests/reflow_oracle.seeded_weights; the default init zeroes WaveNet's output projection); ``ddsp``: a key of
-    DDSP_MODELS for a DDSP checkpoint with the same data section"""
-    from ddsp_svc_b200 import diffusion_vocoder, dropin
-    from tests import reflow_oracle
-    torch.manual_seed(0)
-    data, voc = write_front(d, encoder)
-    model = {"type": model_type, "n_layers": n_layers, "n_chans": n_chans, "n_hidden": 256, "win_length": 2048,
-             "k_step_max": k_step_max, "use_pitch_aug": True, "n_spk": n_spk}
-    cfg = dropin.DotDict({"data": data, "model": model, "vocoder": voc})
-    os.makedirs(os.path.join(d, "diff"), exist_ok=True)
-    with open(os.path.join(d, "diff", "config.yaml"), "w") as f:
-        yaml.safe_dump(dict(cfg), f)
-    net = diffusion_vocoder.build_model(cfg, HIFIGAN["num_mels"])
-    denoiser = (net.decoder if model_type == "Diffusion" else net.diff_model).denoise_fn
-    reflow_oracle.seeded_weights(denoiser, 7, gain=0.5)
-    torch.save({"model": net.state_dict()}, os.path.join(d, "diff", "model.pt"))
-    ddsp_path = None
-    if ddsp is not None:
-        os.makedirs(os.path.join(d, "ddsp"), exist_ok=True)
-        dcfg = {"data": data, "model": DDSP_MODELS[ddsp]}
-        with open(os.path.join(d, "ddsp", "config.yaml"), "w") as f:
-            yaml.safe_dump(dcfg, f)
-        ddsp_path = os.path.join(d, "ddsp", "model.pt")
-        torch.save({"model": dropin.build_model(dropin.DotDict(dcfg)).state_dict()}, ddsp_path)
-    return ddsp_path, os.path.join(d, "diff", "model.pt"), os.path.join(d, "rmvpe.pt")
-
-
-class GuiDiffBlock(GuiBlock):
-    """gui_diff.py's audio_callback and SvcDDSP.infer in their own order on a RealtimeDiffVC's modules and draws (the
-    session's static buffers, which hold its last draws), with host numpy and eager torch in between"""
-
-    def __call__(self, indata):
-        s = self.s
-        f0, volume, mask, units = self.front(indata)
-        volume = volume[..., None]
-        with torch.no_grad():
-            if s.ddsp_model is None:
-                output = None
-            else:
-                output, _, _ = s.ddsp_model(units, f0, volume, spk_id=s.spk_id, spk_mix_dict=s.spk_mix_dict,
-                                            noise=s.ext_noise)
-            output = s.diff.infer(output, f0, units, volume, acc=s.diff_acc, spk_id=s.spk_id, k_step=s.k_step,
-                                  method=s.diff_method, silence_front=s.silence_front, use_silence=s.diff_silence,
-                                  spk_mix_dict=s.spk_mix_dict, **s.draws())
-            output *= mask
-        return self.tail(output, s.model_sr)
 
 
 def stage_times(s, xs):

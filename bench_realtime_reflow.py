@@ -22,79 +22,14 @@ import time
 
 import numpy as np
 import torch
-import yaml
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-from bench_realtime import HIFIGAN, GuiBlock  # noqa: E402
+from conversion_fixtures import GuiReflowBlock, write_synthetic_reflow  # noqa: E402
 
 STAGES = ("rmvpe", "units", "ddsp", "mel", "sampler", "vocoder", "tail")
 SAMPLERS = {"euler20": dict(sampling_method="euler", infer_step=20), "rk4_5": dict(sampling_method="rk4", infer_step=5)}
-
-
-def write_front(d, encoder="contentvec768l12"):
-    """seeded checkpoints of what every diffusion / reflow session loads besides its model, in directory d: the units
-    encoder, RMVPE and NSF-HiFiGAN (voc/model.ckpt) -> the config's data and vocoder sections"""
-    import ddsp_svc_b200 as pkg
-    from ddsp_svc_b200 import dropin
-    from ddsp_svc_b200.hifigan import Generator
-    os.makedirs(os.path.join(d, "voc"), exist_ok=True)
-    if encoder == "hubertsoft":
-        enc_path, n_unit = os.path.join(d, "hubert.pt"), 256
-        torch.save(pkg.HubertSoft().state_dict(), enc_path)
-    else:
-        from tests import units_oracle
-        enc_path, n_unit = os.path.join(d, "contentvec.pt"), 768
-        units_oracle.save_fairseq(enc_path, units_oracle.fairseq_state_dict(0)[1], args=units_oracle.fairseq_args())
-    torch.save({"model": pkg.E2E0(4, 1, (2, 2)).state_dict()}, os.path.join(d, "rmvpe.pt"))
-    with open(os.path.join(d, "voc", "config.json"), "w") as f:
-        json.dump(HIFIGAN, f)
-    gen = Generator(dropin.DotDict(HIFIGAN))
-    torch.save({"generator": gen.state_dict()}, os.path.join(d, "voc", "model.ckpt"))
-    return ({"sampling_rate": 44100, "block_size": 512, "encoder": encoder, "encoder_ckpt": enc_path,
-             "encoder_sample_rate": 16000, "encoder_hop_size": 320, "encoder_out_channels": n_unit},
-            {"type": "nsf-hifigan", "ckpt": os.path.join(d, "voc", "model.ckpt")})
-
-
-def write_synthetic_reflow(d, n_chans=512, n_layers=6, encoder="contentvec768l12", n_spk=2, model_type="RectifiedFlow"):
-    """seeded checkpoints of a reflow session in directory d -> (model path, rmvpe path).  The velocity network's
-    parameters are all non-zero (tests/reflow_oracle.seeded_weights; the default init zeroes its output projection);
-    ``encoder``: 'contentvec768l12' (reflow.yaml) or 'hubertsoft'"""
-    import ddsp_svc_b200 as pkg
-    from tests import reflow_oracle
-    torch.manual_seed(0)
-    data, voc = write_front(d, encoder)
-    n_unit = data["encoder_out_channels"]
-    cfg = {"data": data,
-           "model": {"type": model_type, "win_length": 2048, "n_layers": n_layers, "n_chans": n_chans,
-                     "use_pitch_aug": True, "n_spk": n_spk},
-           "vocoder": voc}
-    with open(os.path.join(d, "config.yaml"), "w") as f:
-        yaml.safe_dump(cfg, f)
-    model = pkg.Unit2Wav(44100, 512, 2048, n_unit, n_spk, True, HIFIGAN["num_mels"], n_layers, n_chans)
-    reflow_oracle.seeded_weights(model.reflow_model.velocity_fn, 7)
-    torch.save({"model": model.state_dict()}, os.path.join(d, "model.pt"))
-    return os.path.join(d, "model.pt"), os.path.join(d, "rmvpe.pt")
-
-
-class GuiReflowBlock(GuiBlock):
-    """gui_reflow.py's audio_callback and SvcDDSP.infer in their own order on a RealtimeReflowVC's modules and draws
-    (the session's static buffers, which hold its last draws), with host numpy and eager torch in between.  The speaker
-    mix is the session's (gated on use_spk_mix, where gui_reflow.py:137 passes spk_mix_dict regardless)."""
-
-    def __call__(self, indata):
-        s = self.s
-        f0, volume, mask, units = self.front(indata)
-        formant_shift_key = torch.from_numpy(np.array([[float(s.formant_shift_key)]])).float().to(s.device)
-        with torch.no_grad():
-            output = s.model(units, f0, volume[..., None], spk_id=s.spk_id, spk_mix_dict=s.spk_mix_dict,
-                             aug_shift=formant_shift_key, vocoder=s.vocoder, infer=True, return_wav=True,
-                             infer_step=s.infer_step, method=s.method, t_start=s.t_start,
-                             silence_front=s.silence_front, use_tqdm=False, ddsp_noise=s.noise,
-                             reflow_noise=s.reflow_noise, rand_ini=s.gen_rand_ini, sine_noise=s.gen_noise)
-            output *= mask[:, -output.shape[-1]:]
-        return self.tail(output, s.model_sr)
 
 
 def stage_times(s, xs):

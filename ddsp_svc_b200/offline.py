@@ -39,7 +39,7 @@ import torch
 from . import diffusion_vocoder, frontend, ops
 from .dropin import load_model
 from .enhancer import Enhancer
-from .realtime import model_hop, units_encoder
+from .realtime import cuda_device, model_hop, units_encoder
 from .reflow_vocoder import load_model_vocoder
 from .rmvpe import RMVPE
 
@@ -161,12 +161,7 @@ class _Offline:
     / mask, the per-segment inputs and the assembly"""
 
     def _init_device(self, device, pitch_extractor, who):
-        if pitch_extractor != "rmvpe":
-            raise ValueError("%s extracts f0 with 'rmvpe' only: %r has no kernels" % (who, pitch_extractor))
-        self.device = torch.device("cuda" if device is None else device)
-        if self.device.type != "cuda":
-            raise ValueError("%s runs on the CUDA kernels: device must be a CUDA device" % who)
-        self.who = who
+        self.device, self.who = cuda_device(device, who, pitch_extractor), who
 
     def _init_front(self, data, rmvpe_ckpt):
         self.model_sr, self.block_size = int(data.sampling_rate), int(data.block_size)
@@ -234,6 +229,7 @@ class _Offline:
         return result
 
     def convert(self, audio, sample_rate, *args, **kwargs):
+        """the whole-file conversion: ``render``'s arguments -> (output [N_out] CUDA fp32, its sample rate)"""
         rendered, out_sr = self.render(audio, sample_rate, *args, **kwargs)
         with torch.cuda.device(self.device):
             return self.assemble(rendered, out_sr), out_sr
@@ -251,8 +247,9 @@ class OfflineVC(_Offline):
 
     def render(self, audio, sample_rate, key=0, spk_id=1, spk_mix_dict=None, f0_min=50, f0_max=1100, threhold=-60,
                enhancer_adaptive_key=0, segments=None):
-        """convert() without the assembly -> ([(start_frame, output [T])], output sample rate).  f0_max is accepted
-        for main.py's signature: RMVPE's f0 is not bounded above"""
+        """main.py's conversion without the assembly -> ([(start_frame, output [T])], output sample rate); ``convert``
+        takes the same arguments and returns the assembled output.  f0_max is accepted for main.py's signature: RMVPE's
+        f0 is not bounded above"""
         _need_audio(audio)
         sample_rate = int(sample_rate)
         out_sr = self.enhancer.enhancer_sample_rate if self.enhancer is not None else self.model_sr
@@ -268,25 +265,20 @@ class OfflineVC(_Offline):
                 rendered.append((start, out.reshape(-1)))
         return rendered, out_sr
 
-    def convert(self, audio, sample_rate, key=0, spk_id=1, spk_mix_dict=None, f0_min=50, f0_max=1100, threhold=-60,
-                enhancer_adaptive_key=0, segments=None):
-        """main.py's whole-file conversion -> (output [N_out] CUDA fp32, its sample rate)"""
-        return super().convert(audio, sample_rate, key=key, spk_id=spk_id, spk_mix_dict=spk_mix_dict, f0_min=f0_min,
-                               f0_max=f0_max, threhold=threhold, enhancer_adaptive_key=enhancer_adaptive_key,
-                               segments=segments)
+
+def _infer_setting(args, key):
+    """the config's infer.<key>, which a setting of 'auto' reads; ValueError without one"""
+    section = args.infer
+    if section is None or section.get(key) is None:
+        raise ValueError("%s='auto' needs infer.%s in the model's config" % (key, key))
+    return section.get(key)
 
 
 def reflow_settings(args, infer_step="auto", method="auto", t_start="auto"):
     """main_reflow.py's sampler settings -> (infer_step, method, t_start): 'auto' from the config's infer section and
     model.t_start (0 without one); a given t_start is raised to model.t_start.  A negative infer_step raises"""
-    def infer(key):
-        section = args.infer
-        if section is None or section.get(key) is None:
-            raise ValueError("%s='auto' needs infer.%s in the model's config" % (key, key))
-        return section.get(key)
-
-    method = infer("method") if method == "auto" else method
-    infer_step = int(infer("infer_step")) if infer_step == "auto" else int(infer_step)
+    method = _infer_setting(args, "method") if method == "auto" else method
+    infer_step = int(_infer_setting(args, "infer_step")) if infer_step == "auto" else int(infer_step)
     floor = args.model.t_start
     if t_start == "auto":
         t_start = float(floor) if floor is not None else 0.0
@@ -311,7 +303,8 @@ class OfflineReflowVC(_Offline):
 
     def render(self, audio, sample_rate, key=0, spk_id=1, spk_mix_dict=None, f0_min=50, f0_max=1100, threhold=-60,
                formant_shift_key=0, infer_step="auto", method="auto", t_start="auto", segments=None):
-        """convert() without the assembly -> ([(start_frame, output [T])], the model's sample rate)"""
+        """main_reflow.py's conversion without the assembly -> ([(start_frame, output [T])], the model's sample rate);
+        ``convert`` takes the same arguments and returns the assembled output"""
         _need_audio(audio)
         sample_rate = int(sample_rate)
         infer_step, method, t_start = reflow_settings(self.args, infer_step, method, t_start)
@@ -325,13 +318,6 @@ class OfflineReflowVC(_Offline):
                                  method=method, t_start=t_start, use_tqdm=False)
                 rendered.append((start, self._mask(out, mask, start).reshape(-1)))
         return rendered, self.model_sr
-
-    def convert(self, audio, sample_rate, key=0, spk_id=1, spk_mix_dict=None, f0_min=50, f0_max=1100, threhold=-60,
-                formant_shift_key=0, infer_step="auto", method="auto", t_start="auto", segments=None):
-        """main_reflow.py's whole-file conversion -> (output [N_out] CUDA fp32, the model's sample rate)"""
-        return super().convert(audio, sample_rate, key=key, spk_id=spk_id, spk_mix_dict=spk_mix_dict, f0_min=f0_min,
-                               f0_max=f0_max, threhold=threhold, formant_shift_key=formant_shift_key,
-                               infer_step=infer_step, method=method, t_start=t_start, segments=segments)
 
 
 DiffSettings = collections.namedtuple("DiffSettings", "mode k_step infer_speedup method diff_spk_id")
@@ -352,14 +338,8 @@ def diff_settings(args, ddsp_args, k_step=None, speedup="auto", method="auto", d
     k_step is clamped to model.k_step_max (its default when None) for 'DiffusionNew' and 'DiffusionFast' only; a
     'Diffusion' model keeps the given k_step or None.  'auto' speedup / method read infer.speedup / infer.method and
     raise ValueError without them; ``diff_spk_id`` is None for 'auto' (the DDSP model's speaker) or the given id."""
-    def infer(key):
-        section = args.infer
-        if section is None or section.get(key) is None:
-            raise ValueError("%s='auto' needs infer.%s in the model's config" % (key, key))
-        return section.get(key)
-
-    infer_speedup = infer("speedup") if speedup == "auto" else int(speedup)
-    method = infer("method") if method == "auto" else method
+    infer_speedup = _infer_setting(args, "speedup") if speedup == "auto" else int(speedup)
+    method = _infer_setting(args, "method") if method == "auto" else method
     usable = ddsp_args is not None and not diffusion_vocoder.data_mismatches(ddsp_args, args)
     kind = args.model.type
     if kind in ("DiffusionNew", "DiffusionFast"):
@@ -431,7 +411,8 @@ class OfflineDiffVC(_Offline):
 
     def render(self, audio, sample_rate, key=0, spk_id=1, spk_mix_dict=None, f0_min=50, f0_max=1100, threhold=-60,
                formant_shift_key=0, diff_spk_id="auto", speedup="auto", method="auto", k_step=None, segments=None):
-        """convert() without the assembly -> ([(start_frame, output [T])], the model's sample rate)"""
+        """main_diff.py's conversion, sliced, without the cross-faded assembly -> ([(start_frame, output [T])], the
+        model's sample rate); ``convert`` takes the same arguments and returns the assembled output"""
         _need_audio(audio)
         sample_rate = int(sample_rate)
         s = self.settings(k_step, speedup, method, diff_spk_id, whole=False)
@@ -445,15 +426,6 @@ class OfflineDiffVC(_Offline):
                                        seg_mel)
                 rendered.append((start, self._mask(out, mask, start).reshape(-1)))
         return rendered, self.model_sr
-
-    def convert(self, audio, sample_rate, key=0, spk_id=1, spk_mix_dict=None, f0_min=50, f0_max=1100, threhold=-60,
-                formant_shift_key=0, diff_spk_id="auto", speedup="auto", method="auto", k_step=None, segments=None):
-        """main_diff.py's whole-file conversion, sliced and cross-faded -> (output [N_out] CUDA fp32, the model's
-        sample rate)"""
-        return super().convert(audio, sample_rate, key=key, spk_id=spk_id, spk_mix_dict=spk_mix_dict, f0_min=f0_min,
-                               f0_max=f0_max, threhold=threhold, formant_shift_key=formant_shift_key,
-                               diff_spk_id=diff_spk_id, speedup=speedup, method=method, k_step=k_step,
-                               segments=segments)
 
     def convert_whole(self, audio, sample_rate, key=0, spk_id=1, spk_mix_dict=None, f0_min=50, f0_max=1100,
                       threhold=-60, formant_shift_key=0, diff_spk_id="auto", speedup="auto", method="auto",

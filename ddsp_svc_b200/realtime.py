@@ -37,10 +37,12 @@ torch's CUDA generator, and GaussianDiffusion keeps its step rows and coefficien
 ``BatchedRealtimeVC(model_path, sessions, ...)`` is gui.py's block for N independent sessions on one model, one RMVPE
 and one units encoder: rows of one batch, the same two graphs replayed for all of them (see its docstring).
 
-The sessions share ``_Session``: the ring buffer, the upload and the owned stream, capture with a warm-up and a state
-restore, the f0 / volume / mask / units front half, the resampling -> SOLA -> crossfade -> pinned-copy tail and
-SineGen's draws.  ``reflow_frames`` and ``diff_frames`` are the reflow and diffusion blocks' frame bookkeeping as pure
-functions.
+The sessions share ``_Session``: the ring buffer, the upload and the owned stream, one launch path for every stage
+(eager, or captured with a warm-up and a state restore, then replayed), ``process``, the f0 / volume / mask / units
+front half, the resampling -> SOLA -> crossfade -> pinned-copy tail, and the draws: each session declares its static
+draw buffers per stage in ``draw_buffers``, in the order they are drawn (torch's CUDA generator advances in that order,
+so every seeded result depends on it).  ``reflow_frames`` and ``diff_frames`` are the reflow and diffusion blocks' frame
+bookkeeping as pure functions.
 """
 import gc
 
@@ -48,17 +50,38 @@ import numpy as np
 import torch
 
 from . import frontend, ops
-from .diffusion_vocoder import DiffGtMel, Unit2WavFast, read_config
+from .diffusion_vocoder import DiffGtMel, read_config
 from .dropin import load_model
 from .enhancer import Enhancer, adaptive_rate, auto_key
 from .hubert import Units_Encoder
 from .reflow_vocoder import load_model_vocoder
 from .rmvpe import RMVPE, Resampler, resampled_length
 from .unit2control import spk_mix_embedding
+from .vocoder import CombSubSuperFast
 
 # the largest f0 RMVPE decodes (cents 20 * 359 + 1997.38 above 10 Hz): bounds the keys 'auto' can pick
 RMVPE_F0_MAX = 10 * 2 ** ((20 * 359 + 1997.3794084376191) / 1200)
 SINEGEN_DIM = 9                                                         # NSF-HiFiGAN's SineGen: harmonic_num 8
+# the distributions of the static draw buffers: standard normal, uniform in [-1, 1), and SineGen's rand_ini (uniform in
+# [0, 1) with its first entry zeroed)
+NORMAL, UNIFORM, RAND_INI = "normal", "uniform", "rand_ini"
+
+
+def cuda_device(device, who, pitch_extractor="rmvpe"):
+    """the torch.device a converter runs on (default 'cuda'); ValueError for any pitch extractor but 'rmvpe' or a
+    device that is not CUDA: only those have kernels"""
+    if pitch_extractor != "rmvpe":
+        raise ValueError("%s extracts f0 with 'rmvpe' only: %r has no kernels" % (who, pitch_extractor))
+    device = torch.device("cuda" if device is None else device)
+    if device.type != "cuda":
+        raise ValueError("%s runs on the CUDA kernels: device must be a CUDA device" % who)
+    return device
+
+
+def noise_kind(model):
+    """the distribution of a DDSP synthesizer's noise: randn for CombSubSuperFast, uniform in [-1, 1) for the others
+    (ddsp/vocoder.py)"""
+    return NORMAL if isinstance(model, CombSubSuperFast) else UNIFORM
 
 
 def gui_frames(samplerate, block_time, crossfade_time, extra_time):
@@ -167,13 +190,15 @@ def diff_frames(samplerate, block_time, crossfade_time, extra_time, model_sr, bl
 class _Session:
     """What the real-time sessions share (see the module's docstring)"""
 
-    def _init_block(self, samplerate, block_time, crossfade_time, extra_time, device, who):
-        self.device = torch.device("cuda" if device is None else device)
-        if self.device.type != "cuda":
-            raise ValueError("%s runs on the CUDA kernels: device must be a CUDA device" % who)
+    def _init_block(self, samplerate, block_time, crossfade_time, extra_time, f0_max, use_phase_vocoder, graph, device,
+                    who, pitch_extractor="rmvpe"):
+        self.device = cuda_device(device, who, pitch_extractor)
         f = gui_frames(samplerate, block_time, crossfade_time, extra_time)
         self.sr, self.block, self.cf, self.search, self.delay = f["sr"], f["block"], f["cf"], f["search"], f["delay"]
         self.n_in, self.silence_front = f["n_in"], f["silence_front"]
+        self.f0_max = float(f0_max)
+        self.use_pv, self.graph = bool(use_phase_vocoder), bool(graph)
+        self.graphs = {}                                    # key -> (CUDA graph, its static outputs), see _run
 
     def _init_front(self, data, f0_min, threhold, pitch_adjust, spk_id, use_spk_mix, spk_mix_dict, rmvpe_ckpt, who):
         """the f0 / volume / mask / units half (models, frames, ring and staging buffers) and the SOLA state; ``data``:
@@ -212,12 +237,37 @@ class _Session:
         self.in_host = torch.zeros(*rows, self.block, dtype=torch.float32).pin_memory()
         self.out_host = torch.zeros(*rows, self.block, dtype=torch.float32).pin_memory()
 
-    @staticmethod
-    def _draw_sinegen(rand_ini, noise):
-        """SineGen's draws into static buffers: rand_ini torch.rand with its first entry zeroed, noise randn"""
-        rand_ini.uniform_()
-        rand_ini[..., 0] = 0
-        noise.normal_()
+    def _init_enhancer(self, keys, rows, top):
+        """the enhancer's SineGen draw buffers for ``rows`` rows, long enough for adaptive key ``top``, as graph B's
+        draws, and its resampling tables for ``keys``"""
+        ehop = self.enhancer.enhancer_hop_size
+        rate = adaptive_rate(self.enhancer.enhancer_sample_rate, top)[0]
+        n_mel = int(self.noise.shape[1] * rate / self.model_sr) // ehop + 4
+        self.gen_rand_ini = torch.zeros(1, 1, SINEGEN_DIM, device=self.device)
+        self.gen_noise = torch.zeros(rows, n_mel * ehop, SINEGEN_DIM, device=self.device)
+        self.draw_buffers["enhancer_noise"] = [("gen_rand_ini", RAND_INI), ("gen_noise", NORMAL)]
+        self.enhancer.prepare(self.model_sr, keys)
+
+    def _draw_noise(self):
+        """the draws of graph A, or of the whole block: the synthesizer's noise and, in the reflow and diffusion
+        blocks, the sampler's and the vocoder's"""
+        self._draw("noise")
+
+    def _draw_enhancer_noise(self):
+        """the draws of graph B: the enhancer's SineGen rand_ini and noise"""
+        self._draw("enhancer_noise")
+
+    def _draw(self, stage):
+        """fill the static draw buffers of ``stage``, in the order ``draw_buffers[stage]`` lists them"""
+        for name, kind in self.draw_buffers[stage]:
+            t = getattr(self, name)
+            if kind == NORMAL:
+                t.normal_()
+            elif kind == UNIFORM:
+                t.uniform_(-1, 1)
+            else:
+                t.uniform_()
+                t[..., 0] = 0
 
     def _front(self):
         """ring buffer -> f0 [1, n_frames, 1] (pitch factor applied), volume [1, n_frames], mask [1, n_frames], units"""
@@ -272,6 +322,32 @@ class _Session:
                 gc.enable()
         return g, static
 
+    def _run(self, key, stage, state):
+        """enqueue ``stage`` on the session's stream -> its outputs.  With graph=False it runs eagerly; otherwise it is
+        captured as graph ``key`` on first use (``state``: the tensors the warm-up must leave as it found them) and
+        replayed, and the outputs are the graph's static ones."""
+        if not self.graph:
+            with torch.cuda.stream(self.stream):
+                return stage()
+        if key not in self.graphs:
+            self.graphs[key] = self._capture(stage, state)
+        g, static = self.graphs[key]
+        with torch.cuda.stream(self.stream):                            # a replay runs on the current stream
+            g.replay()
+        return static
+
+    def run(self):
+        """enqueue the block's graph (or its eager code) on the session's stream"""
+        self._run("block", self._stage, [self.ring, self.sola_buffer])
+
+    def process(self, indata):
+        """audio_callback's math: indata [frames, channels] -> outdata [frames, 2] (float32); BatchedRealtimeVC takes
+        [N, frames(, channels)] and returns [N, frames, 2]"""
+        self.upload(indata)
+        self.run()
+        self.stream.synchronize()
+        return np.repeat(self.out_host.numpy()[..., None], 2, axis=-1)
+
     def upload(self, indata):
         """the new block (mono as librosa.to_mono averages channels) into the device staging buffer"""
         x = np.asarray(indata, dtype=np.float32)
@@ -282,22 +358,15 @@ class _Session:
         with torch.cuda.stream(self.stream):
             self.new_block.copy_(self.in_host, non_blocking=True)
 
-    def _output(self):
-        self.stream.synchronize()
-        return np.repeat(self.out_host.numpy()[:, None], 2, axis=1)
-
 
 class RealtimeVC(_Session):
     def __init__(self, model_path, samplerate=44100, block_time=0.3, crossfade_time=0.04, extra_time=2.0, f0_min=50,
                  f0_max=1100, threhold=-45, spk_id=1, pitch_adjust=0.0, use_spk_mix=False, spk_mix_dict=None,
                  use_enhancer=True, enhancer_adaptive_key=0, use_phase_vocoder=False, graph=True,
                  pitch_extractor_type="rmvpe", rmvpe_ckpt="pretrain/rmvpe/model.pt", device=None):
-        if pitch_extractor_type != "rmvpe":
-            raise ValueError("RealtimeVC extracts f0 with 'rmvpe' only: %r has no kernels" % (pitch_extractor_type,))
-        self._init_block(samplerate, block_time, crossfade_time, extra_time, device, "RealtimeVC")
-        self.f0_max = float(f0_max)
+        self._init_block(samplerate, block_time, crossfade_time, extra_time, f0_max, use_phase_vocoder, graph, device,
+                         "RealtimeVC", pitch_extractor_type)
         self.use_enhancer, self.key = bool(use_enhancer), enhancer_adaptive_key
-        self.use_pv, self.graph = bool(use_phase_vocoder), bool(graph)
 
         self.model, self.args = load_model(model_path, device=self.device)
         self._init_front(self.args.data, f0_min, threhold, pitch_adjust, spk_id, use_spk_mix, spk_mix_dict,
@@ -305,32 +374,15 @@ class RealtimeVC(_Session):
         self.enhancer = Enhancer(self.args.enhancer.type, self.args.enhancer.ckpt, self.device) if use_enhancer else None
         self.out_sr = self.enhancer.enhancer_sample_rate if use_enhancer else self.model_sr
 
-        dev = self.device
-        # the synthesizer's noise: randn for CombSubSuperFast, uniform in [-1, 1) for the others (ddsp/vocoder.py)
-        self.noise = torch.zeros(1, self.n_frames * self.block_size, device=dev)
-        self.noise_normal = self.args.model.type == "CombSubSuperFast"
+        self.noise = torch.zeros(1, self.n_frames * self.block_size, device=self.device)
+        self.draw_buffers = {"noise": [("noise", noise_kind(self.model))], "enhancer_noise": []}
         if use_enhancer:
-            ehop = self.enhancer.enhancer_hop_size
-            top = adaptive_rate(self.enhancer.enhancer_sample_rate, self.max_key())[0]
-            n_mel = int(self.noise.shape[1] * top / self.model_sr) // ehop + 4
-            self.gen_rand_ini = torch.zeros(1, 1, SINEGEN_DIM, device=dev)
-            self.gen_noise = torch.zeros(1, n_mel * ehop, SINEGEN_DIM, device=dev)
-            self.enhancer.prepare(self.model_sr, [self.key] if self.key != "auto" else range(self.max_key() + 1))
+            self._init_enhancer([self.key] if self.key != "auto" else range(self.max_key() + 1), 1, self.max_key())
         self.ratio_host = torch.zeros(1, dtype=torch.float32).pin_memory()
-        self.graph_a, self.graphs_b = None, {}
 
     def max_key(self):
         """the largest adaptive key 'auto' can pick for the f0 RMVPE decodes, after the pitch factor"""
         return int(auto_key(max(RMVPE_F0_MAX, self.f0_min) * self.pitch_factor / 760))
-
-    def _draw_noise(self):
-        if self.noise_normal:
-            self.noise.normal_()
-        else:
-            self.noise.uniform_(-1, 1)
-
-    def _draw_enhancer_noise(self):
-        self._draw_sinegen(self.gen_rand_ini, self.gen_noise)
 
     # ---- the two halves of the block ----------------------------------------------------------------------------------
     def _stage_a(self):
@@ -346,8 +398,8 @@ class RealtimeVC(_Session):
 
     def _stage_b(self, out, f0, key):
         """synthesizer output -> the block in the pinned output buffer; the SOLA buffer advanced"""
+        self._draw_enhancer_noise()
         if self.use_enhancer:
-            self._draw_enhancer_noise()
             out, _ = self.enhancer.enhance(out, self.model_sr, f0, self.block_size, adaptive_key=key,
                                            silence_front=self.silence_front, rand_ini=self.gen_rand_ini,
                                            noise=self.gen_noise)
@@ -356,14 +408,7 @@ class RealtimeVC(_Session):
     # ---- one callback -------------------------------------------------------------------------------------------------
     def run_a(self):
         """enqueue graph A (or its eager code) on the session's stream"""
-        if not self.graph:
-            with torch.cuda.stream(self.stream):
-                self._a = self._stage_a()
-        else:
-            if self.graph_a is None:
-                self.graph_a, self._a = self._capture(self._stage_a, [self.ring])
-            with torch.cuda.stream(self.stream):                        # a replay runs on the current stream
-                self.graph_a.replay()
+        self._a = self._run("a", self._stage_a, [self.ring])
 
     def pick_key(self):
         """the adaptive key of this block; with 'auto', reads max f0 from the device (the block's one mid-block sync)"""
@@ -376,26 +421,12 @@ class RealtimeVC(_Session):
 
     def run_b(self, key):
         """enqueue graph B[key] (or its eager code) on the session's stream"""
-        out, f0, _ = self._a
-        if not self.graph:
-            with torch.cuda.stream(self.stream):
-                self._stage_b(out, f0, key)
-            return
-        g = self.graphs_b.get(key)
-        if g is None:
-            if self.use_enhancer:
-                self.enhancer.prepare(self.model_sr, [key])
-            g, _ = self._capture(lambda: self._stage_b(out, f0, key), [self.sola_buffer])
-            self.graphs_b[key] = g
-        with torch.cuda.stream(self.stream):
-            g.replay()
+        self._run(("b", key), lambda: self._stage_b(self._a[0], self._a[1], key), [self.sola_buffer])
 
-    def process(self, indata):
-        """audio_callback's math: indata [frames, channels] -> outdata [frames, 2] (float32)"""
-        self.upload(indata)
+    def run(self):
+        """enqueue the block: graph A, the adaptive key, graph B[key]"""
         self.run_a()
         self.run_b(self.pick_key())
-        return self._output()
 
 
 # a session's settings in BatchedRealtimeVC and their defaults (RealtimeVC's)
@@ -452,10 +483,9 @@ class BatchedRealtimeVC(_Session):
         self.n = len(self.settings)
         if self.n == 0:
             raise ValueError("BatchedRealtimeVC needs at least one session")
-        self._init_block(samplerate, block_time, crossfade_time, extra_time, device, "BatchedRealtimeVC")
-        self.f0_max = float(f0_max)
+        self._init_block(samplerate, block_time, crossfade_time, extra_time, f0_max, use_phase_vocoder, graph, device,
+                         "BatchedRealtimeVC")
         self.use_enhancer, self.key = bool(use_enhancer), key
-        self.use_pv, self.graph = bool(use_phase_vocoder), bool(graph)
 
         self.model, self.args = load_model(model_path, device=self.device)
         self._init_models(self.args.data, f0_min, rmvpe_ckpt, "BatchedRealtimeVC")
@@ -477,19 +507,10 @@ class BatchedRealtimeVC(_Session):
             for i in range(N):
                 self._write_speaker(i)
         self.noise = torch.zeros(N, self.n_frames * self.block_size, device=dev)
-        self.noise_normal = self.args.model.type == "CombSubSuperFast"
+        self.draw_buffers = {"noise": [("noise", noise_kind(self.model))], "enhancer_noise": []}
         if use_enhancer:
-            ehop = self.enhancer.enhancer_hop_size
-            rate = adaptive_rate(self.enhancer.enhancer_sample_rate, key)[0]
-            n_mel = int(self.noise.shape[1] * rate / self.model_sr) // ehop + 4
-            self.gen_rand_ini = torch.zeros(1, 1, SINEGEN_DIM, device=dev)
-            self.gen_noise = torch.zeros(N, n_mel * ehop, SINEGEN_DIM, device=dev)
-            self.enhancer.prepare(self.model_sr, [key])
-        self.graph_a = self.graph_b = None
+            self._init_enhancer([key], N, key)
         self.stream.synchronize()
-
-    _draw_noise = RealtimeVC._draw_noise
-    _draw_enhancer_noise = RealtimeVC._draw_enhancer_noise
 
     # ---- per-session settings ---------------------------------------------------------------------------------------
     def _write_speaker(self, i):
@@ -547,8 +568,8 @@ class BatchedRealtimeVC(_Session):
 
     def _stage_b(self, out, f0):
         """synthesizer output -> the N blocks in the pinned output buffer; the SOLA buffers advanced"""
+        self._draw_enhancer_noise()
         if self.use_enhancer:
-            self._draw_enhancer_noise()
             out, _ = self.enhancer.enhance(out, self.model_sr, f0, self.block_size, adaptive_key=self.key,
                                            silence_front=self.silence_front, rand_ini=self.gen_rand_ini,
                                            noise=self.gen_noise)
@@ -578,33 +599,26 @@ class BatchedRealtimeVC(_Session):
 
     def run_a(self):
         """enqueue graph A (or its eager code) on the session's stream"""
-        if not self.graph:
-            with torch.cuda.stream(self.stream):
-                self._a = self._stage_a()
-        else:
-            if self.graph_a is None:
-                self.graph_a, self._a = self._capture(self._stage_a, [self.ring])
-            with torch.cuda.stream(self.stream):
-                self.graph_a.replay()
+        self._a = self._run("a", self._stage_a, [self.ring])
 
     def run_b(self):
         """enqueue graph B (or its eager code) on the session's stream"""
-        if not self.graph:
-            with torch.cuda.stream(self.stream):
-                self._stage_b(*self._a)
-            return
-        if self.graph_b is None:
-            self.graph_b, _ = self._capture(lambda: self._stage_b(*self._a), [self.sola_buffer])
-        with torch.cuda.stream(self.stream):
-            self.graph_b.replay()
+        self._run("b", lambda: self._stage_b(*self._a), [self.sola_buffer])
 
-    def process(self, indata):
-        """one callback for every session: indata [N, frames] or [N, frames, channels] -> outdata [N, frames, 2]"""
-        self.upload(indata)
+    @property
+    def graph_a(self):
+        """graph A once captured, else None"""
+        return self.graphs.get("a", (None,))[0]
+
+    @property
+    def graph_b(self):
+        """graph B once captured, else None"""
+        return self.graphs.get("b", (None,))[0]
+
+    def run(self):
+        """enqueue the block for every session: graph A, then graph B"""
         self.run_a()
         self.run_b()
-        self.stream.synchronize()
-        return np.repeat(self.out_host.numpy()[:, :, None], 2, axis=2)
 
 
 class RealtimeReflowVC(_Session):
@@ -616,18 +630,14 @@ class RealtimeReflowVC(_Session):
                  f0_max=1100, threhold=-45, spk_id=1, pitch_adjust=0.0, formant_shift_key=0.0, use_spk_mix=False,
                  spk_mix_dict=None, use_phase_vocoder=False, t_start=0.7, infer_step=30, sampling_method="euler",
                  graph=True, pitch_extractor_type="rmvpe", rmvpe_ckpt="pretrain/rmvpe/model.pt", device=None):
-        if pitch_extractor_type != "rmvpe":
-            raise ValueError("RealtimeReflowVC extracts f0 with 'rmvpe' only: %r has no kernels"
-                             % (pitch_extractor_type,))
+        self._init_block(samplerate, block_time, crossfade_time, extra_time, f0_max, use_phase_vocoder, graph, device,
+                         "RealtimeReflowVC", pitch_extractor_type)
         if int(infer_step) != infer_step or infer_step < 1:
             raise ValueError("infer_step must be an integer >= 1, got %r" % (infer_step,))
         if sampling_method not in ("euler", "rk4"):
             raise ValueError("sampling_method must be 'euler' or 'rk4', got %r" % (sampling_method,))
-        self._init_block(samplerate, block_time, crossfade_time, extra_time, device, "RealtimeReflowVC")
-        self.f0_max = float(f0_max)
         self.formant_shift_key, self.t_start = float(formant_shift_key), float(t_start)
         self.infer_step, self.method = int(infer_step), sampling_method
-        self.use_pv, self.graph = bool(use_phase_vocoder), bool(graph)
 
         self.model, self.vocoder, self.args = load_model_vocoder(model_path, device=self.device)
         data = self.args.data
@@ -643,13 +653,8 @@ class RealtimeReflowVC(_Session):
         self.reflow_noise = torch.zeros(1, 1, self.vocoder.dimension, T, device=dev)
         self.gen_rand_ini = torch.zeros(1, 1, SINEGEN_DIM, device=dev)
         self.gen_noise = torch.zeros(1, T * self.vocoder.vocoder_hop_size, SINEGEN_DIM, device=dev)
-        self.graph_block = None
-
-    def _draw_noise(self):
-        """the block's draws: the DDSP noise, the sampler's initial noise, SineGen's rand_ini and noise"""
-        self.noise.normal_()
-        self.reflow_noise.normal_()
-        self._draw_sinegen(self.gen_rand_ini, self.gen_noise)
+        self.draw_buffers = {"noise": [("noise", NORMAL), ("reflow_noise", NORMAL), ("gen_rand_ini", RAND_INI),
+                                       ("gen_noise", NORMAL)]}
 
     def _stage(self):
         f0, volume, mask, units = self._front()
@@ -662,23 +667,6 @@ class RealtimeReflowVC(_Session):
                              reflow_noise=self.reflow_noise, rand_ini=self.gen_rand_ini, sine_noise=self.gen_noise)
         out = frontend.mask_apply_(out.reshape(1, -1).contiguous(), mask, self.block_size, self.mask_offset)
         self._tail(out, self.model_sr)
-
-    def run(self):
-        """enqueue the block's graph (or its eager code) on the session's stream"""
-        if not self.graph:
-            with torch.cuda.stream(self.stream):
-                self._stage()
-            return
-        if self.graph_block is None:
-            self.graph_block, _ = self._capture(self._stage, [self.ring, self.sola_buffer])
-        with torch.cuda.stream(self.stream):
-            self.graph_block.replay()
-
-    def process(self, indata):
-        """audio_callback's math: indata [frames, channels] -> outdata [frames, 2] (float32)"""
-        self.upload(indata)
-        self.run()
-        return self._output()
 
 
 DIFF_METHODS = ("ddim", "pndm", "dpm-solver", "unipc")
@@ -699,8 +687,8 @@ class RealtimeDiffVC(_Session):
                  spk_mix_dict=None, use_phase_vocoder=False, k_step=100, diff_acc=10, diff_method="ddim",
                  diff_silence=False, graph=True, pitch_extractor_type="rmvpe", rmvpe_ckpt="pretrain/rmvpe/model.pt",
                  device=None):
-        if pitch_extractor_type != "rmvpe":
-            raise ValueError("RealtimeDiffVC extracts f0 with 'rmvpe' only: %r has no kernels" % (pitch_extractor_type,))
+        self._init_block(samplerate, block_time, crossfade_time, extra_time, f0_max, use_phase_vocoder, graph, device,
+                         "RealtimeDiffVC", pitch_extractor_type)
         if diff_method not in DIFF_METHODS:
             raise ValueError("diff_method must be one of %s, got %r" % (", ".join(DIFF_METHODS), diff_method))
         if int(k_step) != k_step or k_step < 0:
@@ -708,10 +696,8 @@ class RealtimeDiffVC(_Session):
         if int(diff_acc) != diff_acc or (k_step > 0 and not 1 <= diff_acc <= k_step // 2):
             raise ValueError("diff_acc must be an integer in [1, k_step // 2] = [1, %d] (1: DDPM), got %r"
                              % (int(k_step) // 2, diff_acc))
-        self._init_block(samplerate, block_time, crossfade_time, extra_time, device, "RealtimeDiffVC")
-        self.f0_max = float(f0_max)
         self.k_step, self.diff_acc, self.diff_method = int(k_step), int(diff_acc), diff_method
-        self.diff_silence, self.use_pv, self.graph = bool(diff_silence), bool(use_phase_vocoder), bool(graph)
+        self.diff_silence = bool(diff_silence)
 
         # SvcDDSP.update_model: the DDSP checkpoint's config is checked against the diffusion model's (check_args)
         args = read_config(diff_model_path)
@@ -739,13 +725,15 @@ class RealtimeDiffVC(_Session):
 
         dev, fr, M = self.device, self.frames, self.vocoder.dimension
         T = fr["cond_frames"]
-        self.ext_noise = None                 # the external DDSP model's noise: randn for CombSubSuperFast, else uniform
+        draws = []
+        self.ext_noise = None                 # the external DDSP model's noise
         if self.ddsp_model is not None:
             self.ext_noise = torch.zeros(1, self.n_frames * self.block_size, device=dev)
-            self.ext_normal = self.ddsp_args.model.type == "CombSubSuperFast"
-        self.ddsp_noise = None                # Unit2Wav's CombSubFast (uniform) / Unit2WavFast's CombSubSuperFast (randn)
+            draws.append(("ext_noise", noise_kind(self.ddsp_model)))
+        self.ddsp_noise = None                # Unit2Wav's CombSubFast / Unit2WavFast's CombSubSuperFast
         if kind != "Diffusion":
             self.ddsp_noise = torch.zeros(1, T * self.block_size, device=dev)
+            draws.append(("ddsp_noise", noise_kind(self.model.ddsp_model)))
         # the sampler's start: with a gt_spec, randn_like of the transposed [B, 1, M, T] view; without, torch.randn
         has_gt = kind != "Diffusion" or self.ddsp_model is not None
         runs = kind == "Diffusion" or self.k_step > 0
@@ -753,30 +741,14 @@ class RealtimeDiffVC(_Session):
         if runs:
             self.diff_noise = (torch.empty_strided((1, 1, M, T), (T * M, T * M, 1, M), device=dev) if has_gt else
                                torch.empty(1, 1, M, T, device=dev)).zero_()
+            draws.append(("diff_noise", NORMAL))
             if self.diff_acc == 1:
                 n_steps = self.k_step if has_gt else self.model.decoder.k_step
                 self.step_noise = torch.zeros(n_steps, 1, 1, M, T, device=dev)
+                draws.append(("step_noise", NORMAL))
         self.gen_rand_ini = torch.zeros(1, 1, SINEGEN_DIM, device=dev)
         self.gen_noise = torch.zeros(1, fr["voc_frames"] * self.vocoder.vocoder_hop_size, SINEGEN_DIM, device=dev)
-        self.graph_block = None
-
-    def _draw_noise(self):
-        """the block's draws: the DDSP noise, the sampler's start, DDPM's per-step noise, SineGen's rand_ini and noise"""
-        if self.ext_noise is not None:
-            if self.ext_normal:
-                self.ext_noise.normal_()
-            else:
-                self.ext_noise.uniform_(-1, 1)
-        if self.ddsp_noise is not None:
-            if isinstance(self.model, Unit2WavFast):
-                self.ddsp_noise.normal_()
-            else:
-                self.ddsp_noise.uniform_(-1, 1)
-        if self.diff_noise is not None:
-            self.diff_noise.normal_()
-        if self.step_noise is not None:
-            self.step_noise.normal_()
-        self._draw_sinegen(self.gen_rand_ini, self.gen_noise)
+        self.draw_buffers = {"noise": draws + [("gen_rand_ini", RAND_INI), ("gen_noise", NORMAL)]}
 
     def draws(self):
         """the draws DiffGtMel.infer takes, from the static buffers"""
@@ -798,20 +770,3 @@ class RealtimeDiffVC(_Session):
                                   use_silence=self.diff_silence, spk_mix_dict=self.spk_mix_dict, **self.draws())
         out = frontend.mask_apply_(out.reshape(1, -1).contiguous(), mask, self.block_size)
         self._tail(out, self.model_sr)
-
-    def run(self):
-        """enqueue the block's graph (or its eager code) on the session's stream"""
-        if not self.graph:
-            with torch.cuda.stream(self.stream):
-                self._stage()
-            return
-        if self.graph_block is None:
-            self.graph_block, _ = self._capture(self._stage, [self.ring, self.sola_buffer])
-        with torch.cuda.stream(self.stream):
-            self.graph_block.replay()
-
-    def process(self, indata):
-        """audio_callback's math: indata [frames, channels] -> outdata [frames, 2] (float32)"""
-        self.upload(indata)
-        self.run()
-        return self._output()

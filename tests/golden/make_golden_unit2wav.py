@@ -8,7 +8,7 @@ Needs a reference checkout (DDSP_REFERENCE_ROOT; librosa / soundfile stubbed as 
 Weights are not stored: ``state_dict`` / ``generator_state_dict`` rebuild them from a seed without the reference (the
 package's Unit2Wav and Generator have the reference's trees): the DDSP model at its default init under
 ``torch.manual_seed``, the velocity network and the vocoder through tests/reflow_oracle.seeded_weights (every parameter
-non-zero).  The vocoder is bench_realtime.HIFIGAN (44.1 kHz, hop 512, 128 mels).  unit2wav_state_dicts.json lists the
+non-zero).  The vocoder is conversion_fixtures.HIFIGAN (44.1 kHz, hop 512, 128 mels).  unit2wav_state_dicts.json lists the
 reference Unit2Wav's keys and shapes for each model.
 
 Each file holds the inputs (units, f0, volume, spk_id, aug_shift), the case's settings, the reference's fp32 output
@@ -33,8 +33,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-from bench_realtime import HIFIGAN  # noqa: E402
 from tests import reflow_oracle  # noqa: E402
+from conversion_fixtures import HIFIGAN  # noqa: E402
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 N_UNIT, N_SPK, UPP = 256, 2, 512

@@ -11,7 +11,7 @@ import math
 import pytest
 import torch
 
-from bench_realtime import HIFIGAN
+from conversion_fixtures import HIFIGAN, write_synthetic_diff
 from ddsp_svc_b200 import _lib
 from ddsp_svc_b200 import diffusion_vocoder as dv
 from ddsp_svc_b200.nsf_vocoder import Vocoder
@@ -214,7 +214,6 @@ def test_u2c_embed_with_phase_is_unchanged():
 
 
 def test_load_model_vocoder_round_trip(tmp_path):
-    from bench_realtime_diff import write_synthetic_diff
     with contextlib.redirect_stdout(io.StringIO()):
         _, path, _ = write_synthetic_diff(str(tmp_path), "DiffusionFast", n_chans=128, n_layers=2, encoder="hubertsoft")
         model, vocoder, args = dv.load_model_vocoder(path, device=DEV)

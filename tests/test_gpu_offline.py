@@ -1,10 +1,8 @@
 """OfflineVC / OfflineReflowVC (ddsp_svc_b200/offline.py) on the GPU: the Slicer's RMS kernel against float64 and the
 goldens' chunks, and whole-file conversions against main.py's / main_reflow.py's own loops over the same modules
 (tests/offline_oracle.py) with the same torch seed -- every segment's output bit for bit, the assembled waveform within
-one fp32 ulp of the float64 result and only on faded samples.  Synthetic seeded checkpoints (bench_realtime and
-bench_realtime_reflow's writers)."""
-import contextlib
-import io
+one fp32 ulp of the float64 result and only on faded samples.  Synthetic seeded checkpoints (conversion_fixtures'
+writers)."""
 import os
 
 import numpy as np
@@ -12,8 +10,7 @@ import pytest
 import torch
 import yaml
 
-from bench_realtime import write_synthetic
-from bench_realtime_reflow import write_synthetic_reflow
+from conversion_fixtures import quiet, write_synthetic, write_synthetic_reflow
 from ddsp_svc_b200 import frontend, offline
 from ddsp_svc_b200.offline import OfflineReflowVC, OfflineVC
 from tests import offline_oracle as oo
@@ -27,11 +24,6 @@ CLIPS = {"three_pauses": [("v", 6.0), ("s", 1.0), ("v", 6.0), ("s", 7.0), ("v", 
          "two_pauses": [("s", 0.5), ("v", 8.0), ("s", 2.5), ("v", 7.0), ("s", 3.0)],
          "four_pauses": [("v", 5.5), ("s", 0.6), ("v", 5.5), ("s", 1.2), ("v", 6.0), ("s", 0.4), ("v", 5.2),
                          ("s", 0.8), ("v", 5.0)]}
-
-
-def quiet(fn, *a, **k):
-    with contextlib.redirect_stdout(io.StringIO()):
-        return fn(*a, **k)
 
 
 @pytest.fixture(scope="module")

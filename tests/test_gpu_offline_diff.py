@@ -6,10 +6,8 @@ Each segment's output is bit-identical to the loop's, the assembled waveform is 
 result and differs only on faded samples, and convert_whole equals infer() bit for bit.  The cases reach every mode of
 each model type under both drivers ('ddsp': the external DDSP model's mel; 'input_mel'; 'none'), DDPM and four samplers
 at speedup 10 or more, k_step above k_step_max, formant keys 0 and +-3, a speaker mix and an explicit diffusion speaker.
-Checkpoints are synthetic and seeded (bench_realtime_diff.write_synthetic_diff, small widths), with a CombSubSuperFast
+Checkpoints are synthetic and seeded (conversion_fixtures.write_synthetic_diff, small widths), with a CombSubSuperFast
 DDSP checkpoint that fits and a CombSub one at block_size 256 that does not."""
-import contextlib
-import io
 import os
 
 import numpy as np
@@ -17,7 +15,7 @@ import pytest
 import torch
 import yaml
 
-from bench_realtime_diff import DDSP_MODELS, write_synthetic_diff
+from conversion_fixtures import DDSP_MODELS, quiet, write_synthetic_diff, write_synthetic_reflow
 from ddsp_svc_b200 import dropin, offline
 from ddsp_svc_b200.offline import OfflineDiffVC
 from tests import offline_diff_oracle as odo
@@ -29,11 +27,6 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 TYPES = ("Diffusion", "DiffusionNew", "DiffusionFast")
 MIX = {1: 0.25, 2: 0.75}
-
-
-def quiet(fn, *a, **k):
-    with contextlib.redirect_stdout(io.StringIO()):
-        return fn(*a, **k)
 
 
 @pytest.fixture(scope="module")
@@ -216,7 +209,6 @@ def test_value_errors(ckpts):
 def test_reflow_first_call_matches_main_reflow_py(tmp_path):
     """the first Unit2Wav call after loading equals main_reflow.py's loop under the same seed: the vocoder's generator,
     built on that call, no longer advances torch's CPU generator, from which SineGen's noise seed is drawn"""
-    from bench_realtime_reflow import write_synthetic_reflow
     from ddsp_svc_b200.offline import OfflineReflowVC
     model_path, rmvpe_path = quiet(write_synthetic_reflow, str(tmp_path), n_chans=128, n_layers=2, encoder="hubertsoft")
     rf = quiet(OfflineReflowVC, model_path, device=DEV, rmvpe_ckpt=rmvpe_path)

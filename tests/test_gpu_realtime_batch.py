@@ -1,15 +1,16 @@
 """BatchedRealtimeVC (ddsp_svc_b200/realtime.py) on the GPU: every row against a single RealtimeVC with that session's
 settings, input and draws over consecutive blocks; rows independent of each other bit for bit; graph replay against
 the eager batched session; replays without hidden synchronisation; update() and reset() without recapture; the batched
-kernels against the single-session ones row by row.  Synthetic seeded checkpoints (bench_realtime.write_synthetic)."""
-import contextlib
-import io
+kernels against the single-session ones row by row.  Synthetic seeded checkpoints
+(conversion_fixtures.write_synthetic)."""
+import functools
+import types
 
 import numpy as np
 import pytest
 import torch
 
-from bench_realtime import write_synthetic
+from conversion_fixtures import build_session, copy_draws, quiet, write_synthetic
 from ddsp_svc_b200 import frontend, ops
 from ddsp_svc_b200 import realtime as rt
 from ddsp_svc_b200.realtime import BatchedRealtimeVC, RealtimeVC
@@ -25,21 +26,14 @@ SESSIONS = [dict(spk_id=1, pitch_adjust=0.0, threhold=-45),
 
 @pytest.fixture(scope="module", params=["Sins", "CombSubSuperFast"])
 def ckpt(request, tmp_path_factory):
-    d = tmp_path_factory.mktemp(request.param)
-    with contextlib.redirect_stdout(io.StringIO()):
-        return write_synthetic(str(d), request.param)
+    return quiet(write_synthetic, str(tmp_path_factory.mktemp(request.param)), request.param)
 
 
-def batched(ckpt, sessions=SESSIONS, **kw):
-    model_path, rmvpe_path = ckpt
-    with contextlib.redirect_stdout(io.StringIO()):
-        return BatchedRealtimeVC(model_path, sessions, rmvpe_ckpt=rmvpe_path, device=DEV, **kw)
+batched = functools.partial(build_session, BatchedRealtimeVC, sessions=SESSIONS)
 
 
 def single(ckpt, settings, **kw):
-    model_path, rmvpe_path = ckpt
-    with contextlib.redirect_stdout(io.StringIO()):
-        return RealtimeVC(model_path, rmvpe_ckpt=rmvpe_path, device=DEV, **settings, **kw)
+    return build_session(RealtimeVC, ckpt, **settings, **kw)
 
 
 def voice(n, sr, f, seed):
@@ -55,19 +49,6 @@ def inputs(s, seed=0, n_blocks=N_BLOCKS):
     x = np.stack([voice(n_blocks * s.block, s.sr, 150 + 40 * i, seed + i) for i in range(s.n)])
     x = np.stack([x, 0.5 * x], 2)
     return [x[:, k * s.block:(k + 1) * s.block] for k in range(n_blocks)]
-
-
-def follow(one, b, i):
-    """single session `one` takes row i of batched session b's draws of each block"""
-    one._draw_noise = lambda: one.noise.copy_(b.noise[i:i + 1])
-    if one.use_enhancer:
-        L = b.gen_noise.shape[1]
-        assert one.gen_noise.shape[1] >= L
-
-        def draw():
-            one.gen_rand_ini.copy_(b.gen_rand_ini)
-            one.gen_noise[:, :L].copy_(b.gen_noise[i:i + 1])
-        one._draw_enhancer_noise = draw
 
 
 def record_shifts(monkeypatch):
@@ -92,7 +73,7 @@ def test_rows_match_single_sessions(ckpt, monkeypatch, pv, key):
     b = batched(ckpt, graph=False, use_phase_vocoder=pv, enhancer_adaptive_key=key)
     ones = [single(ckpt, c, graph=False, use_phase_vocoder=pv, enhancer_adaptive_key=key) for c in SESSIONS]
     for i, one in enumerate(ones):
-        follow(one, b, i)
+        copy_draws(one, b, row=i)                                    # one takes row i of b's draws
     shifts = record_shifts(monkeypatch)
     for k, x in enumerate(inputs(b)):
         got = b.process(x)
@@ -114,9 +95,9 @@ def test_rows_are_independent(ckpt):
         b = batched(ckpt, graph=True)
         if draws is None:
             g = torch.Generator(device=DEV).manual_seed(0)
-            draws = [torch.randn(t.shape, device=DEV, generator=g) for t in (b.noise, b.gen_rand_ini, b.gen_noise)]
-        b._draw_noise = lambda b=b: b.noise.copy_(draws[0])
-        b._draw_enhancer_noise = lambda b=b: (b.gen_rand_ini.copy_(draws[1]), b.gen_noise.copy_(draws[2]))
+            draws = types.SimpleNamespace(**{name: torch.randn(getattr(b, name).shape, device=DEV, generator=g)
+                                             for name in ("noise", "gen_rand_ini", "gen_noise")})
+        copy_draws(b, draws)
         outs = []
         for k, x in enumerate(inputs(b)):
             x = x.copy()
@@ -137,8 +118,7 @@ def test_rows_are_independent(ckpt):
 def test_graph_replay_is_bit_identical_to_eager(ckpt, pv):
     g = batched(ckpt, graph=True, use_phase_vocoder=pv, enhancer_adaptive_key=3)
     e = batched(ckpt, graph=False, use_phase_vocoder=pv, enhancer_adaptive_key=3)
-    e._draw_noise = lambda: e.noise.copy_(g.noise)
-    e._draw_enhancer_noise = lambda: (e.gen_rand_ini.copy_(g.gen_rand_ini), e.gen_noise.copy_(g.gen_noise))
+    copy_draws(e, g)
     for x in inputs(g, seed=1):
         assert np.array_equal(g.process(x), e.process(x))
 
@@ -168,8 +148,7 @@ def test_update_matches_fresh_session(ckpt):
                                   spk_mix_dict={1: 0.5, 2: 0.5}), dict(SESSIONS[2])]
     a = batched(ckpt, graph=True)
     f = batched(ckpt, sessions=new, graph=True)
-    f._draw_noise = lambda: f.noise.copy_(a.noise)
-    f._draw_enhancer_noise = lambda: (f.gen_rand_ini.copy_(a.gen_rand_ini), f.gen_noise.copy_(a.gen_noise))
+    copy_draws(f, a)
     xs = inputs(a, seed=3)
     a.process(xs[0])
     graphs = (a.graph_a, a.graph_b)
@@ -190,7 +169,7 @@ def test_reset_matches_fresh_single_session(ckpt):
         b.process(x)
     b.reset(2)
     one = single(ckpt, SESSIONS[2], graph=False)
-    follow(one, b, 2)
+    copy_draws(one, b, row=2)
     for x in xs[2:]:
         got = b.process(x)
         rms, rel = rel_rms(got[2], one.process(x[2]))

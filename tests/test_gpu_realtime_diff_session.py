@@ -1,8 +1,9 @@
 """RealtimeDiffVC (ddsp_svc_b200/realtime.py) on the GPU: the eager session against gui_diff.py's order on the same
 modules and draws over consecutive blocks (the SOLA state carries over), graph replay against the eager session bit
 for bit, replays without hidden synchronisation, and the session's ValueErrors.  Synthetic seeded checkpoints
-(bench_realtime_diff.write_synthetic_diff: 128-channel, 2-layer denoisers and HuBERT-soft units to keep it short)."""
+(conversion_fixtures.write_synthetic_diff: 128-channel, 2-layer denoisers and HuBERT-soft units to keep it short)."""
 import contextlib
+import functools
 import gc
 import io
 import os
@@ -13,42 +14,27 @@ import pytest
 import torch
 import yaml
 
-from bench_realtime_diff import GuiDiffBlock, write_synthetic_diff
+from conversion_fixtures import GuiDiffBlock, blocks, build_session, copy_draws, quiet, write_synthetic_diff
 from ddsp_svc_b200.realtime import RealtimeDiffVC
 from tests import report
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-N_BLOCKS = 5
 MODELS = {"mel_combsub": ("Diffusion", "CombSub"), "mel_superfast": ("Diffusion", "CombSubSuperFast"),
           "mel_none": ("Diffusion", None), "new": ("DiffusionNew", None), "fast": ("DiffusionFast", None)}
 
 
 @pytest.fixture(scope="module")
 def ckpts(tmp_path_factory):
-    out = {}
-    with contextlib.redirect_stdout(io.StringIO()):
-        for name, (kind, ddsp) in MODELS.items():
-            d = tmp_path_factory.mktemp(name)
-            out[name] = write_synthetic_diff(str(d), kind, n_chans=128, n_layers=2, encoder="hubertsoft", ddsp=ddsp)
-    return out
+    return {name: quiet(write_synthetic_diff, str(tmp_path_factory.mktemp(name)), kind, n_chans=128, n_layers=2,
+                        encoder="hubertsoft", ddsp=ddsp) for name, (kind, ddsp) in MODELS.items()}
 
 
 def session(ckpts, model, **kw):
-    ddsp_path, diff_path, rmvpe_path = ckpts[model]
-    kw.setdefault("k_step", 20)
-    kw.setdefault("diff_acc", 5)
-    with contextlib.redirect_stdout(io.StringIO()):
-        return RealtimeDiffVC(ddsp_path, diff_path, rmvpe_ckpt=rmvpe_path, device=DEV, **kw)
+    return build_session(RealtimeDiffVC, ckpts[model], **dict(dict(k_step=20, diff_acc=5), **kw))
 
 
-def blocks(s, seed=0):
-    rng = np.random.default_rng(seed)
-    t = np.arange(N_BLOCKS * s.block) / s.sr
-    x = 0.3 * np.sin(2 * np.pi * (180 * t + 20 * np.sin(2 * np.pi * t))) + 0.01 * rng.standard_normal(t.size)
-    x[s.block // 3:s.block // 2] *= 1e-4                                 # a quiet stretch: the mask closes
-    x = np.stack([x, 0.5 * x], 1).astype(np.float32)
-    return [x[i * s.block:(i + 1) * s.block] for i in range(N_BLOCKS)]
+blocks = functools.partial(blocks, quiet_stretch=True)                 # the mask closes in the first block
 
 
 CASES = {
@@ -81,29 +67,17 @@ def test_eager_session_matches_gui_diff_order(ckpts, case):
         assert rms > 0 and rel < 1e-5, (i, rel)
 
 
-def copy_draws(e, g):
-    """the eager session takes the graph session's draws of each block"""
-    def draw():
-        for name in ("ext_noise", "ddsp_noise", "diff_noise", "step_noise", "gen_rand_ini", "gen_noise"):
-            if getattr(g, name) is not None:
-                getattr(e, name).copy_(getattr(g, name))
-    e._draw_noise = draw
-
-
 @pytest.mark.parametrize("case", ["mel_superfast_pndm_pv", "fast_dpm_silence_pv", "new_ddpm_mix", "mel_combsub_ddim"])
 def test_graph_replay_is_bit_identical_to_eager(ckpts, case):
     model, kw = CASES[case]
     kw = dict(kw, diff_method="ddim") if case == "mel_superfast_pndm_pv" else kw     # DDIM with the phase vocoder
     g = session(ckpts, model, graph=True, **kw)
     e = session(ckpts, model, graph=False, **kw)
-    copy_draws(e, g)
-    try:
-        for x in blocks(g, seed=1):
-            a = g.process(x)
-            b = e.process(x)
-            assert np.array_equal(a, b)
-    finally:
-        del e._draw_noise                                            # no reference cycle outlives the test
+    copy_draws(e, g)                                                 # the eager session takes g's draws
+    for x in blocks(g, seed=1):
+        a = g.process(x)
+        b = e.process(x)
+        assert np.array_equal(a, b)
 
 
 def test_capture_runs_without_the_cycle_collector(ckpts):

@@ -1,8 +1,9 @@
 """RealtimeReflowVC (ddsp_svc_b200/realtime.py) on the GPU: the eager session against gui_reflow.py's order on the same
 modules and draws over consecutive blocks (the SOLA state carries over), graph replay against the eager session bit
 for bit, replays without hidden synchronisation, and the session's ValueErrors.  Synthetic seeded checkpoints
-(bench_realtime_reflow.write_synthetic_reflow, a 128 x 2 velocity network and HuBERT-soft units to keep it short)."""
+(conversion_fixtures.write_synthetic_reflow, a 128 x 2 velocity network and HuBERT-soft units to keep it short)."""
 import contextlib
+import functools
 import io
 import os
 
@@ -11,36 +12,22 @@ import pytest
 import torch
 import yaml
 
-from bench_realtime_reflow import GuiReflowBlock, write_synthetic_reflow
+from conversion_fixtures import GuiReflowBlock, blocks, build_session, copy_draws, quiet, write_synthetic_reflow
 from ddsp_svc_b200.realtime import RealtimeReflowVC
 from tests import report
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-N_BLOCKS = 5
 
 
 @pytest.fixture(scope="module")
 def ckpt(tmp_path_factory):
     d = tmp_path_factory.mktemp("reflow")
-    with contextlib.redirect_stdout(io.StringIO()):
-        return write_synthetic_reflow(str(d), n_chans=128, n_layers=2, encoder="hubertsoft")
+    return quiet(write_synthetic_reflow, str(d), n_chans=128, n_layers=2, encoder="hubertsoft")
 
 
-def session(ckpt, **kw):
-    model_path, rmvpe_path = ckpt
-    kw.setdefault("infer_step", 4)
-    with contextlib.redirect_stdout(io.StringIO()):
-        return RealtimeReflowVC(model_path, rmvpe_ckpt=rmvpe_path, device=DEV, **kw)
-
-
-def blocks(s, seed=0):
-    rng = np.random.default_rng(seed)
-    t = np.arange(N_BLOCKS * s.block) / s.sr
-    x = 0.3 * np.sin(2 * np.pi * (180 * t + 20 * np.sin(2 * np.pi * t))) + 0.01 * rng.standard_normal(t.size)
-    x[s.block // 3:s.block // 2] *= 1e-4                                 # a quiet stretch: the mask closes
-    x = np.stack([x, 0.5 * x], 1).astype(np.float32)
-    return [x[i * s.block:(i + 1) * s.block] for i in range(N_BLOCKS)]
+session = functools.partial(build_session, RealtimeReflowVC, infer_step=4)
+blocks = functools.partial(blocks, quiet_stretch=True)                 # the mask closes in the first block
 
 
 CASES = {
@@ -69,19 +56,11 @@ def test_eager_session_matches_gui_reflow_order(ckpt, case):
         assert rms > 0 and rel < 1e-5, (i, rel)
 
 
-def copy_draws(e, g):
-    """the eager session takes the graph session's draws of each block"""
-    def draw():
-        for name in ("noise", "reflow_noise", "gen_rand_ini", "gen_noise"):
-            getattr(e, name).copy_(getattr(g, name))
-    e._draw_noise = draw
-
-
 @pytest.mark.parametrize("case", ["euler_pv", "rk4"])
 def test_graph_replay_is_bit_identical_to_eager(ckpt, case):
     g = session(ckpt, graph=True, **CASES[case])
     e = session(ckpt, graph=False, **CASES[case])
-    copy_draws(e, g)
+    copy_draws(e, g)                                                 # the eager session takes g's draws
     for x in blocks(g, seed=1):
         a = g.process(x)
         b = e.process(x)

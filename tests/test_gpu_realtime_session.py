@@ -1,41 +1,28 @@
 """RealtimeVC (ddsp_svc_b200/realtime.py) on the GPU: the eager session against gui.py's order on the same modules and
 noise over consecutive blocks (the SOLA state carries over), graph replay against the eager session bit for bit, and
-replays without hidden synchronisation.  Synthetic seeded checkpoints (bench_realtime.write_synthetic)."""
+replays without hidden synchronisation.  Synthetic seeded checkpoints (conversion_fixtures.write_synthetic)."""
 import contextlib
+import functools
 import io
 
 import numpy as np
 import pytest
 import torch
 
-from bench_realtime import GuiBlock, write_synthetic
+from conversion_fixtures import GuiBlock, blocks, build_session, copy_draws, quiet, write_synthetic
 from ddsp_svc_b200.realtime import RealtimeVC
 from tests import report
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-N_BLOCKS = 5
 
 
 @pytest.fixture(scope="module", params=["Sins", "CombSubSuperFast"])
 def ckpt(request, tmp_path_factory):
-    d = tmp_path_factory.mktemp(request.param)
-    with contextlib.redirect_stdout(io.StringIO()):
-        return write_synthetic(str(d), request.param)
+    return quiet(write_synthetic, str(tmp_path_factory.mktemp(request.param)), request.param)
 
 
-def session(ckpt, **kw):
-    model_path, rmvpe_path = ckpt
-    with contextlib.redirect_stdout(io.StringIO()):
-        return RealtimeVC(model_path, rmvpe_ckpt=rmvpe_path, device=DEV, **kw)
-
-
-def blocks(s, seed=0):
-    rng = np.random.default_rng(seed)
-    t = np.arange(N_BLOCKS * s.block) / s.sr
-    x = 0.3 * np.sin(2 * np.pi * (180 * t + 20 * np.sin(2 * np.pi * t))) + 0.01 * rng.standard_normal(t.size)
-    x = np.stack([x, 0.5 * x], 1).astype(np.float32)
-    return [x[i * s.block:(i + 1) * s.block] for i in range(N_BLOCKS)]
+session = functools.partial(build_session, RealtimeVC)
 
 
 @pytest.mark.parametrize("pv,key", [(True, 0), (False, 3), (True, "auto"), (False, "auto")])
@@ -57,9 +44,7 @@ def test_eager_session_matches_gui_order(ckpt, pv, key):
 def test_graph_replay_is_bit_identical_to_eager(ckpt, pv, key):
     g = session(ckpt, graph=True, use_phase_vocoder=pv, enhancer_adaptive_key=key)
     e = session(ckpt, graph=False, use_phase_vocoder=pv, enhancer_adaptive_key=key)
-    # the eager session takes the graph session's draws of each block
-    e._draw_noise = lambda: e.noise.copy_(g.noise)
-    e._draw_enhancer_noise = lambda: (e.gen_rand_ini.copy_(g.gen_rand_ini), e.gen_noise.copy_(g.gen_noise))
+    copy_draws(e, g)                                                 # the eager session takes g's draws
     for x in blocks(g, seed=1):
         a = g.process(x)
         b = e.process(x)
